@@ -1,6 +1,6 @@
-"""bench.py -- Monte-Carlo free-integration throughput on B200 (BASELINE.json metric).
+"""bench.py -- Monte-Carlo free-integration throughput on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     torchrun ... bench.py --gpus N ...          (one rank per GPU, NCCL)
 
 Workload = BASELINE.json configs[1]: free_integration on motion_def-90deg_turn.csv
@@ -18,6 +18,11 @@ history (72 B per run-step) to the host, which is what the reference's Sim.run l
 L2 is flushed between timed steps.  `extra` carries the other BASELINE configurations measured in
 the same process (config 3 sharded over the ranks, config 4 at N = 1) and, for N > 1, the check
 that the sharded statistics equal the single-GPU ones.  See DESIGN.md section 7.
+
+--dump-outputs DIR writes what the last timed step returned on rank 0, as float64 .npy files:
+error_stats.npy [3, 9] (max |e|, mean, std of the att/pos/vel end-point errors over all runs) and
+end_err.npy [runs on this rank, 9].  The inputs are fixed by SEED, so two builds run with the same
+arguments can be compared output for output.
 """
 import argparse
 import ctypes
@@ -54,10 +59,6 @@ SEED = 12345
 TRAJ = os.path.join(ROOT, 'tests', 'golden', 'traj_90deg_turn_100hz_rf1.npz')
 WORKLOAD = ("free_integration, motion_def-90deg_turn.csv (n=1000 @100Hz), 'mid-accuracy' IMU, "
             "ref_frame=1, 1000 MC runs per GPU")
-# what the roofline fields need from an ncu capture of the dominant kernel at THIS workload
-# (tools/ncu_summary.py output): FP64 thread-instructions per run-step, DRAM bytes per launch, and the
-# launch shape they were counted on -- read at run time, never copied into this file
-ROOFLINE_INPUTS = os.path.join(ROOT, 'profiles', 'roofline_inputs_r02.json')
 C3_CSV = os.path.join(ROOT, 'tests', 'golden', 'motion_def-long_drive.csv')
 C3_RUNS, C3_FS = 100000, 200.0
 
@@ -277,20 +278,12 @@ def cpu_baseline_sample(g, nav, imu, budget_s=4.0):
     return out
 
 
-# ------------------------------------------------------------------ B200 arm ---------------------
-def roofline_inputs(lanes, shape):
-    """FP64 instructions per run-step and DRAM bytes per launch of the dominant kernel, from the
-    committed ncu summary named in profiles/roofline_inputs_r02.json -- valid only for the launch
-    shape they were counted on."""
-    try:
-        with open(ROOFLINE_INPUTS) as f:
-            d = json.load(f)
-    except (OSError, ValueError):
-        return None, 'profiles/roofline_inputs_r02.json missing'
-    if int(d.get('lanes_per_run', -1)) != int(lanes) or d.get('shape') != shape:
-        return None, 'capture is for lanes=%s shape=%s, this run used lanes=%s shape=%s' % (
-            d.get('lanes_per_run'), d.get('shape'), lanes, shape)
-    return d, d.get('source')
+# ------------------------------------------------------------------ GPU arm ----------------------
+def dump_outputs(out_dir, arrays):
+    """Write {name: array} as out_dir/<name>.npy in float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def run_b200(args):
@@ -321,7 +314,7 @@ def run_b200(args):
     cfg = engine.make_mc_config(1, FS, n, R, SEED, imu.gyro_err, imu.accel_err, 1, 9,
                                 run_offset=rank * R, ini_offset=rank * R, lanes_per_run=args.lanes)
     res = engine.McResult()
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')   # > the 50 MB L2 of an H100
     sms = torch.cuda.get_device_properties(local).multi_processor_count
     lanes_used = args.lanes or lib.b2ins_diag_auto_lanes(R, 1, sms)
     shape_used = _lib.mc_shape(lanes_used, 1)
@@ -372,6 +365,9 @@ def run_b200(args):
         evs.append((e0, e1))
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'error_stats': stats.cpu().numpy() if hasattr(stats, 'cpu') else stats,
+                                         'end_err': res.end_err.cpu().numpy()})
     dev_ms = allmax(sum(a.elapsed_time(b) for a, b in evs))
     value = total_runs * n * args.steps / (dev_ms * 1e-3)
     stats = stats.cpu().numpy().copy() if hasattr(stats, 'cpu') else stats
@@ -390,7 +386,7 @@ def run_b200(args):
 
     # ---- dominant kernel alone: launch duration -> roofline --------------------------------
     kev = []
-    for _ in range(max(args.steps, 5)):
+    for _ in range(args.steps):
         flush.fill_(1)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
@@ -408,33 +404,15 @@ def run_b200(args):
             peaks = json.load(f)
     except OSError:
         pass
-    hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
+    hbm_peak = float(peaks.get('hbm_gbs', 3350.0))     # fallback: H100 SXM data sheet
     achieved = alg_bytes / (k_ms * 1e-3) / 1e9
     dfma = ctypes.c_double(0.0)
     _lib.check(lib.b2ins_diag_dfma_rate(ctypes.byref(dfma)))
     k_rate = R * n / (k_ms * 1e-3)
-    rin, rsrc = roofline_inputs(lanes_used, shape_used)
     fp64 = {'bound': 'fp64-issue', 'peak_dfma_per_s': dfma.value, 'peak_source': 'measured live '
             '(b2ins_diag_dfma_rate)', 'kernel_run_steps_per_s': k_rate,
             'dfma_slots_per_run_step': dfma.value / k_rate, 'lanes_per_run': lanes_used,
-            'launch_shape': shape_used, 'inputs_from': rsrc}
-    traffic = None
-    if rin is not None:
-        fp64['fp64_inst_per_run_step'] = rin['fp64_thread_instructions_per_run_step']
-        fp64['frac'] = rin['fp64_thread_instructions_per_run_step'] * k_rate / dfma.value
-        fp64['frac_note'] = ('FP64 thread-instructions issued / measured FP64-FMA issue rate.  1000 runs '
-                             'put ONE attitude warp on an SM: the serial recurrence is bound by the '
-                             'dependent-issue latency of that warp (8.8 cycles per dependent DFMA, '
-                             'profiles/ilp_probe_r02.jsonl), not by the pipe')
-        if 'fp64_thread_instructions_per_run_step_one_lane' in rin:
-            # the same count for ONE lane per run: the share of the issued FP64 work that is not a
-            # replica of another lane's (lane groups replicate the strapdown step)
-            fp64['fp64_inst_per_run_step_one_lane'] = rin['fp64_thread_instructions_per_run_step_one_lane']
-            fp64['frac_nonreplicated'] = (rin['fp64_thread_instructions_per_run_step_one_lane'] * k_rate
-                                          / dfma.value)
-        traffic = rin.get('dram_bytes_per_launch')
-    else:
-        fp64['frac'] = None
+            'launch_shape': shape_used}
 
     if args.quick:
         if rank == 0:
@@ -469,7 +447,7 @@ def run_b200(args):
         return total_runs * n * steps / allmax(time.perf_counter() - t0)
 
     e2e_value = timed_e2e(False, args.steps)
-    e2e_hist_value = timed_e2e(True, max(3, args.steps // 2))
+    e2e_hist_value = timed_e2e(True, args.steps)
     # plan path (N = 1): true IMU samples + last ref_nav row + initial state up,
     # statistics + per-run end-point errors down
     h2d = (n * 6 + 9 + 9) * 8
@@ -508,7 +486,7 @@ def run_b200(args):
         # per step: the K12 kernel + stats_small_kernel (N = 1) / stats_exchange_kernel (N > 1)
         'gpu_launches': args.steps * 2,
         'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': hbm_peak, 'unit': 'GB/s',
-                     'frac': achieved / hbm_peak, 'traffic': traffic,
+                     'frac': achieved / hbm_peak,
                      'peak_source': 'MEASURED_PEAKS.json' if peaks else 'fallback',
                      'kernel': 'mc_av_kernel (K12, attitude / velocity split form)' if shape_used == '6,2,0' else 'mc_spec_kernel (K12)', 'kernel_ms': k_ms,
                      'algorithmic_bytes_per_launch': alg_bytes,
@@ -697,6 +675,8 @@ def main():
     ap.add_argument('--c3-runs', type=int, default=C3_RUNS, help='Monte-Carlo runs of the config-3 block')
     ap.add_argument('--no-config4', action='store_true')
     ap.add_argument('--c5-runs', type=int, default=10000, help='Monte-Carlo runs of the config-5 block')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/<name>.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference(args)

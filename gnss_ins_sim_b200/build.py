@@ -1,4 +1,4 @@
-"""Build csrc/libb2ins.so in-tree with nvcc for sm_100a.
+"""Build csrc/libb2ins.so in-tree with nvcc for sm_90a (H100).
 
     python -m gnss_ins_sim_b200.build [--force] [-v]
 
@@ -29,7 +29,8 @@ DEPS = UNITS + ['internal.h', 'mc_plain_launch.cuh', 'mc_spec_launch.cuh', 'comm
                 'mech.cuh', 'mc_kernel.cuh', 'mc_spec_kernel.cuh', 'mc_av_kernel.cuh', 'noise_kernel.cuh', 'stats_kernel.cuh',
                 'allan_kernel.cuh', 'psd_kernel.cuh', 'gps_kernel.cuh', 'ekf_kernel.cuh', 'pathgen_host.h',
                 os.path.join('..', '..', 'include', 'b2ins.h')]
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC']
 LAST_BUILD = 'not checked'     # 'compiled' | 'reused' after build()
 
@@ -106,7 +107,7 @@ def build(force=False, verbose=False):
             raise RuntimeError('nvcc failed on %s:\n%s%s' % (u, res.stdout, res.stderr))
         if verbose:
             sys.stderr.write(res.stderr)
-    res = subprocess.run([nvcc, '-gencode', 'arch=compute_100a,code=sm_100a', '-shared', '-o', LIB] +
+    res = subprocess.run([nvcc] + ARCH + ['-shared', '-o', LIB] +
                          [obj for _, obj, _ in results], cwd=CSRC, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError('link failed:\n' + res.stdout + res.stderr)

@@ -1,7 +1,7 @@
 // K12, ref_frame 1, few runs: the STEP ITSELF split over two warps.
 //
-// With 1000 runs a B200 has one integrator warp per SM, and that warp needs ~350 cycles per step: ~120
-// instructions, most of them FP64, on dependency chains at 8.8 cycles per dependent issue (DESIGN.md 3.2).
+// With 1000 runs an H100 has about one integrator warp per SM, and that warp's step is ~120 instructions,
+// most of them FP64, on dependency chains: it is bound by the dependent-issue latency of one warp (DESIGN.md 3.2).
 // In the virtual inertial frame the attitude recurrence does not read velocity or position
 // (free_integration.py:104), so it runs ahead in its own warp and hands the sin/cos of every step
 // through a shared-memory ring to a second warp that does velocity and position (:109-116):
@@ -11,7 +11,7 @@
 //
 // One named barrier per round of kAvRound samples couples the three stages: in interval i the
 // producers fill round i, A integrates round i-1, V round i-2 (slots triple-buffered, the ring
-// double-buffered).  A (~273 cycles per step alone) is the critical path; the warp placement is in the
+// double-buffered).  A is the critical path; the warp placement is in the
 // role tables below.
 #pragma once
 #include "mc_spec_kernel.cuh"

@@ -287,7 +287,7 @@ __device__ __forceinline__ double ipow(double a, int e) {
 // (G = 1) wants many warps per scheduler to cover FP64 latency; wide groups are latency bound
 // by the serial recurrence and keep their registers
 #ifndef B2INS_G1_MINBLOCKS
-#define B2INS_G1_MINBLOCKS 5   // measured: 1.614 / 1.642 / 1.658e10 run-steps/s for 3 / 4 / 5 (profiles/variants_r01.jsonl)
+#define B2INS_G1_MINBLOCKS 5   // tools/variants.sh times 3 / 4 / 5
 #endif
 template <int G>
 struct MinBlocks {

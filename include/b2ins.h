@@ -1,5 +1,5 @@
 /*
- * b2ins -- B200-native Monte-Carlo strapdown-INS engine: C ABI.
+ * b2ins -- H100-native Monte-Carlo strapdown-INS engine: C ABI.
  *
  * This is the drop-in boundary for the Monte-Carlo free-integration hot path of
  * gnss-ins-sim (SURVEY.md section 8b).  Every entry point names the reference
@@ -373,7 +373,7 @@ int64_t b2ins_path_gen_host(const double* ini, const double* motion_def, int64_t
 int b2ins_diag_dfma_rate(double* dfma_per_s);
 
 /* The lanes-per-run value lanes_per_run = 0 resolves to, for `runs` runs on `sm_count` SMs
- * (0: the current device, 148 if there is none).  fused: the launch is the fused Monte-Carlo kernel
+ * (0: the current device, 132 if there is none).  fused: the launch is the fused Monte-Carlo kernel
  * with end-point statistics only (the warp-specialised form applies); otherwise supplied data or
  * process statistics.  A pure function of its arguments: usable without a GPU. */
 int b2ins_diag_auto_lanes(int64_t runs, int fused, int sm_count);

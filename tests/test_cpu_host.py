@@ -434,12 +434,12 @@ def test_csv_files_round_trip(tmp_path):
 def test_lanes_per_run_choice():
     """lanes_per_run = 0: the narrowest lane group that still gives every SM a CTA of the
     warp-specialised kernel (32 / G runs per CTA), one lane per run for large ensembles; supplied data /
-    process statistics keep the one-warp-per-sub-partition rule.  Pure host logic (148 SMs given
-    explicitly)."""
+    process statistics keep the one-warp-per-sub-partition rule.  Pure host logic (an H100's 132 SMs
+    given explicitly)."""
     from gnss_ins_sim_b200 import _lib
     lib = _lib.load()
-    pick = lambda runs, fused: lib.b2ins_diag_auto_lanes(runs, fused, 148)   # noqa: E731
-    assert [pick(r, 1) for r in (100, 500, 592, 593, 1000, 1184, 1185, 2000, 4000, 4736, 4737, 12500)] == \
+    pick = lambda runs, fused: lib.b2ins_diag_auto_lanes(runs, fused, 132)   # noqa: E731
+    assert [pick(r, 1) for r in (100, 500, 528, 529, 1000, 1056, 1057, 2000, 4000, 4224, 4225, 12500)] == \
         [8, 8, 8, 4, 4, 4, 2, 2, 2, 2, 1, 1]
     assert pick(40001, 1) == 1 and pick(10 ** 6, 1) == 1
     assert [pick(r, 0) for r in (500, 1000, 2000, 4000, 10000, 20000, 10 ** 6)] == [32, 16, 8, 4, 2, 1, 1]

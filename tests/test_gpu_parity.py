@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): the CUDA path through the C ABI against the
+"""GPU parity tests (run on an H100): the CUDA path through the C ABI against the
 golden vectors produced by the unmodified reference and against the NumPy oracle.
 Tolerance: |x - ref| <= 1e-6 * max(|ref|, scale) as BASELINE north_star states (SURVEY 8c);
 the observed deviation is ~1e-12 and a tighter bound is asserted beside it."""

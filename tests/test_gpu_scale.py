@@ -117,7 +117,7 @@ def test_k4_allan_millions_of_samples(eng):
 @pytest.mark.parametrize('n', [200004, 150001])
 def test_k4_allan_contiguous_series_both_front_ends(eng, n):
     """Contiguous series: even n keeps every row 16-byte aligned (persistent bulk-copy front end,
-    several tiles per CTA: 8 x 39 tiles on 148 SMs), odd n does not (per-thread loads)."""
+    several tiles per CTA: 8 x 39 tiles on 132 SMs), odd n does not (per-thread loads)."""
     rng = np.random.RandomState(n % 1000)
     nser, fs = 8, 200.0
     x = 3.7 + 1e-2 * rng.randn(nser, n) + np.cumsum(1e-5 * rng.randn(nser, n), axis=1)

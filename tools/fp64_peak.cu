@@ -1,6 +1,6 @@
 // Measures the FP64 FMA issue rate of the device (the co-roofline of the b2ins kernels,
 // which are FP64-instruction-bound rather than HBM-bound) and the cost of the double
-// precision libm calls the kernels lean on.   nvcc -gencode arch=compute_100a,code=sm_100a
+// precision libm calls the kernels lean on.   nvcc -gencode arch=compute_90a,code=sm_90a
 // -O3 -o fp64_peak fp64_peak.cu && ./fp64_peak
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
 // Issue rate of independent FP64 / integer chains from ONE warp per SM sub-partition: cycles per
 // instruction for K independent chains (K = 1..16).  With one warp per scheduler the kernels'
 // serial parts are bound by this, not by the pipe's aggregate rate.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ilp_probe ilp_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ilp_probe ilp_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

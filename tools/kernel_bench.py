@@ -48,7 +48,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except OSError:
         pass
-    hbm = float(peaks.get('hbm_gbs', 6650.0))
+    hbm = float(peaks.get('hbm_gbs', 3350.0))     # fallback: H100 SXM data sheet
     dfma = ctypes.c_double()
     _lib.check(_lib.load().b2ins_diag_dfma_rate(ctypes.byref(dfma)))
     emit(kernel='peaks', hbm_gbs=hbm, hbm_source='MEASURED_PEAKS.json' if peaks else 'fallback',

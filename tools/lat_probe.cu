@@ -1,5 +1,5 @@
 // Dependent-issue latencies (cycles) of the instructions on the strapdown critical path,
-// one warp on one SM.   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o lat_probe lat_probe.cu
+// one warp on one SM.   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lat_probe lat_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

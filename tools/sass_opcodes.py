@@ -28,7 +28,7 @@ def main():
         m = re.match(r'\s+/\*[0-9a-f]{4,5}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_]+)', line)
         if m and fam:
             counts[fam][m.group(1)] += 1
-    print('# Static SASS opcode counts of csrc/libb2ins.so (cuobjdump -sass, sm_100a), per kernel family '
+    print('# Static SASS opcode counts of csrc/libb2ins.so (cuobjdump -sass, sm_90a), per kernel family '
           '(all instantiations summed); tools/sass_opcodes.py.')
     print('# UBLKCP = cp.async.bulk (1-D TMA copy), SYNCS = mbarrier ops; no tensor-core opcodes (HMMA / UTC*MMA) '
           'anywhere: the path has no contraction.')

@@ -24,7 +24,8 @@ SHAPES = {1: ['3,1,0', '6,1,0', '0'], 2: ['3,1,0', '6,1,0'], 4: ['3,1,0', '6,1,0
 def main():
     quick = len(sys.argv) > 1 and sys.argv[1] == 'quick'
     sweeps = [(1000, [4, 8, 16, 32, 2]), (500, [4, 8, 16]), (2000, [2, 4, 1]), (4000, [1, 2, 4]),
-              (8000, [1, 2]), (12500, [1, 2, 4]), (40000, [1, 2]), (100000, [1]), (1000000, [1])]
+              (8000, [1, 2]), (12500, [1, 2, 4]), (40000, [1, 2]), (65536, [1]), (100000, [1]),
+              (262144, [1]), (1000000, [1])]
     if quick:
         sweeps = [(1000, [4, 8]), (500, [8, 4]), (2000, [4, 2])]
     flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')

@@ -4,7 +4,7 @@
 #   bash tools/variants.sh build          -> tools/libb2ins_mb{3,4,5}.so
 #   bash tools/variants.sh time > gpurun_out/variants_r02.jsonl
 cd "$(dirname "$0")/../gnss_ins_sim_b200/csrc" || exit 1
-FLAGS="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC"
 if [ "$1" = "build" ]; then
   for mb in 3 4 5; do
     mkdir -p _obj/mb$mb
@@ -12,7 +12,7 @@ if [ "$1" = "build" ]; then
       nvcc $FLAGS -DB2INS_G1_MINBLOCKS=$mb -c -o _obj/mb$mb/$u.o $u.cu &
     done
     wait
-    nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../../tools/libb2ins_mb$mb.so _obj/mb$mb/*.o || exit 1
+    nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../tools/libb2ins_mb$mb.so _obj/mb$mb/*.o || exit 1
   done
   exit 0
 fi
