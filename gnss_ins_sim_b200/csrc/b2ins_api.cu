@@ -151,7 +151,9 @@ bool shape_override(McShape* sh) {
 // per warp) where the group is narrow, the paired layout (producer and integrator of a group on the
 // same sub-partition) for the widest groups.
 // (ref_frame 1, groups of 4 and 8 lanes: the step itself split over an attitude and a velocity warp,
-// mc_av_kernel.cuh, key "6,2,0" -- on an H100 0.165 against 0.177 ms at 1000 runs, 0.146 against 0.173 at 500)
+// mc_av_kernel.cuh, key "6,2,0" -- on an H100 0.165 against 0.177 ms at 1000 runs, 0.146 against 0.173 at 500
+// at a 700 W power limit; with the shorter attitude block and lighter producers 0.137 ms at 1000 runs and
+// 0.119 ms at 500 at a 400 W limit, the fused form not measured again)
 McShape default_shape(int G, int rf) {
   if (rf == 1 && (G == 4 || G == 8)) return McShape{G, 6, 2, false, true};
   switch (G) {
@@ -1166,11 +1168,12 @@ int b2ins_diag_dfma_rate(double* dfma_per_s) {
 }
 
 #ifdef B2INS_PHASE_CLOCKS
-// tools only: cumulative warp-cycles in (tile wait, phase A noise, phase A incl. GM scan, phase B)
-int b2ins_diag_phase_clocks(unsigned long long* out8, int reset) {
-  if (out8) cudaMemcpyFromSymbol(out8, g_phase_clocks, sizeof(unsigned long long) * 8);
+// tools only: the kPhaseClocks cumulative warp-cycle counters (slots: mc_kernel.cuh, mc_spec_kernel.cuh,
+// mc_av_kernel.cuh)
+int b2ins_diag_phase_clocks(unsigned long long* out16, int reset) {
+  if (out16) cudaMemcpyFromSymbol(out16, g_phase_clocks, sizeof(unsigned long long) * kPhaseClocks);
   if (reset) {
-    unsigned long long z[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    unsigned long long z[kPhaseClocks] = {};
     cudaMemcpyToSymbol(g_phase_clocks, z, sizeof(z));
   }
   return B2INS_OK;

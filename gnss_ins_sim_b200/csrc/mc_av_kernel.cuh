@@ -12,8 +12,15 @@
 // One named barrier per round of kAvRound samples couples the three stages: in interval i the
 // producers fill round i, A integrates round i-1, V round i-2 (slots triple-buffered, the ring
 // double-buffered).  A is the critical path; the warp placement is in the
-// role tables below.
+// role tables below.  Phase clocks per role (tools/spec2_phase.py, one H100 SXM 80 GB at a 400 W power
+// limit, 1000 runs, G = 4): A spends ~95 % of a round stepping and ~5 % at the barrier, V and the producers
+// wait ~50 % and ~30 % of it.  So A's block is what a round costs: its slot loads are issued at the start
+// of the block, and the time-based re-evaluation runs in a speculative block like the others.  The producers
+// issue fewer instructions per round too (with groups of 4 one of them shares A's sub-partition).  Config 2:
+// 0.170 -> 0.137 ms (0.160 with the lighter producers alone); 500 runs, G = 8: 0.142 -> 0.119 ms.
 #pragma once
+#include <type_traits>
+
 #include "mc_spec_kernel.cuh"
 
 namespace b2ins {
@@ -34,6 +41,11 @@ struct AvShape {
 // with groups of 4; V, idle more than half of the time, shares sub-partition 1 with two / three producers.
 __device__ constexpr int kAvRole8[12] = {-1, -2, 0, 1, -3, 2, 3, 4, -3, 5, -3, -3};
 __device__ constexpr int kAvRole4[16] = {-1, -2, 0, 1, 2, 3, 4, 5, -3, 6, 7, 8, -3, 9, 10, 11};
+
+// Phase clocks (-DB2INS_PHASE_CLOCKS, tools/spec2_phase.py): g_phase_clocks[8] A stepping, [9] A at the
+// barrier, [10] A's vote, redo and exact re-evaluation after a block, [11] V stepping, [12] V at the barrier,
+// [13] producers waiting for a tile, [14] producing, [15] producers at the barrier.  B2INS_MC_DEBUG idles
+// the producers (1), A (2) or V (4).
 
 template <int G>
 struct AvSmem {
@@ -78,6 +90,15 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
     }
     mbar_fence_init();
   }
+#ifdef B2INS_PHASE_CLOCKS
+  // isolation runs read slots or a ring nobody wrote: zeros keep A off the exact path
+  if (p.debug) {
+    for (int q = threadIdx.x; q < static_cast<int>(sizeof(sm.slot) / 8); q += blockDim.x)
+      reinterpret_cast<double*>(sm.slot)[q] = 0.0;
+    for (int q = threadIdx.x; q < static_cast<int>(sizeof(sm.ring) / 8); q += blockDim.x)
+      reinterpret_cast<double*>(sm.ring)[q] = 0.0;
+  }
+#endif
   __syncthreads();
   if (!is_a && !is_v && !is_p) return;                     // the spare warps
   // rounds of the whole series: tiles are whole rounds (kTile % kAvRound == 0), the last may be short
@@ -90,8 +111,11 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
     const int c = pp % 6, ax = c % 3;
     const bool is_acc = c < 3;
     const TriadNoise& e = is_acc ? p.accel : p.gyro;
+    // The channel's error model in registers for the whole series: read in the round loop, every
+    // coefficient is a parameter-space load indexed by the channel.
+    const double eb = e.b[ax], ew = e.w[ax], ewd = e.wd[ax], ga = e.gm_a[ax], gb = e.gm_b[ax];
     double carry = 0.0;
-    const double apj = ipow(e.gm_a[ax], j), aG = ipow(e.gm_a[ax], kAvRound);
+    const double apj = ipow(ga, j), aG = ipow(ga, kAvRound);
     double phase[3] = {0.0, 0.0, 0.0};
     if (p.gyro.vib_type == 2) {
 #pragma unroll
@@ -99,52 +123,88 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
         phase[k] = (uniform01(0xFFFFFFFFu, kDrawPhase + k, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
     }
     const bool any_vib = (p.accel.vib_type | p.gyro.vib_type) != 0;
-    for (int64_t i = 0; i < rounds + 2; ++i) {
-      if (i < rounds) {
-        const int64_t r0 = i * kAvRound;                   // first sample of the round
-        const int64_t tile = r0 / kTile;
-        const int s = static_cast<int>(tile % kStagesFast);
-        const int base = static_cast<int>(r0 - tile * kTile);
-        const int cnt = static_cast<int>(min64(kTile, p.n - tile * kTile));
+    // This lane's sample (base + j) of the round in the trajectory tile of stage s is ref0[s kTile 3 +
+    // 3 base]; its slot (sample j of run grp, where the consumers -- G lanes per run, passes of G
+    // samples -- look for it) in slot set buf is out0[buf kSlotSet].
+    const double* ref0 = (is_acc ? sm.accel[0] : sm.gyro[0]) + j * 3 + ax;
+    SampleSlot& slot0 = sm.slot[0][j / G][grp * G + (j % G)];
+    double* out0 = (is_acc ? slot0.a : slot0.g) + ax;
+    constexpr int kSlotSet = static_cast<int>(sizeof(sm.slot[0]) / sizeof(double));
+    const int nrounds = static_cast<int>(rounds);         // n < 2^32 (b2ins_api.cu)
+    const int ntiles = static_cast<int>(num_tiles);
+    // The round loop, with the history output and the vibration models compiled in (SLOW) or out: the
+    // choice is made once per warp.  Tile, stage, parity and slot set advance by counting.
+    auto produce = [&](auto slow) {
+      constexpr bool kSlow = decltype(slow)::value;
+      int tile = 0, s = 0, base = 0, ref_off = 0, out_off = 0;
+      uint32_t parity = 0, t0 = 0;
+      int cnt = static_cast<int>(min64(kTile, p.n));
+      for (int i = 0; i < nrounds; ++i) {
         if (base == 0) {
           // refill the stage the PREVIOUS tile used, then wait for this tile's data
-          if (threadIdx.x == issuer && tile >= 1 && tile - 1 + kStagesFast < num_tiles) {
-            const int sp = static_cast<int>((tile - 1) % kStagesFast);
-            mbar_wait(&sm.empty[sp], static_cast<uint32_t>(((tile - 1) / kStagesFast) & 1));
+          if (threadIdx.x == issuer && tile >= 1 && tile - 1 + kStagesFast < ntiles) {
+            const int sp = (s == 0) ? kStagesFast - 1 : s - 1;
+            mbar_wait(&sm.empty[sp], (s == 0) ? parity ^ 1u : parity);
             spec_issue_tile(sm, p, tile - 1 + kStagesFast, sp);
           }
-          mbar_wait(&sm.full[s], static_cast<uint32_t>((tile / kStagesFast) & 1));
+          B2_CLK(cw0);
+          mbar_wait(&sm.full[s], parity);
+          B2_CLK(cw1);
+          B2_ACC(13, cw0, cw1);
         }
-        const int buf = static_cast<int>(i % 3);
+        B2_CLK(cp0);
+#ifdef B2INS_PHASE_CLOCKS
+        if (!(p.debug & 1))
+#endif
         {
           const int tj = base + j;
-          const int64_t t = tile * kTile + tj;
+          const uint32_t t = t0 + static_cast<uint32_t>(tj);
           const bool live = tj < cnt;
           Normal2 z{0.0, 0.0};
           double m = 0.0;
           if (live) {
-            z = normal_pair(static_cast<uint32_t>(t), c, run_lo, run_hi, p.k0, p.k1);
-            const double ref = is_acc ? sm.accel[s][tj * 3 + ax] : sm.gyro[s][tj * 3 + ax];
-            m = (ref + e.b[ax]) + e.w[ax] * z.z1;
-            if (any_vib)
-              m += vib_term(e, ax, is_acc ? 0 : 1, static_cast<uint32_t>(t), run_lo, run_hi, p.k0, p.k1, run, phase);
+            z = normal_pair(t, c, run_lo, run_hi, p.k0, p.k1);
+            m = (ref0[ref_off] + eb) + ew * z.z1;
+            if (kSlow && any_vib)
+              m += vib_term(e, ax, is_acc ? 0 : 1, t, run_lo, run_hi, p.k0, p.k1, run, phase);
           }
-          const double d = gm_block<kAvRound>(e.gm_b[ax] * z.z0, e.gm_a[ax], apj, aG, j, carry);
-          m += d + e.wd[ax] * z.z0;
+          const double d = gm_block<kAvRound>(gb * z.z0, ga, apj, aG, j, carry);
+          m += d + ewd * z.z0;
           int64_t row;
-          if (warp_dumps && dump && live && p.out_gyro && dump_row(p, t, &row))
+          if (kSlow && warp_dumps && dump && live && p.out_gyro && dump_row(p, t, &row))
             (is_acc ? p.out_accel : p.out_gyro)[run * p.osr + row * p.ost + ax * p.osc] = m;
-          // sample j of run grp, where the consumers (G lanes per run, passes of G samples) look for it
-          SampleSlot& mine = sm.slot[buf][j / G][grp * G + (j % G)];
-          if (is_acc) mine.a[ax] = m; else mine.g[ax] = m;
+          out0[out_off] = m;
         }
+        B2_CLK(cp1);
+        B2_ACC(14, cp0, cp1);
         if (base + kAvRound >= cnt) {                      // last round of the tile: release the stage
           __syncwarp();
           if (lane == 0) mbar_arrive(&sm.empty[s]);
+          ++tile;
+          if (++s == kStagesFast) {
+            s = 0;
+            parity ^= 1u;
+          }
+          base = 0;
+          t0 += kTile;
+          ref_off = s * kTile * 3;
+          cnt = static_cast<int>(min64(kTile, p.n - static_cast<int64_t>(t0)));
+        } else {
+          base += kAvRound;
+          ref_off += kAvRound * 3;
         }
+        out_off = (out_off == 2 * kSlotSet) ? 0 : out_off + kSlotSet;
+        B2_CLK(cb0);
+        stage_sync();                     // intervals 0 .. rounds end in a barrier
+        B2_CLK(cb1);
+        B2_ACC(15, cb0, cb1);
       }
-      if (i <= rounds) stage_sync();     // intervals 0 .. rounds end in a barrier; the last one is V's alone
-    }
+      stage_sync();                       // interval `rounds`: A's last round; the one after is V's alone
+    };
+    if (warp_dumps || any_vib)
+      produce(std::true_type{});
+    else
+      produce(std::false_type{});
     return;
   }
 
@@ -170,21 +230,28 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
       if (p.out_quat) write_quat(p.out_quat + run * p.dump_rows * 4, a.yaw, a.pitch, a.roll);
     }
     for (int64_t i = 0; i < rounds + 2; ++i) {
+      B2_CLK(ca0);
+#ifdef B2INS_PHASE_CLOCKS
+      if (!(p.debug & 2))
+#endif
       if (i >= 1 && i <= rounds) {
         const int64_t r0 = (i - 1) * kAvRound;
         const int sbuf = static_cast<int>((i - 1) % 3), rbuf = static_cast<int>((i - 1) & 1);
         // samples of this round that are followed by a step (the last sample of the series is not)
         const int kmax = static_cast<int>(min64(kAvRound, p.n - 1 - r0));
-        auto a_step = [&](int k) {                        // one step with the exact path and the history rows
-          const SampleSlot& sl = sm.slot[sbuf][k / G][lane - j + (k % G)];
-          const Vec3 w{sl.g[0], sl.g[1], sl.g[2]};
-          att_step(a, w, p.dt, ((r0 + k + 1) & (kResync - 1)) == 0);
+        auto ring_store = [&](int k) {                    // the sin/cos after step k, for V
           if (j == 0) {
             double* o = sm.ring[rbuf][k][grp];
             reinterpret_cast<double2*>(o)[0] = make_double2(a.sc.sy, a.sc.cy);
             reinterpret_cast<double2*>(o)[1] = make_double2(a.sc.sp, a.sc.cp);
             reinterpret_cast<double2*>(o)[2] = make_double2(a.sc.sr, a.sc.cr);
           }
+        };
+        auto a_step = [&](int k) {                        // one step with the exact path and the history rows
+          const SampleSlot& sl = sm.slot[sbuf][k / G][lane - j + (k % G)];
+          const Vec3 w{sl.g[0], sl.g[1], sl.g[2]};
+          att_step(a, w, p.dt, ((r0 + k + 1) & (kResync - 1)) == 0);
+          ring_store(k);
           int64_t row;
           if (warp_dumps && dump && j == 0 && p.out_att && dump_row(p, r0 + k + 1, &row)) {
             const int64_t o = run * p.osr + row * p.ost;
@@ -200,39 +267,49 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
           for (int k = 0; k < kmax; ++k) a_step(k);
         } else {
           // Blocks of four steps as ONE basic block without the exact-path branch (mc_spec_kernel.cuh has
-          // the same scheme): the next step's loads and rate products overlap the tail of the previous
-          // one.  A block that holds a time-based re-evaluation (1 of 16), or in which any lane needed
-          // the exact path, is (re)done step by step from the saved state; the ring is overwritten with
-          // the same or the corrected values before V sees it (V reads after the next barrier).
+          // the same scheme): the next step's rate products overlap the tail of the previous one.  The
+          // block's gyro samples are loaded at its start, so that no shared load waits behind the ring
+          // stores of the step before.  A block in which any lane needed the exact path is redone step
+          // by step from the saved state; the ring is overwritten with the same or the corrected values
+          // before V sees it (V reads after the next barrier).
+          static_assert(kAvRound % 4 == 0 && kResync % 4 == 0, "blocks of four steps");
 #pragma unroll 1
           for (int kb = 0; kb < kAvRound; kb += 4) {
-            bool redo = ((r0 + kb) & (kResync - 1)) + 4 >= kResync;
-            if (!redo) {
-              const AttState saved = a;
-              bool cold = false;
+            const AttState saved = a;
+            Vec3 w[4];
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const SampleSlot& sl = sm.slot[sbuf][(kb + k) / G][lane - j + ((kb + k) % G)];
-                const Vec3 w{sl.g[0], sl.g[1], sl.g[2]};
-                cold |= att_step<true>(a, w, p.dt, false);
-                if (j == 0) {
-                  double* o = sm.ring[rbuf][kb + k][grp];
-                  reinterpret_cast<double2*>(o)[0] = make_double2(a.sc.sy, a.sc.cy);
-                  reinterpret_cast<double2*>(o)[1] = make_double2(a.sc.sp, a.sc.cp);
-                  reinterpret_cast<double2*>(o)[2] = make_double2(a.sc.sr, a.sc.cr);
-                }
-              }
-              redo = __any_sync(0xffffffffu, cold);
-              if (__builtin_expect(redo, 0)) a = saved;
+            for (int k = 0; k < 4; ++k) {
+              const SampleSlot& sl = sm.slot[sbuf][(kb + k) / G][lane - j + ((kb + k) % G)];
+              w[k] = Vec3{sl.g[0], sl.g[1], sl.g[2]};
             }
-            if (redo) {
+            bool cold = false;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              cold |= att_step<true>(a, w[k], p.dt, false);
+              ring_store(kb + k);
+            }
+            B2_CLK(cr0);
+            if (__builtin_expect(__any_sync(0xffffffffu, cold), 0)) {
+              a = saved;
 #pragma unroll 1
               for (int k = 0; k < 4; ++k) a_step(kb + k);
+            } else if (((r0 + kb + 4) & (kResync - 1)) == 0) {
+              // the time-based re-evaluation (1 block of 16) falls on the block's last step: att_step's
+              // exact path after it, as att_step(..., resync = true) takes it
+              att_exact(a);
+              a.icp = rcp_nr(a.sc.cp) * p.dt;
+              ring_store(kb + 3);
             }
+            B2_CLK(cr1);
+            B2_ACC(10, cr0, cr1);
           }
         }
       }
+      B2_CLK(ca1);
+      B2_ACC(8, ca0, ca1);
       if (i <= rounds) stage_sync();
+      B2_CLK(ca2);
+      B2_ACC(9, ca1, ca2);
     }
     if (active && j == 0) {
       const double* r = p.ref_nav + (p.n - 1) * 9;
@@ -267,6 +344,10 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
     p.out_vel[o + 2 * p.osc] = v.vel.z;
   }
   for (int64_t i = 0; i < rounds + 2; ++i) {
+    B2_CLK(cv0);
+#ifdef B2INS_PHASE_CLOCKS
+    if (!(p.debug & 4))
+#endif
     if (i >= 2) {
       const int64_t r0 = (i - 2) * kAvRound;
       const int sbuf = static_cast<int>((i - 2) % 3), rbuf = static_cast<int>((i - 2) & 1);
@@ -303,7 +384,11 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
         }
       }
     }
+    B2_CLK(cv1);
+    B2_ACC(11, cv0, cv1);
     if (i <= rounds) stage_sync();        // V's last round follows the last barrier
+    B2_CLK(cv2);
+    B2_ACC(12, cv1, cv2);
   }
   if (active && j == 0) {
     const double* r = p.ref_nav + (p.n - 1) * 9;

@@ -16,9 +16,11 @@
 
 namespace b2ins {
 
-// Optional phase clocks (tools only: -DB2INS_PHASE_CLOCKS builds libb2ins_prof.so)
+// Optional phase clocks (tools only: -DB2INS_PHASE_CLOCKS builds libb2ins_prof.so).  Slots 0-7:
+// mc_kernel / mc_spec_kernel, 8-15: mc_av_kernel (see there).
+constexpr int kPhaseClocks = 16;
 #ifdef B2INS_PHASE_CLOCKS
-__device__ unsigned long long g_phase_clocks[8];
+__device__ unsigned long long g_phase_clocks[kPhaseClocks];
 #define B2_CLK(var) const long long var = clock64()
 #define B2_ACC(i, t0, t1) \
   if ((threadIdx.x & 31) == 0) atomicAdd(&g_phase_clocks[i], static_cast<unsigned long long>((t1) - (t0)))
@@ -88,7 +90,8 @@ struct McParams {
   double* end_state;   // [runs][9]
   double* proc_stats;  // [runs][3][9]
   int64_t stats_start;
-  int debug;           // tools (B2INS_PHASE_CLOCKS builds only): 1 = producers idle, 2 = integrators idle
+  int debug;           // tools (B2INS_PHASE_CLOCKS builds only): 1 = producers idle, 2 = integrators (A in
+                       // mc_av_kernel) idle, 4 = V idle (mc_av_kernel)
 };
 
 // Prepared samples of one block, one slot per lane: phase A stores (gyro xyz, accel xyz),

@@ -401,6 +401,16 @@ struct AttState {
   double icp;   // dt / cos(pitch)
 };
 
+// the exact path of att_step (resync_exact on the attitude); icp is the caller's
+B2_DEV void att_exact(AttState& s) {
+  NavState n;            // the exact path works on the full state type
+  n.yaw = s.yaw; n.pitch = s.pitch; n.roll = s.roll;
+  n.pos = Vec3{0.0, 0.0, 0.0};
+  resync_exact<1>(n);
+  s.yaw = n.yaw; s.pitch = n.pitch; s.roll = n.roll;
+  s.sc = n.sc;
+}
+
 // attitude.euler_update_zyx + euler2dcm's sin/cos for the new angles: the attitude half of nav_step<1>
 // SPEC: without the exact-path branch, returns whether it was due (see nav_step)
 template <bool SPEC = false>
@@ -417,14 +427,7 @@ B2_DEV bool att_step(AttState& s, const Vec3& w, double dt, bool resync) {
   rot_small(s.sc.sy, s.sc.cy, dy);
   rot_small(s.sc.sp, s.sc.cp, dp);
   rot_small(s.sc.sr, s.sc.cr, dr);
-  if (!SPEC && __builtin_expect(cold, 0)) {
-    NavState n;            // the exact path works on the full state type
-    n.yaw = s.yaw; n.pitch = s.pitch; n.roll = s.roll;
-    n.pos = Vec3{0.0, 0.0, 0.0};
-    resync_exact<1>(n);
-    s.yaw = n.yaw; s.pitch = n.pitch; s.roll = n.roll;
-    s.sc = n.sc;
-  }
+  if (!SPEC && __builtin_expect(cold, 0)) att_exact(s);
   s.icp = rcp_nr(s.sc.cp) * dt;
   return cold;
 }

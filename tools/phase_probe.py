@@ -34,7 +34,7 @@ def main():
             cfg = engine.make_mc_config(rf, 100.0, n, runs, 1, mid_g, mid_a, 1, 9, lanes_per_run=lanes)
             res = engine.mc_free_integration(cfg, *dev)
             torch.cuda.synchronize()
-            out = (ctypes.c_ulonglong * 8)()
+            out = (ctypes.c_ulonglong * 16)()
             diag(None, 1)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
