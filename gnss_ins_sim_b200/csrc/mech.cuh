@@ -34,8 +34,10 @@ struct SinCos3 {
 // (|x| < 1e6: error < 1e-10); larger magnitudes are only reachable after the Euler-angle
 // singularity at pitch = +-pi/2 has blown a rate up, where the recurrence is meaningless
 // anyway -- they are mapped to the angle 0 by a select (branch-free, off the critical path).
+// A NaN or an infinite angle maps to x - x = NaN, so its sin/cos are NaN as the reference's np.sin/np.cos
+// are, and the run's later samples are NaN like the reference's (no fast-math: x - x is not folded to 0).
 B2_DEV void sincos_angle(double x, double* s, double* c) {
-  sincos_bounded(fabs(x) <= 1.0e6 ? x : 0.0, s, c);
+  sincos_bounded(fabs(x) <= 1.0e6 ? x : x - x, s, c);
 }
 
 B2_DEV SinCos3 sincos3(double yaw, double pitch, double roll) {
@@ -332,7 +334,8 @@ B2_DEV bool nav_step(NavState& s, const Vec3& gyro, const Vec3& accel, double dt
   s.yaw += dy;
   s.pitch += dp;
   s.roll += dr;
-  // not-(<=) so that a NaN takes the exact path too
+  // not-(<=) so that a NaN takes the exact path too; there sincos_angle keeps it NaN, so that from this
+  // sample on the run is NaN as in the reference
   const bool cold = resync | !(fabs(s.pitch) <= kHalfPi) | !(fabs(dy) <= kRotMax) |
                     !(fabs(dp) <= kRotMax) | !(fabs(dr) <= kRotMax) |
                     (RF == 0 && !(fabs(dlat) <= kLatRotMax));
