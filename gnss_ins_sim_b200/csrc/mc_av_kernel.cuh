@@ -26,6 +26,7 @@
 namespace b2ins {
 
 constexpr int kAvRound = 8;
+static_assert(kAvRound % kSpecBlock == 0, "A's rounds are whole speculative blocks");
 // A producer warp always works on four runs x the eight samples of a round (one Box-Muller pass per round,
 // its own Gauss-Markov carry): six of them with groups of 8 lanes (four runs per CTA), twelve with groups
 // of 4 (eight runs per CTA: two producers per channel, one for each half of the runs).
@@ -43,7 +44,7 @@ __device__ constexpr int kAvRole8[12] = {-1, -2, 0, 1, -3, 2, 3, 4, -3, 5, -3, -
 __device__ constexpr int kAvRole4[16] = {-1, -2, 0, 1, 2, 3, 4, 5, -3, 6, 7, 8, -3, 9, 10, 11};
 
 // Phase clocks (-DB2INS_PHASE_CLOCKS, tools/spec2_phase.py): g_phase_clocks[8] A stepping, [9] A at the
-// barrier, [10] A's vote, redo and exact re-evaluation after a block, [11] V stepping, [12] V at the barrier,
+// barrier, [10] A's time-based re-evaluation after a warm block, [11] V stepping, [12] V at the barrier,
 // [13] producers waiting for a tile, [14] producing, [15] producers at the barrier.  B2INS_MC_DEBUG idles
 // the producers (1), A (2) or V (4).
 
@@ -72,13 +73,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
   // A and V: G lanes per run.  Producers: eight lanes per run (the samples of a round), four runs.
   const int j = is_p ? (lane & 7) : lane % G;
   const int grp = is_p ? (pp / 6) * 4 + (lane >> 3) : lane / G;      // run within the CTA
-  const int64_t run_raw = static_cast<int64_t>(blockIdx.x) * kRunsPerCta + grp;
-  const bool active = run_raw < p.runs;
-  const int64_t run = active ? run_raw : p.runs - 1;
-  const int64_t grun = p.run_offset + run;
-  const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
-  const bool dump = active && run < p.dump_runs;
-  const bool warp_dumps = __any_sync(0xffffffffu, dump);
+  const McRun mr = mc_run(p, static_cast<int64_t>(blockIdx.x) * kRunsPerCta + grp);
   const int64_t num_tiles = (p.n + kTile - 1) / kTile;
   const int issuer = 2 * 32;                               // lane 0 of the first producer warp
   auto stage_sync = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(kAvSync) : "memory"); };
@@ -107,7 +102,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
   if (is_p) {
     // =============================== producer: channel pp =========================================
     if (threadIdx.x == issuer)
-      for (int s = 0; s < kStagesFast && s < num_tiles; ++s) spec_issue_tile(sm, p, s, s);
+      for (int s = 0; s < kStagesFast && s < num_tiles; ++s) issue_tile<false, false>(sm, p, s, s);
     const int c = pp % 6, ax = c % 3;
     const bool is_acc = c < 3;
     const TriadNoise& e = is_acc ? p.accel : p.gyro;
@@ -120,7 +115,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
     if (p.gyro.vib_type == 2) {
 #pragma unroll
       for (int k = 0; k < 3; ++k)
-        phase[k] = (uniform01(0xFFFFFFFFu, kDrawPhase + k, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
+        phase[k] = (uniform01(0xFFFFFFFFu, kDrawPhase + k, mr.lo, mr.hi, p.k0, p.k1) * 2.0) * kPi;
     }
     const bool any_vib = (p.accel.vib_type | p.gyro.vib_type) != 0;
     // This lane's sample (base + j) of the round in the trajectory tile of stage s is ref0[s kTile 3 +
@@ -140,18 +135,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
       uint32_t parity = 0, t0 = 0;
       int cnt = static_cast<int>(min64(kTile, p.n));
       for (int i = 0; i < nrounds; ++i) {
-        if (base == 0) {
-          // refill the stage the PREVIOUS tile used, then wait for this tile's data
-          if (threadIdx.x == issuer && tile >= 1 && tile - 1 + kStagesFast < ntiles) {
-            const int sp = (s == 0) ? kStagesFast - 1 : s - 1;
-            mbar_wait(&sm.empty[sp], (s == 0) ? parity ^ 1u : parity);
-            spec_issue_tile(sm, p, tile - 1 + kStagesFast, sp);
-          }
-          B2_CLK(cw0);
-          mbar_wait(&sm.full[s], parity);
-          B2_CLK(cw1);
-          B2_ACC(13, cw0, cw1);
-        }
+        if (base == 0) refill_and_wait<false, false>(sm, p, threadIdx.x == issuer, tile, ntiles, s, parity, 13);
         B2_CLK(cp0);
 #ifdef B2INS_PHASE_CLOCKS
         if (!(p.debug & 1))
@@ -163,16 +147,16 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
           Normal2 z{0.0, 0.0};
           double m = 0.0;
           if (live) {
-            z = normal_pair(t, c, run_lo, run_hi, p.k0, p.k1);
+            z = normal_pair(t, c, mr.lo, mr.hi, p.k0, p.k1);
             m = (ref0[ref_off] + eb) + ew * z.z1;
             if (kSlow && any_vib)
-              m += vib_term(e, ax, is_acc ? 0 : 1, t, run_lo, run_hi, p.k0, p.k1, run, phase);
+              m += vib_term(e, ax, is_acc ? 0 : 1, t, mr.lo, mr.hi, p.k0, p.k1, mr.run, phase);
           }
           const double d = gm_block<kAvRound>(gb * z.z0, ga, apj, aG, j, carry);
           m += d + ewd * z.z0;
           int64_t row;
-          if (kSlow && warp_dumps && dump && live && p.out_gyro && dump_row(p, t, &row))
-            (is_acc ? p.out_accel : p.out_gyro)[run * p.osr + row * p.ost + ax * p.osc] = m;
+          if (kSlow && mr.warp_dumps && mr.dump && live && p.out_gyro && dump_row(p, t, &row))
+            (is_acc ? p.out_accel : p.out_gyro)[mr.run * p.osr + row * p.ost + ax * p.osc] = m;
           out0[out_off] = m;
         }
         B2_CLK(cp1);
@@ -201,7 +185,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
       }
       stage_sync();                       // interval `rounds`: A's last round; the one after is V's alone
     };
-    if (warp_dumps || any_vib)
+    if (mr.warp_dumps || any_vib)
       produce(std::true_type{});
     else
       produce(std::false_type{});
@@ -209,12 +193,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
   }
 
   // initial state (both A and V derive what they need from it)
-  NavState st0;
-  {
-    const int64_t irun = p.ini_offset + run;
-    const int64_t set = (irun < p.ini_sets) ? irun : 0;  // free_integration.py:85-87
-    nav_init<1>(st0, p.ini + set * p.ini_rows, p.ini_rows, p.dt);
-  }
+  const NavState st0 = mc_init<1>(p, mr.run);
 
   if (is_a) {
     // ================================= A: attitude =================================================
@@ -222,13 +201,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
     a.yaw = st0.yaw; a.pitch = st0.pitch; a.roll = st0.roll;
     a.sc = st0.sc;
     a.icp = st0.icp;
-    if (dump && j == 0 && p.out_att) {
-      const int64_t o = run * p.osr;
-      p.out_att[o] = a.yaw;
-      p.out_att[o + p.osc] = a.pitch;
-      p.out_att[o + 2 * p.osc] = a.roll;
-      if (p.out_quat) write_quat(p.out_quat + run * p.dump_rows * 4, a.yaw, a.pitch, a.roll);
-    }
+    if (mr.dump && j == 0 && p.out_att) put_att_row(p, mr.run, 0, a.yaw, a.pitch, a.roll);
     for (int64_t i = 0; i < rounds + 2; ++i) {
       B2_CLK(ca0);
 #ifdef B2INS_PHASE_CLOCKS
@@ -253,55 +226,40 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
           att_step(a, w, p.dt, ((r0 + k + 1) & (kResync - 1)) == 0);
           ring_store(k);
           int64_t row;
-          if (warp_dumps && dump && j == 0 && p.out_att && dump_row(p, r0 + k + 1, &row)) {
-            const int64_t o = run * p.osr + row * p.ost;
-            const double y = wrap_once(a.yaw), r = wrap_once(a.roll);
-            p.out_att[o] = y;
-            p.out_att[o + p.osc] = a.pitch;
-            p.out_att[o + 2 * p.osc] = r;
-            if (p.out_quat) write_quat(p.out_quat + (run * p.dump_rows + row) * 4, y, a.pitch, r);
-          }
+          if (mr.warp_dumps && mr.dump && j == 0 && p.out_att && dump_row(p, r0 + k + 1, &row))
+            put_att_row(p, mr.run, row, wrap_once(a.yaw), a.pitch, wrap_once(a.roll));
         };
-        if (warp_dumps || kmax < kAvRound) {
+        if (mr.warp_dumps || kmax < kAvRound) {
 #pragma unroll 1
           for (int k = 0; k < kmax; ++k) a_step(k);
         } else {
-          // Blocks of four steps as ONE basic block without the exact-path branch (mc_spec_kernel.cuh has
-          // the same scheme): the next step's rate products overlap the tail of the previous one.  The
-          // block's gyro samples are loaded at its start, so that no shared load waits behind the ring
-          // stores of the step before.  A block in which any lane needed the exact path is redone step
-          // by step from the saved state; the ring is overwritten with the same or the corrected values
-          // before V sees it (V reads after the next barrier).
-          static_assert(kAvRound % 4 == 0 && kResync % 4 == 0, "blocks of four steps");
+          // Blocks of four steps (spec_block).  The block's gyro samples are loaded at its start, so that no
+          // shared load waits behind the ring stores of the step before.  A redone block rewrites the ring
+          // with the same or the corrected values before V sees it (V reads after the next barrier).
 #pragma unroll 1
-          for (int kb = 0; kb < kAvRound; kb += 4) {
-            const AttState saved = a;
-            Vec3 w[4];
+          for (int kb = 0; kb < kAvRound; kb += kSpecBlock) {
+            Vec3 w[kSpecBlock];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
+            for (int k = 0; k < kSpecBlock; ++k) {
               const SampleSlot& sl = sm.slot[sbuf][(kb + k) / G][lane - j + ((kb + k) % G)];
               w[k] = Vec3{sl.g[0], sl.g[1], sl.g[2]};
             }
-            bool cold = false;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              cold |= att_step<true>(a, w[k], p.dt, false);
+            AttState saved;
+            const bool redone = spec_block(true, a, saved, [&](int k) {
+              const bool cold = att_step<true>(a, w[k], p.dt, false);
               ring_store(kb + k);
-            }
-            B2_CLK(cr0);
-            if (__builtin_expect(__any_sync(0xffffffffu, cold), 0)) {
-              a = saved;
-#pragma unroll 1
-              for (int k = 0; k < 4; ++k) a_step(kb + k);
-            } else if (((r0 + kb + 4) & (kResync - 1)) == 0) {
+              return cold;
+            }, [&](int k) { a_step(kb + k); });
+            if (!redone && ((r0 + kb + kSpecBlock) & (kResync - 1)) == 0) {
               // the time-based re-evaluation (1 block of 16) falls on the block's last step: att_step's
               // exact path after it, as att_step(..., resync = true) takes it
+              B2_CLK(cr0);
               att_exact(a);
               a.icp = rcp_nr(a.sc.cp) * p.dt;
-              ring_store(kb + 3);
+              ring_store(kb + kSpecBlock - 1);
+              B2_CLK(cr1);
+              B2_ACC(10, cr0, cr1);
             }
-            B2_CLK(cr1);
-            B2_ACC(10, cr0, cr1);
           }
         }
       }
@@ -311,19 +269,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
       B2_CLK(ca2);
       B2_ACC(9, ca1, ca2);
     }
-    if (active && j == 0) {
-      const double* r = p.ref_nav + (p.n - 1) * 9;
-      if (p.end_err) {
-        double* e = p.end_err + run * 9;
-        e[0] = angle_range_pi(a.yaw - r[0]);
-        e[1] = angle_range_pi(a.pitch - r[1]);
-        e[2] = angle_range_pi(a.roll - r[2]);
-      }
-      if (p.end_state) {
-        double* e = p.end_state + run * 9;
-        e[0] = wrap_once(a.yaw); e[1] = a.pitch; e[2] = wrap_once(a.roll);
-      }
-    }
+    if (mr.active && j == 0) put_end<true, false>(p, mr.run, a.yaw, a.pitch, a.roll, Vec3{}, Vec3{});
     return;
   }
 
@@ -334,15 +280,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
   v.pos = st0.pos;
   v.gdt = st0.g * p.dt;
   SinCos3 old = st0.sc;
-  if (dump && j == 0 && p.out_att) {
-    const int64_t o = run * p.osr;
-    p.out_pos[o] = v.pos.x;
-    p.out_pos[o + p.osc] = v.pos.y;
-    p.out_pos[o + 2 * p.osc] = v.pos.z;
-    p.out_vel[o] = v.vel.x;
-    p.out_vel[o + p.osc] = v.vel.y;
-    p.out_vel[o + 2 * p.osc] = v.vel.z;
-  }
+  if (mr.dump && j == 0 && p.out_att) put_pv_row(p, mr.run, 0, v.pos, v.vel);
   for (int64_t i = 0; i < rounds + 2; ++i) {
     B2_CLK(cv0);
 #ifdef B2INS_PHASE_CLOCKS
@@ -363,17 +301,9 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
         vel_step(v, w, f, old, now, p.dt);
         old = now;
         int64_t row;
-        if (hist && dump && j == 0 && p.out_att && dump_row(p, r0 + k + 1, &row)) {
-          const int64_t oo = run * p.osr + row * p.ost;
-          p.out_pos[oo] = v.pos.x;
-          p.out_pos[oo + p.osc] = v.pos.y;
-          p.out_pos[oo + 2 * p.osc] = v.pos.z;
-          p.out_vel[oo] = v.vel.x;
-          p.out_vel[oo + p.osc] = v.vel.y;
-          p.out_vel[oo + 2 * p.osc] = v.vel.z;
-        }
+        if (hist && mr.dump && j == 0 && p.out_att && dump_row(p, r0 + k + 1, &row)) put_pv_row(p, mr.run, row, v.pos, v.vel);
       };
-      if (warp_dumps || kmax < kAvRound) {
+      if (mr.warp_dumps || kmax < kAvRound) {
 #pragma unroll 1
         for (int k = 0; k < kmax; ++k) v_step(k, true);
       } else {
@@ -390,23 +320,7 @@ __global__ void __launch_bounds__(AvShape<G>::kWarps * 32, 1) mc_av_kernel(const
     B2_CLK(cv2);
     B2_ACC(12, cv1, cv2);
   }
-  if (active && j == 0) {
-    const double* r = p.ref_nav + (p.n - 1) * 9;
-    if (p.end_err) {
-      double* e = p.end_err + run * 9;
-      e[3] = v.pos.x - r[3];
-      e[4] = v.pos.y - r[4];
-      e[5] = v.pos.z - r[5];
-      e[6] = v.vel.x - r[6];
-      e[7] = v.vel.y - r[7];
-      e[8] = v.vel.z - r[8];
-    }
-    if (p.end_state) {
-      double* e = p.end_state + run * 9;
-      e[3] = v.pos.x; e[4] = v.pos.y; e[5] = v.pos.z;
-      e[6] = v.vel.x; e[7] = v.vel.y; e[8] = v.vel.z;
-    }
-  }
+  if (mr.active && j == 0) put_end<false, true>(p, mr.run, 0.0, 0.0, 0.0, v.pos, v.vel);
 }
 
 }  // namespace b2ins

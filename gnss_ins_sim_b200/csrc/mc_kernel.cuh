@@ -114,39 +114,58 @@ struct TileSmem {
 
 // Issue the copies of one tile: the 16-byte-multiple part by bulk async copy (TMA)
 // completing on full[s]; an odd sample count leaves one 8-byte tail copied by hand.
-template <bool FED, bool PROC>
-__device__ __forceinline__ void issue_tile(TileSmem<PROC>& sm, const McParams& p, int64_t tile, int s) {
+// Smem: TileSmem, or the warp-specialised kernels' layouts (gyro and accel only: FED = PROC = false).
+template <bool FED, bool PROC, class Smem>
+__device__ __forceinline__ void issue_tile(Smem& sm, const McParams& p, int64_t tile, int s) {
   const int64_t t0 = tile * kTile;
   const uint32_t cnt = static_cast<uint32_t>(min64(kTile, p.n - t0));
   uint32_t tx = 0;
   if (!FED) tx += 2u * ((cnt * 24u) & ~15u);
   if (PROC) tx += (cnt * 72u) & ~15u;
   // the hand-copied tails are ordered before the arrive (release) below
-  if (!FED) {
+  if constexpr (!FED) {
     if ((cnt * 24u) & 8u) {
       const uint32_t o = ((cnt * 24u) & ~15u) / 8;
       sm.gyro[s][o] = p.ref_gyro[t0 * 3 + o];
       sm.accel[s][o] = p.ref_accel[t0 * 3 + o];
     }
   }
-  if (PROC) {
+  if constexpr (PROC) {
     if ((cnt * 72u) & 8u) {
       const uint32_t o = ((cnt * 72u) & ~15u) / 8;
       sm.nav[s][o] = p.ref_nav[t0 * 9 + o];
     }
   }
   mbar_arrive_expect_tx(&sm.full[s], tx);
-  if (!FED) {
+  if constexpr (!FED) {
     const uint32_t b = (cnt * 24u) & ~15u;
     if (b) {
       bulk_g2s(sm.gyro[s], p.ref_gyro + t0 * 3, b, &sm.full[s]);
       bulk_g2s(sm.accel[s], p.ref_accel + t0 * 3, b, &sm.full[s]);
     }
   }
-  if (PROC) {
+  if constexpr (PROC) {
     const uint32_t b = (cnt * 72u) & ~15u;
     if (b) bulk_g2s(sm.nav[s], p.ref_nav + t0 * 9, b, &sm.full[s]);
   }
+}
+
+// Refill the stage the PREVIOUS tile used (its consumers have had a whole tile to release it, so the
+// issuing thread hardly ever waits), then wait for tile `tile`'s data in stage s, phase `parity`.
+// 32-bit counts: n < 2^32 (b2ins_api.cu).  Phase clock slot `clk` times the wait.
+template <bool FED, bool PROC, class Smem>
+__device__ __forceinline__ void refill_and_wait(Smem& sm, const McParams& p, bool issuer, int tile,
+                                                int num_tiles, int s, uint32_t parity, int clk) {
+  constexpr int kStages = sizeof(Smem::full) / sizeof(uint64_t);
+  if (issuer && tile >= 1 && tile - 1 + kStages < num_tiles) {
+    const int sp = (tile - 1) % kStages;
+    mbar_wait(&sm.empty[sp], static_cast<uint32_t>(((tile - 1) / kStages) & 1));
+    issue_tile<FED, PROC>(sm, p, tile - 1 + kStages, sp);
+  }
+  B2_CLK(cw0);
+  mbar_wait(&sm.full[s], parity);
+  B2_CLK(cw1);
+  B2_ACC(clk, cw0, cw1);
 }
 
 // Vibration term of one axis (pathgen.py:477-493 / :540-555); only called when a model is on.
@@ -247,6 +266,110 @@ __device__ __forceinline__ void write_quat(double* q, double yaw, double pitch, 
   q[3] = sy * cp * cr - cy * sp * sr;
 }
 
+// ---- the per-run skeleton of the three Monte-Carlo kernels ------------------------------------------
+// The run a lane works on, from its place in the grid (run_raw).
+struct McRun {
+  int64_t run;       // the run of this launch; groups past the last run shadow it (and write nothing)
+  uint32_t lo, hi;   // the global run id (Philox key words)
+  bool active;       // run_raw is a run of this launch
+  bool dump;         // the run's histories are written
+  bool warp_dumps;   // some lane of the warp writes histories
+};
+__device__ __forceinline__ McRun mc_run(const McParams& p, int64_t run_raw) {
+  McRun r;
+  r.active = run_raw < p.runs;
+  r.run = r.active ? run_raw : p.runs - 1;
+  const int64_t grun = p.run_offset + r.run;
+  r.lo = static_cast<uint32_t>(grun);
+  r.hi = static_cast<uint32_t>(grun >> 32);
+  r.dump = r.active && r.run < p.dump_runs;
+  r.warp_dumps = __any_sync(0xffffffffu, r.dump);
+  return r;
+}
+
+// sample 0 of a run: its initial-state set (free_integration.py:85-87: one set for every run, or one each)
+template <int RF>
+__device__ __forceinline__ NavState mc_init(const McParams& p, int64_t run) {
+  NavState st;
+  const int64_t irun = p.ini_offset + run;
+  const int64_t set = (irun < p.ini_sets) ? irun : 0;
+  nav_init<RF>(st, p.ini + set * p.ini_rows, p.ini_rows, p.dt);
+  return st;
+}
+
+// History rows: the attitude (and its quaternion), position and velocity of one kept sample
+__device__ __forceinline__ void put_att_row(const McParams& p, int64_t run, int64_t row, double yaw, double pitch,
+                                            double roll) {
+  const int64_t o = run * p.osr + row * p.ost;
+  p.out_att[o] = yaw;
+  p.out_att[o + p.osc] = pitch;
+  p.out_att[o + 2 * p.osc] = roll;
+  if (p.out_quat) write_quat(p.out_quat + (run * p.dump_rows + row) * 4, yaw, pitch, roll);
+}
+__device__ __forceinline__ void put_pv_row(const McParams& p, int64_t run, int64_t row, const Vec3& pos,
+                                           const Vec3& vel) {
+  const int64_t o = run * p.osr + row * p.ost;
+  p.out_pos[o] = pos.x;
+  p.out_pos[o + p.osc] = pos.y;
+  p.out_pos[o + 2 * p.osc] = pos.z;
+  p.out_vel[o] = vel.x;
+  p.out_vel[o + p.osc] = vel.y;
+  p.out_vel[o + 2 * p.osc] = vel.z;
+}
+__device__ __forceinline__ void put_state_row(const McParams& p, int64_t run, int64_t row, double yaw, double pitch,
+                                              double roll, const Vec3& pos, const Vec3& vel) {
+  put_pv_row(p, run, row, pos, vel);
+  put_att_row(p, run, row, yaw, pitch, roll);
+}
+
+// Lane k of a group keeps the state after step k of a pass (the outputs' wrap applied) ...
+__device__ __forceinline__ void keep_state(double* keep, const NavState& st) {
+  keep[0] = wrap_once(st.yaw); keep[1] = st.pitch; keep[2] = wrap_once(st.roll);
+  keep[3] = st.pos.x; keep[4] = st.pos.y; keep[5] = st.pos.z;
+  keep[6] = st.vel.x; keep[7] = st.vel.y; keep[8] = st.vel.z;
+}
+// ... and writes it after the pass as the row of sample t + 1 (t: the lane's sample of the pass)
+__device__ __forceinline__ void put_kept_row(const McParams& p, int64_t run, int64_t t, const double* keep) {
+  int64_t row;
+  if (p.out_att && t + 1 < p.n && dump_row(p, t + 1, &row))
+    put_state_row(p, run, row, keep[0], keep[1], keep[2], Vec3{keep[3], keep[4], keep[5]},
+                  Vec3{keep[6], keep[7], keep[8]});
+}
+
+// Per-run results at the last sample: the end-point error against the reference (angles by
+// angle_range_pi) and the end state (yaw and roll wrapped once); ATT: the attitude part, PV: position, velocity
+template <bool ATT, bool PV>
+__device__ __forceinline__ void put_end(const McParams& p, int64_t run, double yaw, double pitch, double roll,
+                                        const Vec3& pos, const Vec3& vel) {
+  if (p.end_err) {
+    const double* r = p.ref_nav + (p.n - 1) * 9;
+    double* e = p.end_err + run * 9;
+    if (ATT) {
+      e[0] = angle_range_pi(yaw - r[0]);
+      e[1] = angle_range_pi(pitch - r[1]);
+      e[2] = angle_range_pi(roll - r[2]);
+    }
+    if (PV) {
+      e[3] = pos.x - r[3];
+      e[4] = pos.y - r[4];
+      e[5] = pos.z - r[5];
+      e[6] = vel.x - r[6];
+      e[7] = vel.y - r[7];
+      e[8] = vel.z - r[8];
+    }
+  }
+  if (p.end_state) {
+    double* e = p.end_state + run * 9;
+    if (ATT) {
+      e[0] = wrap_once(yaw); e[1] = pitch; e[2] = wrap_once(roll);
+    }
+    if (PV) {
+      e[3] = pos.x; e[4] = pos.y; e[5] = pos.z;
+      e[6] = vel.x; e[7] = vel.y; e[8] = vel.z;
+    }
+  }
+}
+
 // process-error accumulation of one sample (ins_data_manager.py:536-541, :761-808)
 __device__ __forceinline__ void proc_accumulate(const NavState& st, const double* r, double* pe_max,
                                                 double* pe_sum, double* pe_sq, double* pe_k,
@@ -308,14 +431,7 @@ mc_kernel(const __grid_constant__ McParams p) {
   const int warp = threadIdx.x >> 5;
   const int j = lane % G;
   const int role = lane & 3;
-  const int64_t run_raw =
-      (static_cast<int64_t>(blockIdx.x) * kWarps + warp) * kRunsPerWarp + lane / G;
-  const bool active = run_raw < p.runs;
-  const int64_t run = active ? run_raw : p.runs - 1;  // idle groups shadow the last run
-  const int64_t grun = p.run_offset + run;            // global run id
-  const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
-  const bool dump = active && run < p.dump_runs;
-  const bool warp_dumps = __any_sync(0xffffffffu, dump);
+  const McRun mr = mc_run(p, (static_cast<int64_t>(blockIdx.x) * kWarps + warp) * kRunsPerWarp + lane / G);
   const bool odo_mode = p.algo == 1;
   constexpr bool kStaged = !FED || PROC;
   constexpr int kStages = Stages<PROC>::value;
@@ -336,12 +452,7 @@ mc_kernel(const __grid_constant__ McParams p) {
   }
 
   // ---- sample 0 ----------------------------------------------------------
-  NavState st;
-  {
-    const int64_t irun = p.ini_offset + run;
-    const int64_t set = (irun < p.ini_sets) ? irun : 0;  // free_integration.py:85-87
-    nav_init<RF>(st, p.ini + set * p.ini_rows, p.ini_rows, p.dt);
-  }
+  NavState st = mc_init<RF>(p, mr.run);
   // Gauss-Markov drift carried across blocks (d[0] = 0), and the powers a^j, a^G
   double carry[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   double apj[6], aG[6];
@@ -357,21 +468,9 @@ mc_kernel(const __grid_constant__ McParams p) {
   if (!FED && p.gyro.vib_type == 2) {
 #pragma unroll
     for (int c = 0; c < 3; ++c)  // np.random.rand(1)*2*pi, pathgen.py:553-555
-      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
+      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, mr.lo, mr.hi, p.k0, p.k1) * 2.0) * kPi;
   }
-  if (dump && j == 0 && p.out_att) {
-    const int64_t o = run * p.osr;
-    p.out_att[o] = st.yaw;
-    p.out_att[o + p.osc] = st.pitch;
-    p.out_att[o + 2 * p.osc] = st.roll;
-    p.out_pos[o] = st.pos.x;
-    p.out_pos[o + p.osc] = st.pos.y;
-    p.out_pos[o + 2 * p.osc] = st.pos.z;
-    p.out_vel[o] = st.vel.x;
-    p.out_vel[o + p.osc] = st.vel.y;
-    p.out_vel[o + 2 * p.osc] = st.vel.z;
-    if (p.out_quat) write_quat(p.out_quat + run * p.dump_rows * 4, st.yaw, st.pitch, st.roll);
-  }
+  if (mr.dump && j == 0 && p.out_att) put_state_row(p, mr.run, 0, st.yaw, st.pitch, st.roll, st.pos, st.vel);
   // process-error accumulators (shifted sums: K = first error sample)
   double pe_max[9], pe_sum[9], pe_sq[9], pe_k[9];
   int64_t pe_cnt = 0;
@@ -386,19 +485,9 @@ mc_kernel(const __grid_constant__ McParams p) {
     const uint32_t parity = static_cast<uint32_t>((tile / kStages) & 1);
     const int64_t t0 = tile * kTile;
     const int cnt = static_cast<int>(min64(kTile, p.n - t0));
-    if (kStaged) {
-      // refill the stage the PREVIOUS tile used (all warps have had a whole tile to release
-      // it, so the issuing thread hardly ever waits), then wait for this tile's data
-      if (threadIdx.x == 0 && tile >= 1 && tile - 1 + kStages < num_tiles) {
-        const int sp = static_cast<int>((tile - 1) % kStages);
-        mbar_wait(&sm.empty[sp], static_cast<uint32_t>(((tile - 1) / kStages) & 1));
-        issue_tile<FED, PROC>(sm, p, tile - 1 + kStages, sp);
-      }
-      B2_CLK(cw0);
-      mbar_wait(&sm.full[s], parity);
-      B2_CLK(cw1);
-      B2_ACC(0, cw0, cw1);
-    }
+    if (kStaged)
+      refill_and_wait<FED, PROC>(sm, p, threadIdx.x == 0, static_cast<int>(tile),
+                                 static_cast<int>(num_tiles), s, parity, 0);
 
     for (int base = 0; base < cnt; base += G) {
       B2_CLK(ca0);
@@ -410,13 +499,13 @@ mc_kernel(const __grid_constant__ McParams p) {
       {
       if (FED) {
         if (tj < cnt) {
-          const int64_t o = run * p.sr + t * p.st;
+          const int64_t o = mr.run * p.sr + t * p.st;
 #pragma unroll
           for (int c = 0; c < 3; ++c) {
             mg[c] = p.fed_gyro[o + c * p.sc];
             ma[c] = odo_mode ? 0.0 : p.fed_accel[o + c * p.sc];
           }
-          if (odo_mode) mo = p.fed_odo[run * p.so_r + t * p.so_t];
+          if (odo_mode) mo = p.fed_odo[mr.run * p.so_r + t * p.so_t];
         } else {
 #pragma unroll
           for (int c = 0; c < 3; ++c) mg[c] = ma[c] = 0.0;
@@ -424,8 +513,8 @@ mc_kernel(const __grid_constant__ McParams p) {
       } else {
         double zg[3], za[3];
         if (tj < cnt) {
-          noisy_sample(p, &sm.accel[s][tj * 3], &sm.gyro[s][tj * 3], static_cast<uint32_t>(t), run_lo,
-                       run_hi, run, phase, ma, mg, za, zg);
+          noisy_sample(p, &sm.accel[s][tj * 3], &sm.gyro[s][tj * 3], static_cast<uint32_t>(t), mr.lo,
+                       mr.hi, mr.run, phase, ma, mg, za, zg);
         } else {
 #pragma unroll
           for (int c = 0; c < 3; ++c) mg[c] = ma[c] = zg[c] = za[c] = 0.0;
@@ -443,20 +532,20 @@ mc_kernel(const __grid_constant__ McParams p) {
           mg[c] += dg + p.gyro.wd[c] * zg[c];
         }
         if (odo_mode) {   // pathgen.odo_gen, pathgen.py:627-641: scale*ref + stdv*randn
-          const double zo = (tj < cnt) ? normal_pair(static_cast<uint32_t>(t), kDrawOdo, run_lo, run_hi,
+          const double zo = (tj < cnt) ? normal_pair(static_cast<uint32_t>(t), kDrawOdo, mr.lo, mr.hi,
                                                      p.k0, p.k1).z0 : 0.0;
           mo = (tj < cnt) ? p.odo_scale * p.ref_odo[t] + p.odo_stdv * zo : 0.0;
         }
       }
       int64_t row;
-      if (warp_dumps && dump && tj < cnt && p.out_gyro && dump_row(p, t, &row)) {
-        const int64_t o = run * p.osr + row * p.ost;
+      if (mr.warp_dumps && mr.dump && tj < cnt && p.out_gyro && dump_row(p, t, &row)) {
+        const int64_t o = mr.run * p.osr + row * p.ost;
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           p.out_gyro[o + c * p.osc] = mg[c];
           p.out_accel[o + c * p.osc] = ma[c];
         }
-        if (odo_mode && p.out_odo) p.out_odo[run * p.dump_rows + row] = mo;
+        if (odo_mode && p.out_odo) p.out_odo[mr.run * p.dump_rows + row] = mo;
       }
       if (odo_mode) {   // the odometer sample rides to phase B in the accel.x slot
         ma[0] = mo;
@@ -500,13 +589,9 @@ mc_kernel(const __grid_constant__ McParams p) {
         // every lane-group width)
         const bool resync = ((t0 + base + k + 1) & (kResync - 1)) == 0;
         nav_step<RF, kSplit, 2>(st, w, f, p.dt, p.earth_rot != 0, role, resync, odo_mode);
-        if (hist && j == k) {
-          keep[0] = wrap_once(st.yaw); keep[1] = st.pitch; keep[2] = wrap_once(st.roll);
-          keep[3] = st.pos.x; keep[4] = st.pos.y; keep[5] = st.pos.z;
-          keep[6] = st.vel.x; keep[7] = st.vel.y; keep[8] = st.vel.z;
-        }
+        if (hist && j == k) keep_state(keep, st);
       };
-      if (warp_dumps) {            // history output: the rare path keeps the simple loop
+      if (mr.warp_dumps) {         // history output: the rare path keeps the simple loop
 #pragma unroll 1
         for (int k = 0; k < kmax; ++k) one_step(k, true);
       } else {
@@ -524,18 +609,7 @@ mc_kernel(const __grid_constant__ McParams p) {
       B2_CLK(cb1);
       B2_ACC(3, cb0, cb1);
       // ---------------- histories: lane j writes the state of sample base+j+1 ---------
-      int64_t hrow;
-      if (warp_dumps && dump && tj < cnt && p.out_att && t + 1 < p.n && dump_row(p, t + 1, &hrow)) {
-        const int64_t row = hrow;
-        const int64_t o = run * p.osr + row * p.ost;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          p.out_att[o + c * p.osc] = keep[c];
-          p.out_pos[o + c * p.osc] = keep[3 + c];
-          p.out_vel[o + c * p.osc] = keep[6 + c];
-        }
-        if (p.out_quat) write_quat(p.out_quat + (run * p.dump_rows + row) * 4, keep[0], keep[1], keep[2]);
-      }
+      if (mr.warp_dumps && mr.dump && tj < cnt) put_kept_row(p, mr.run, t, keep);
     }
 
     if (kStaged) {
@@ -549,28 +623,10 @@ mc_kernel(const __grid_constant__ McParams p) {
     if (p.n - 1 >= p.stats_start)
       proc_accumulate(st, p.ref_nav + (p.n - 1) * 9, pe_max, pe_sum, pe_sq, pe_k, pe_cnt);
   }
-  if (active && j == 0) {
-    if (p.end_err) {
-      const double* r = p.ref_nav + (p.n - 1) * 9;
-      double* e = p.end_err + run * 9;
-      e[0] = angle_range_pi(st.yaw - r[0]);
-      e[1] = angle_range_pi(st.pitch - r[1]);
-      e[2] = angle_range_pi(st.roll - r[2]);
-      e[3] = st.pos.x - r[3];
-      e[4] = st.pos.y - r[4];
-      e[5] = st.pos.z - r[5];
-      e[6] = st.vel.x - r[6];
-      e[7] = st.vel.y - r[7];
-      e[8] = st.vel.z - r[8];
-    }
-    if (p.end_state) {
-      double* e = p.end_state + run * 9;
-      e[0] = wrap_once(st.yaw); e[1] = st.pitch; e[2] = wrap_once(st.roll);
-      e[3] = st.pos.x; e[4] = st.pos.y; e[5] = st.pos.z;
-      e[6] = st.vel.x; e[7] = st.vel.y; e[8] = st.vel.z;
-    }
+  if (mr.active && j == 0) {
+    put_end<true, true>(p, mr.run, st.yaw, st.pitch, st.roll, st.pos, st.vel);
     if (PROC && p.proc_stats) {
-      double* o = p.proc_stats + run * 27;
+      double* o = p.proc_stats + mr.run * 27;
       const double inv = pe_cnt > 0 ? 1.0 / static_cast<double>(pe_cnt) : 0.0;
 #pragma unroll
       for (int c = 0; c < 9; ++c) {

@@ -34,9 +34,9 @@ struct SpecShape {
   static constexpr bool kSpare = (P == 6 && WI == 1);
   static constexpr int kThreads = (WI * (1 + P) + (kSpare ? 1 : 0)) * 32;
   static constexpr int kChan = 6 / P;                 // channels per producer warp
-  // speculative straight-line blocks (see the integrator loop): groups of 4 and 8 lanes, the shapes of
-  // the few-runs configurations, which run without a register cap
-  static constexpr int kSpecBlock = (G == 4 || G == 8) ? 4 : 0;
+  // speculative blocks (spec_block, mech.cuh): groups of 4 and 8 lanes, the shapes of the few-runs
+  // configurations, which run without a register cap
+  static constexpr bool kSpec = (G == 4 || G == 8);
   static_assert(6 % P == 0 && kTile % kRound == 0 && 32 % G == 0, "shape");
 };
 
@@ -46,28 +46,10 @@ struct SpecSmem {
   alignas(128) double accel[kStagesFast][kTile * 3];
   alignas(16) SampleSlot slot[2][SpecShape<G, P, WI>::kPasses][WI][32];
   // the state before a speculative block (integrator lanes; one dummy element where there are none)
-  alignas(16) NavState saved[SpecShape<G, P, WI>::kSpecBlock ? WI : 1][SpecShape<G, P, WI>::kSpecBlock ? 32 : 1];
+  alignas(16) NavState saved[SpecShape<G, P, WI>::kSpec ? WI : 1][SpecShape<G, P, WI>::kSpec ? 32 : 1];
   alignas(8) uint64_t full[kStagesFast];
   alignas(8) uint64_t empty[kStagesFast];
 };
-
-// copies of one trajectory tile (gyro + accel) into stage s; see issue_tile in mc_kernel.cuh
-template <class Smem>
-__device__ __forceinline__ void spec_issue_tile(Smem& sm, const McParams& p, int64_t tile, int s) {
-  const int64_t t0 = tile * kTile;
-  const uint32_t cnt = static_cast<uint32_t>(min64(kTile, p.n - t0));
-  const uint32_t b = (cnt * 24u) & ~15u;
-  if ((cnt * 24u) & 8u) {   // odd sample count: the 8-byte tail by hand, ordered before the arrive
-    const uint32_t o = b / 8;
-    sm.gyro[s][o] = p.ref_gyro[t0 * 3 + o];
-    sm.accel[s][o] = p.ref_accel[t0 * 3 + o];
-  }
-  mbar_arrive_expect_tx(&sm.full[s], 2u * b);
-  if (b) {
-    bulk_g2s(sm.gyro[s], p.ref_gyro + t0 * 3, b, &sm.full[s]);
-    bulk_g2s(sm.accel[s], p.ref_accel + t0 * 3, b, &sm.full[s]);
-  }
-}
 
 template <int G, int RF, int P, int WI, bool SPLIT, int MINB>
 __global__ void __launch_bounds__(SpecShape<G, P, WI>::kThreads, MINB)
@@ -77,7 +59,6 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
   __shared__ SpecSmem<G, P, WI> sm;
   constexpr int kRunsPerWarp = 32 / G;
   constexpr int kChan = Sh::kChan;
-  constexpr int kSpecBlock = Sh::kSpecBlock;
   const int lane = threadIdx.x & 31;
   const int pwarp = threadIdx.x >> 5;
   const bool integrator = pwarp < WI;
@@ -87,13 +68,7 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
   const int pp = integrator ? 0 : pidx % P;                // producer index within the group
   const int j = lane % G;
   const int role = lane & 3;
-  const int64_t run_raw = (static_cast<int64_t>(blockIdx.x) * WI + gi) * kRunsPerWarp + lane / G;
-  const bool active = run_raw < p.runs;
-  const int64_t run = active ? run_raw : p.runs - 1;       // idle groups shadow the last run
-  const int64_t grun = p.run_offset + run;
-  const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
-  const bool dump = active && run < p.dump_runs;
-  const bool warp_dumps = __any_sync(0xffffffffu, dump);
+  const McRun mr = mc_run(p, (static_cast<int64_t>(blockIdx.x) * WI + gi) * kRunsPerWarp + lane / G);
   // (the odometer variant, cfg.algo = 1, takes the single-warp form: mc_kernel)
   const int64_t num_tiles = (p.n + kTile - 1) / kTile;
   const int issuer = WI * 32;                              // lane 0 of the first producer warp
@@ -112,7 +87,7 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
   if (!integrator) {
     // =============================== producer ===============================================
     if (threadIdx.x == issuer)
-      for (int s = 0; s < kStagesFast && s < num_tiles; ++s) spec_issue_tile(sm, p, s, s);
+      for (int s = 0; s < kStagesFast && s < num_tiles; ++s) issue_tile<false, false>(sm, p, s, s);
     // error model of this producer's channels (c < 3: accel axis c, else gyro axis c - 3)
     double carry[kChan], apj[kChan], aG[kChan];
 #pragma unroll
@@ -127,7 +102,7 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
     if (p.gyro.vib_type == 2) {
 #pragma unroll
       for (int c = 0; c < 3; ++c)  // np.random.rand(1)*2*pi, pathgen.py:553-555
-        phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
+        phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, mr.lo, mr.hi, p.k0, p.k1) * 2.0) * kPi;
     }
     const bool any_vib = (p.accel.vib_type | p.gyro.vib_type) != 0;
     int rnd = 0;
@@ -136,17 +111,8 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
       const uint32_t parity = static_cast<uint32_t>((tile / kStagesFast) & 1);
       const int64_t t0 = tile * kTile;
       const int cnt = static_cast<int>(min64(kTile, p.n - t0));
-      // refill the stage the PREVIOUS tile used (every producer warp has had a whole tile to release
-      // it), then wait for this tile's data
-      if (threadIdx.x == issuer && tile >= 1 && tile - 1 + kStagesFast < num_tiles) {
-        const int sp = static_cast<int>((tile - 1) % kStagesFast);
-        mbar_wait(&sm.empty[sp], static_cast<uint32_t>(((tile - 1) / kStagesFast) & 1));
-        spec_issue_tile(sm, p, tile - 1 + kStagesFast, sp);
-      }
-      B2_CLK(cw0);
-      mbar_wait(&sm.full[s], parity);
-      B2_CLK(cw1);
-      B2_ACC(0, cw0, cw1);
+      refill_and_wait<false, false>(sm, p, threadIdx.x == issuer, static_cast<int>(tile),
+                                    static_cast<int>(num_tiles), s, parity, 0);
       for (int base = 0; base < cnt; base += Sh::kRound, ++rnd) {
         const int buf = rnd & 1;
         B2_CLK(cp0);
@@ -166,8 +132,8 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
             for (int q = 0; q < kChan; ++q) {
               z[bi][q] = Normal2{0.0, 0.0};
               if (kIlp > 1 || base + (b0 + bi) * G + j < cnt)
-                z[bi][q] = normal_pair(static_cast<uint32_t>(t0 + base + (b0 + bi) * G + j), pp * kChan + q, run_lo,
-                                       run_hi, p.k0, p.k1);
+                z[bi][q] = normal_pair(static_cast<uint32_t>(t0 + base + (b0 + bi) * G + j), pp * kChan + q, mr.lo,
+                                       mr.hi, p.k0, p.k1);
             }
 #pragma unroll
           for (int bi = 0; bi < kIlp; ++bi) {
@@ -188,15 +154,15 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
                 const double ref = is_acc ? sm.accel[s][tj * 3 + ax] : sm.gyro[s][tj * 3 + ax];
                 m = (ref + e.b[ax]) + e.w[ax] * z[bi][q].z1;
                 if (any_vib)
-                  m += vib_term(e, ax, is_acc ? 0 : 1, static_cast<uint32_t>(t), run_lo, run_hi, p.k0, p.k1,
-                                run, phase);
+                  m += vib_term(e, ax, is_acc ? 0 : 1, static_cast<uint32_t>(t), mr.lo, mr.hi, p.k0, p.k1,
+                                mr.run, phase);
               }
               // + drift: the GM state d[t] (pathgen.py:583-590) or drift*z[t] if tau = inf (:591-593)
               const double d = gm_block<G>(e.gm_b[ax] * z0, e.gm_a[ax], apj[q], aG[q], j, carry[q]);
               m += d + e.wd[ax] * z0;
               int64_t row;
-              if (warp_dumps && dump && live && p.out_gyro && dump_row(p, t, &row))
-                (is_acc ? p.out_accel : p.out_gyro)[run * p.osr + row * p.ost + ax * p.osc] = m;
+              if (mr.warp_dumps && mr.dump && live && p.out_gyro && dump_row(p, t, &row))
+                (is_acc ? p.out_accel : p.out_gyro)[mr.run * p.osr + row * p.ost + ax * p.osc] = m;
               if (is_acc) mine.a[ax] = m; else mine.g[ax] = m;
             }
           }
@@ -214,25 +180,8 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
   }
 
   // ================================= integrator ===============================================
-  NavState st;
-  {
-    const int64_t irun = p.ini_offset + run;
-    const int64_t set = (irun < p.ini_sets) ? irun : 0;  // free_integration.py:85-87
-    nav_init<RF>(st, p.ini + set * p.ini_rows, p.ini_rows, p.dt);
-  }
-  if (dump && j == 0 && p.out_att) {
-    const int64_t o = run * p.osr;
-    p.out_att[o] = st.yaw;
-    p.out_att[o + p.osc] = st.pitch;
-    p.out_att[o + 2 * p.osc] = st.roll;
-    p.out_pos[o] = st.pos.x;
-    p.out_pos[o + p.osc] = st.pos.y;
-    p.out_pos[o + 2 * p.osc] = st.pos.z;
-    p.out_vel[o] = st.vel.x;
-    p.out_vel[o + p.osc] = st.vel.y;
-    p.out_vel[o + 2 * p.osc] = st.vel.z;
-    if (p.out_quat) write_quat(p.out_quat + run * p.dump_rows * 4, st.yaw, st.pitch, st.roll);
-  }
+  NavState st = mc_init<RF>(p, mr.run);
+  if (mr.dump && j == 0 && p.out_att) put_state_row(p, mr.run, 0, st.yaw, st.pitch, st.roll, st.pos, st.vel);
   int rnd = 0;
   for (int64_t tile = 0; tile < num_tiles; ++tile) {
     const int64_t t0 = tile * kTile;
@@ -262,56 +211,26 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
           const Vec3 f{sl.a[0], sl.a[1], sl.a[2]};
           const bool resync = ((t0 + pb + k + 1) & (kResync - 1)) == 0;
           nav_step<RF, SPLIT, 0>(st, w, f, p.dt, p.earth_rot != 0, role, resync);
-          if (hist && j == k) {
-            keep[0] = wrap_once(st.yaw); keep[1] = st.pitch; keep[2] = wrap_once(st.roll);
-            keep[3] = st.pos.x; keep[4] = st.pos.y; keep[5] = st.pos.z;
-            keep[6] = st.vel.x; keep[7] = st.vel.y; keep[8] = st.vel.z;
-          }
+          if (hist && j == k) keep_state(keep, st);
         };
-        if (warp_dumps) {            // history output: the rare path keeps the simple loop
+        if (mr.warp_dumps) {         // history output: the rare path keeps the simple loop
 #pragma unroll 1
           for (int k = 0; k < kmax; ++k) one_step(k, true);
           const int tj = pb + j;
-          const int64_t t = t0 + tj;
-          int64_t row;
-          if (dump && tj < cnt && p.out_att && t + 1 < p.n && dump_row(p, t + 1, &row)) {
-            const int64_t o = run * p.osr + row * p.ost;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              p.out_att[o + c * p.osc] = keep[c];
-              p.out_pos[o + c * p.osc] = keep[3 + c];
-              p.out_vel[o + c * p.osc] = keep[6 + c];
-            }
-            if (p.out_quat) write_quat(p.out_quat + (run * p.dump_rows + row) * 4, keep[0], keep[1], keep[2]);
-          }
+          if (mr.dump && tj < cnt) put_kept_row(p, mr.run, t0 + tj, keep);
         } else if (G == 1) {
           if (kmax > 0) one_step(0, false);
-        } else if (kSpecBlock > 0 && kmax == G) {
-          // Blocks of four steps as ONE basic block, no exact-path branch inside -- the next step's loads
-          // and rate products overlap the tail of the previous one -- unless the block holds a time-based
-          // re-evaluation (1 of 16).  If any lane needed the exact path (rare: an increment above
-          // kRotMax, a pitch reflection, a NaN) the warp restores the saved state and redoes the block
-          // step by step; every step computes the same numbers either way.
+        } else if (Sh::kSpec && kmax == G) {
+          // blocks of four steps, speculated unless the block holds a time-based re-evaluation (1 of 16)
 #pragma unroll 1
           for (int kb = 0; kb < G; kb += kSpecBlock) {
-            bool redo = (((t0 + pb + kb) & (kResync - 1)) + kSpecBlock >= kResync);
-            if (!redo) {
-              sm.saved[gi][lane] = st;
-              bool cold = false;
-#pragma unroll
-              for (int k = 0; k < kSpecBlock; ++k) {
-                const SampleSlot& sl = grp[kb + k];
-                const Vec3 w{sl.g[0], sl.g[1], sl.g[2]};
-                const Vec3 f{sl.a[0], sl.a[1], sl.a[2]};
-                cold |= nav_step<RF, SPLIT, 0, true>(st, w, f, p.dt, p.earth_rot != 0, role, false);
-              }
-              redo = __any_sync(0xffffffffu, cold);
-              if (__builtin_expect(redo, 0)) st = sm.saved[gi][lane];
-            }
-            if (redo) {
-#pragma unroll 1
-              for (int k = 0; k < kSpecBlock; ++k) one_step(kb + k, false);
-            }
+            const bool speculate = ((t0 + pb + kb) & (kResync - 1)) + kSpecBlock < kResync;
+            spec_block(speculate, st, sm.saved[gi][lane], [&](int k) {
+              const SampleSlot& sl = grp[kb + k];
+              const Vec3 w{sl.g[0], sl.g[1], sl.g[2]};
+              const Vec3 f{sl.a[0], sl.a[1], sl.a[2]};
+              return nav_step<RF, SPLIT, 0, true>(st, w, f, p.dt, p.earth_rot != 0, role, false);
+            }, [&](int k) { one_step(kb + k, false); });
           }
         } else {
           // two steps per iteration: the off-chain tail of step k overlaps the chain of step k + 1
@@ -330,26 +249,8 @@ mc_spec_kernel(const __grid_constant__ McParams p) {
   }
 
   // ---- per-run results ---------------------------------------------------------------------
-  if (active && j == 0) {
-    if (p.end_err) {
-      const double* r = p.ref_nav + (p.n - 1) * 9;
-      double* e = p.end_err + run * 9;
-      e[0] = angle_range_pi(st.yaw - r[0]);
-      e[1] = angle_range_pi(st.pitch - r[1]);
-      e[2] = angle_range_pi(st.roll - r[2]);
-      e[3] = st.pos.x - r[3];
-      e[4] = st.pos.y - r[4];
-      e[5] = st.pos.z - r[5];
-      e[6] = st.vel.x - r[6];
-      e[7] = st.vel.y - r[7];
-      e[8] = st.vel.z - r[8];
-    }
-    if (p.end_state) {
-      double* e = p.end_state + run * 9;
-      e[0] = wrap_once(st.yaw); e[1] = st.pitch; e[2] = wrap_once(st.roll);
-      e[3] = st.pos.x; e[4] = st.pos.y; e[5] = st.pos.z;
-      e[6] = st.vel.x; e[7] = st.vel.y; e[8] = st.vel.z;
-    }
+  if (mr.active && j == 0) {
+    put_end<true, true>(p, mr.run, st.yaw, st.pitch, st.roll, st.pos, st.vel);
   }
 }
 

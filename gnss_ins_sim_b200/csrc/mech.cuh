@@ -7,7 +7,8 @@
 #include "common.cuh"
 
 // B2INS_HOST_TEST (tools/step_host.cu): the mechanization also compiles for the host, so that the
-// step the kernels run is checked against the oracle on the CPU (tests/test_cpu_step.py)
+// step the kernels run, and their speculative block, are checked against the oracle on the CPU
+// (tests/test_cpu_step.py, tests/test_cpu_exact_path.py)
 #ifdef B2INS_HOST_TEST
 #define B2_DEV __host__ __device__ __forceinline__
 #else
@@ -167,6 +168,50 @@ constexpr double kRotMax = 0.03125;
 constexpr double kLatRotMax = 0.0009765625;   // 2^-10: the latitude moves ~1e-8 rad per step
 constexpr int kResync = 64;
 
+// ---- the speculative block ---------------------------------------------------------------------------
+// Steps with SPEC = true (below) have no exact-path branch, so kSpecBlock of them unroll into one basic
+// block and the scheduler overlaps the next step's rate products with the tail of the previous one.  If
+// any lane of the warp needed the exact path (rare: an increment above kRotMax, a pitch reflection, a NaN)
+// the warp restores the state saved before the block and redoes it step by step; every step computes the
+// same numbers either way.  mc_spec_kernel.cuh, mc_av_kernel.cuh's attitude warp and the host test
+// (tools/step_host.cu) all run spec_block.
+constexpr int kSpecBlock = 4;
+static_assert(kResync % kSpecBlock == 0, "a time-based re-evaluation falls on a block's last step");
+
+// any lane of the warp; on the host (tools/step_host.cu) one lane is the warp
+B2_DEV bool warp_any(bool x) {
+#ifdef __CUDA_ARCH__
+  return __any_sync(0xffffffffu, x);
+#else
+  return x;
+#endif
+}
+
+// One block of kSpecBlock steps of state s.  With `speculate`: save s in `saved` (the caller keeps it in
+// registers or shared memory), run spec(k) -- step k without the exact path, returning whether it was due --
+// for k = 0 .. kSpecBlock - 1, vote, and on a cold vote restore s and run exact(k) for every k.  Without it:
+// exact(k) at once.  Returns whether the block was run by exact().
+#ifdef B2INS_HOST_TEST
+#pragma nv_exec_check_disable   // the host test passes host lambdas
+#endif
+template <class State, class Spec, class Exact>
+B2_DEV bool spec_block(bool speculate, State& s, State& saved, Spec&& spec, Exact&& exact) {
+  bool redo = !speculate;
+  if (speculate) {
+    saved = s;
+    bool cold = false;
+#pragma unroll
+    for (int k = 0; k < kSpecBlock; ++k) cold |= spec(k);
+    redo = warp_any(cold);
+    if (__builtin_expect(redo, 0)) s = saved;
+  }
+  if (redo) {
+#pragma unroll 1
+    for (int k = 0; k < kSpecBlock; ++k) exact(k);
+  }
+  return redo;
+}
+
 B2_DEV void rot_small(double& s, double& c, double d) {
   const double z = d * d;
   double ps = b2_fma(z, -1.98412698412698412698e-04, 8.33333333333333333333e-03);
@@ -285,7 +330,7 @@ B2_DEV void resync_exact(NavState& s) {
 // block), 2 = decided by odo_rt at run time
 // SPEC (speculative): the step WITHOUT the exact-path branch -- straight-line code, so that several steps
 // unroll into one basic block and the scheduler overlaps them.  Returns whether the exact path was due
-// (an increment above kRotMax, a pitch reflection, a NaN); the caller then restores the state it saved
+// (an increment above kRotMax, a pitch reflection, a NaN); spec_block then restores the state it saved
 // and redoes the steps with SPEC = false.  (SPEC = false returns the same flag, already handled.)
 template <int RF, bool SPLIT, int ODO = 0, bool SPEC = false>
 B2_DEV bool nav_step(NavState& s, const Vec3& gyro, const Vec3& accel, double dt, bool earth_rot, int role,

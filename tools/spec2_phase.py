@@ -4,7 +4,7 @@
 mc_spec_kernel: per warp and per step, the cycles an integrator warp spends waiting at the hand-over
 barrier / stepping, and a producer warp waiting for tiles / producing / waiting at the barrier.
 mc_av_kernel (shape "6,2,0"): per warp of each role and per round of 8 samples, the attitude warp A
-stepping (of which in the step-by-step redo / exact re-evaluation) and waiting at the round barrier, the
+stepping (of which in the time-based re-evaluation after a warm block) and waiting at the round barrier, the
 velocity warp V stepping and waiting, the producers waiting for tiles / producing / waiting.
 Each case runs as is (idle: none) and with one role idle (B2INS_MC_DEBUG: 1 producers, 2 integrators or
 A, 4 V).  `spec2_phase.py av` runs the mc_av_kernel cases only.  GPU box only."""
@@ -66,7 +66,7 @@ def av_record(runs, lanes, dbg, ms, out, n):
     per = lambda i, warps: round(out[i] / warps / rounds, 1)     # noqa: E731
     return {'rf': 1, 'runs': runs, 'lanes': lanes, 'shape_P_WI_split': '6,2,0', 'kernel': 'mc_av_kernel',
             'idle': {0: 'none', 1: 'producers', 2: 'A', 4: 'V'}[dbg], 'ms': ms,
-            'A_cycles_per_round': {'stepping': per(8, ctas), 'of_which_redo_resync': per(10, ctas),
+            'A_cycles_per_round': {'stepping': per(8, ctas), 'of_which_reevaluation': per(10, ctas),
                                    'barrier_wait': per(9, ctas)},
             'V_cycles_per_round': {'stepping': per(11, ctas), 'barrier_wait': per(12, ctas)},
             'producer_cycles_per_round': {'warps_per_cta': prod, 'tile_wait': per(13, ctas * prod),

@@ -42,18 +42,18 @@ extern "C" int step_host_free_integration(int ref_frame, int64_t n, double fs, i
 extern "C" int step_host_resync_default(void) { return kResync; }
 
 // ---- the speculative blocks of the fused Monte-Carlo kernels, for one run (one lane of a warp) ----------
-// Steps are taken in blocks of four from step 0 while a whole block is left, the rest one by one, with the
-// time-based re-evaluation after every kResync-th sample, as the kernels do.  The rows of a block are written
-// once it has settled: what the kernels' end state and ring hold, not their (non-speculative) history path.
+// Steps are taken in blocks of kSpecBlock from step 0 while a whole block is left, the rest one by one, with the
+// time-based re-evaluation after every kResync-th sample, as the kernels do.  A block is the kernels' own
+// spec_block (mech.cuh); what is here is what the kernels do around it.  The rows of a block are written once
+// it has settled: what the kernels' end state and ring hold, not their (non-speculative) history path.
 
 static void put_row(double* o, int64_t i, double x, double y, double z) {
   o[i * 3 + 0] = x; o[i * 3 + 1] = y; o[i * 3 + 2] = z;
 }
 
-// mc_av_kernel.cuh (ref_frame 1): warp A runs att_step<true> in blocks of four without the exact path, saving
-// the state before each block; a cold block is redone from the saved state with att_step<false>; after a warm
-// block whose last sample is a multiple of kResync, att_exact and the new 1/cos replace the last step's
-// sin/cos.  Warp V then runs vel_step on the sin/cos before and after every step (the ring).
+// mc_av_kernel.cuh (ref_frame 1): warp A runs att_step<true> in speculative blocks, redone with att_step<false>;
+// after a warm block whose last sample is a multiple of kResync, att_exact and the new 1/cos replace the last
+// step's sin/cos.  Warp V then runs vel_step on the sin/cos before and after every step (the ring).
 extern "C" int step_host_av_blocks(int64_t n, double fs, const double* gyro, const double* accel, const double* ini,
                                    int ini_rows, double* att, double* pos, double* vel) {
   const double dt = 1.0 / fs;
@@ -72,31 +72,28 @@ extern "C" int step_host_av_blocks(int64_t n, double fs, const double* gyro, con
   put_row(pos, 0, v.pos.x, v.pos.y, v.pos.z);
   put_row(vel, 0, v.vel.x, v.vel.y, v.vel.z);
   for (int64_t s = 0; s < n - 1;) {
-    const int len = (s + 4 <= n - 1) ? 4 : 1;
-    SinCos3 ring[4];
-    double ang[4][3];
+    const int len = (s + kSpecBlock <= n - 1) ? kSpecBlock : 1;
+    SinCos3 ring[kSpecBlock];
+    double ang[kSpecBlock][3];
     auto keep = [&](int k) {
       ring[k] = a.sc;
       ang[k][0] = a.yaw; ang[k][1] = a.pitch; ang[k][2] = a.roll;
     };
     auto w_of = [&](int64_t i) { return Vec3{gyro[i * 3], gyro[i * 3 + 1], gyro[i * 3 + 2]}; };
-    if (len == 4) {
-      const AttState saved = a;
-      bool cold = false;
-      for (int k = 0; k < 4; ++k) {
-        cold |= att_step<true>(a, w_of(s + k), dt, false);
+    if (len == kSpecBlock) {
+      AttState saved;
+      const bool redone = spec_block(true, a, saved, [&](int k) {
+        const bool cold = att_step<true>(a, w_of(s + k), dt, false);
         keep(k);
-      }
-      if (cold) {
-        a = saved;
-        for (int k = 0; k < 4; ++k) {
-          att_step(a, w_of(s + k), dt, ((s + k + 1) & (kResync - 1)) == 0);
-          keep(k);
-        }
-      } else if (((s + 4) & (kResync - 1)) == 0) {
+        return cold;
+      }, [&](int k) {
+        att_step(a, w_of(s + k), dt, ((s + k + 1) & (kResync - 1)) == 0);
+        keep(k);
+      });
+      if (!redone && ((s + kSpecBlock) & (kResync - 1)) == 0) {
         att_exact(a);
         a.icp = rcp_nr(a.sc.cp) * dt;
-        keep(3);
+        keep(kSpecBlock - 1);
       }
     } else {
       att_step(a, w_of(s), dt, ((s + 1) & (kResync - 1)) == 0);
@@ -116,9 +113,8 @@ extern "C" int step_host_av_blocks(int64_t n, double fs, const double* gyro, con
   return 0;
 }
 
-// mc_spec_kernel.cuh: nav_step<RF, false, ODO, true> in blocks of four from a saved state, the block redone step
-// by step with the exact path when a step was cold; a block that holds the time-based re-evaluation is not
-// speculated.  (The kernel runs free integration only; the odometer variant shares the step and is checked too.)
+// mc_spec_kernel.cuh: nav_step<RF, false, ODO, true> in speculative blocks, redone step by step with the exact
+// path; a block that holds the time-based re-evaluation is not speculated.  (The kernel runs free integration only; the odometer variant shares the step and is checked too.)
 template <int RF, int ODO>
 static void spec_blocks(int64_t n, double dt, int earth_rot, const double* gyro, const double* accel,
                         const double* ini, int ini_rows, double* att, double* pos, double* vel) {
@@ -129,30 +125,28 @@ static void spec_blocks(int64_t n, double dt, int earth_rot, const double* gyro,
   put_row(pos, 0, st.pos.x, st.pos.y, st.pos.z);
   put_row(vel, 0, st.vel.x, st.vel.y, st.vel.z);
   for (int64_t s = 0; s < n - 1;) {
-    const int len = (s + 4 <= n - 1) ? 4 : 1;
-    NavState after[4];
+    const int len = (s + kSpecBlock <= n - 1) ? kSpecBlock : 1;
+    NavState after[kSpecBlock];
     auto one = [&](int64_t i, bool spec) {
       const Vec3 w{gyro[i * 3], gyro[i * 3 + 1], gyro[i * 3 + 2]};
       const Vec3 f{accel[i * 3], accel[i * 3 + 1], accel[i * 3 + 2]};
       if (spec) return nav_step<RF, false, ODO, true>(st, w, f, dt, earth_rot != 0, 0, false);
       return nav_step<RF, false, ODO>(st, w, f, dt, earth_rot != 0, 0, ((i + 1) & (kResync - 1)) == 0);
     };
-    bool redo = len < 4 || ((s & (kResync - 1)) + 4 >= kResync);
-    if (!redo) {
-      const NavState saved = st;
-      bool cold = false;
-      for (int k = 0; k < 4; ++k) {
-        cold |= one(s + k, true);
+    if (len == kSpecBlock) {
+      NavState saved;
+      const bool speculate = (s & (kResync - 1)) + kSpecBlock < kResync;
+      spec_block(speculate, st, saved, [&](int k) {
+        const bool cold = one(s + k, true);
         after[k] = st;
-      }
-      redo = cold;
-      if (redo) st = saved;
-    }
-    if (redo) {
-      for (int k = 0; k < len; ++k) {
+        return cold;
+      }, [&](int k) {
         one(s + k, false);
         after[k] = st;
-      }
+      });
+    } else {
+      one(s, false);
+      after[0] = st;
     }
     for (int k = 0; k < len; ++k) {
       const NavState& t = after[k];
