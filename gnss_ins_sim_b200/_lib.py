@@ -13,6 +13,7 @@ c_int64_p = ctypes.POINTER(ctypes.c_int64)
 OK, ERR_ARG, ERR_CUDA, ERR_NODEV = 0, 1, 2, 3
 LAYOUT_RUN_MAJOR, LAYOUT_TIME_MAJOR, LAYOUT_CHANNEL_MAJOR = 0, 1, 2
 VIB_NONE, VIB_RANDOM, VIB_SINUSOIDAL, VIB_SERIES = 0, 1, 2, 3
+POS_FRAME_LLA, POS_FRAME_NED, POS_FRAME_ECEF = 0, 1, 2
 
 
 class SensorErr(ctypes.Structure):
@@ -73,6 +74,7 @@ SIGNATURES = {
     'b2ins_imu_noise_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
     'b2ins_gps_noise_f64': (_I, [_L, _L, _P, _P, _P, _I, _U64, _L, _P, _P]),
     'b2ins_mc_free_integration_f64': (_I, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'b2ins_mc_free_integration_ex_f64': (_I, [_MC, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2ins_mc_free_integration_f64_host': (_I, [_MC, _P, _P, _P, _P, _P, _P]),
     'b2ins_mc_plan_create': (_I, [_L, _L, _I, _I, ctypes.POINTER(ctypes.c_void_p)]),
     'b2ins_mc_plan_run': (_I, [_P, _MC, _P, _P, _P, _P, _P, _P]),

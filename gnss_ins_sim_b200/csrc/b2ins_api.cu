@@ -537,14 +537,18 @@ int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n, const double* r
 }
 
 // ---------------------------------------------------------------- K12 -------
-int b2ins_mc_free_integration_f64(const b2ins_mc_config* cfg, const double* ref_gyro,
-                                  const double* ref_accel, const double* ref_nav,
-                                  const double* ini, double* end_err, double* end_state,
-                                  double* proc_stats, double* dump_att, double* dump_pos,
-                                  double* dump_vel, double* dump_gyro, double* dump_accel,
-                                  void* stream) {
+int b2ins_mc_free_integration_ex_f64(const b2ins_mc_config* cfg, int proc_pos_frame, const double* ref_gyro,
+                                     const double* ref_accel, const double* ref_nav,
+                                     const double* ini, double* end_err, double* end_state,
+                                     double* proc_stats, double* dump_att, double* dump_pos,
+                                     double* dump_vel, double* dump_gyro, double* dump_accel,
+                                     void* stream) {
   ARG_CHECK(cfg, "cfg is null");
   ARG_CHECK(cfg->ref_frame == 0 || cfg->ref_frame == 1, "ref_frame must be 0 or 1");
+  ARG_CHECK(proc_pos_frame >= B2INS_POS_FRAME_LLA && proc_pos_frame <= B2INS_POS_FRAME_ECEF,
+            "proc_pos_frame must be B2INS_POS_FRAME_*");
+  ARG_CHECK(proc_pos_frame == B2INS_POS_FRAME_LLA || cfg->ref_frame == 0,
+            "proc_pos_frame NED / ECEF needs ref_frame 0 (LLA positions)");
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0, "runs and n must be non-negative");
   ARG_CHECK(cfg->ini_sets >= 1 && (cfg->ini_rows == 9 || cfg->ini_rows == 10),
@@ -596,6 +600,7 @@ int b2ins_mc_free_integration_f64(const b2ins_mc_config* cfg, const double* ref_
   p.end_state = end_state;
   p.proc_stats = proc_stats;
   p.stats_start = cfg->stats_start;
+  p.proc_pos_frame = proc_pos_frame;
   ARG_CHECK(cfg->algo == 0 || cfg->algo == 1, "algo must be 0 (free integration) or 1 (odometer)");
   p.algo = cfg->algo;
   if (cfg->algo == 1) {
@@ -609,6 +614,17 @@ int b2ins_mc_free_integration_f64(const b2ins_mc_config* cfg, const double* ref_
   const int lanes = cfg->lanes_per_run ? cfg->lanes_per_run : auto_lanes(cfg->runs, cfg->stats_start < 0);
   return launch_mc(p, lanes, cfg->ref_frame, false, cfg->stats_start >= 0,
                    static_cast<cudaStream_t>(stream));
+}
+
+int b2ins_mc_free_integration_f64(const b2ins_mc_config* cfg, const double* ref_gyro,
+                                  const double* ref_accel, const double* ref_nav,
+                                  const double* ini, double* end_err, double* end_state,
+                                  double* proc_stats, double* dump_att, double* dump_pos,
+                                  double* dump_vel, double* dump_gyro, double* dump_accel,
+                                  void* stream) {
+  return b2ins_mc_free_integration_ex_f64(cfg, B2INS_POS_FRAME_LLA, ref_gyro, ref_accel, ref_nav, ini, end_err,
+                                          end_state, proc_stats, dump_att, dump_pos, dump_vel, dump_gyro,
+                                          dump_accel, stream);
 }
 
 int b2ins_mc_free_integration_f64_host(const b2ins_mc_config* cfg, const double* ref_gyro,

@@ -92,6 +92,7 @@ struct McParams {
   int64_t stats_start;
   int debug;           // tools (B2INS_PHASE_CLOCKS builds only): 1 = producers idle, 2 = integrators (A in
                        // mc_av_kernel) idle, 4 = V idle (mc_av_kernel)
+  int proc_pos_frame;  // ref_frame 0 position columns of proc_stats: 0 LLA, 1 NED metres, 2 ECEF metres
 };
 
 // Prepared samples of one block, one slot per lane: phase A stores (gyro xyz, accel xyz),
@@ -370,17 +371,39 @@ __device__ __forceinline__ void put_end(const McParams& p, int64_t run, double y
   }
 }
 
-// process-error accumulation of one sample (ins_data_manager.py:536-541, :761-808)
-__device__ __forceinline__ void proc_accumulate(const NavState& st, const double* r, double* pe_max,
-                                                double* pe_sum, double* pe_sq, double* pe_k,
+// process-error accumulation of one sample (ins_data_manager.py:536-541, :761-808).  In ref_frame 0 a
+// non-zero pos_frame (uniform over the launch) takes the position error in metres, as array_error does
+// for extra_opt 'ned' / 'ecef' (:543-552): d = lla2ecef(x) - lla2ecef(r), and for NED c_ne(r) . d.  Both
+// points are converted from their LLA values, not from the step's carried latitude sin/cos.
+template <int RF>
+__device__ __forceinline__ void proc_accumulate(const NavState& st, const double* r, int pos_frame,
+                                                double* pe_max, double* pe_sum, double* pe_sq, double* pe_k,
                                                 int64_t& pe_cnt) {
   double e[9];
   e[0] = angle_range_pi(st.yaw - r[0]);
   e[1] = angle_range_pi(st.pitch - r[1]);
   e[2] = angle_range_pi(st.roll - r[2]);
-  e[3] = st.pos.x - r[3];
-  e[4] = st.pos.y - r[4];
-  e[5] = st.pos.z - r[5];
+  if (RF == 0 && pos_frame != 0) {
+    const Vec3 x = lla2ecef(st.pos.x, st.pos.y, st.pos.z);
+    const Vec3 xr = lla2ecef(r[3], r[4], r[5]);
+    const Vec3 d{x.x - xr.x, x.y - xr.y, x.z - xr.z};
+    if (pos_frame == 1) {   // attitude.ecef_to_ned(lat, lon) of the truth
+      double sl, cl, so, co;
+      sincos_angle(r[3], &sl, &cl);
+      sincos_angle(r[4], &so, &co);
+      e[3] = -sl * co * d.x - sl * so * d.y + cl * d.z;
+      e[4] = -so * d.x + co * d.y;
+      e[5] = -cl * co * d.x - cl * so * d.y - sl * d.z;
+    } else {
+      e[3] = d.x;
+      e[4] = d.y;
+      e[5] = d.z;
+    }
+  } else {
+    e[3] = st.pos.x - r[3];
+    e[4] = st.pos.y - r[4];
+    e[5] = st.pos.z - r[5];
+  }
   e[6] = st.vel.x - r[6];
   e[7] = st.vel.y - r[7];
   e[8] = st.vel.z - r[8];
@@ -583,7 +606,8 @@ mc_kernel(const __grid_constant__ McParams p) {
         if (PROC) {
           // error of sample t0+base+k (state BEFORE the step), ins_data_manager.py:536-541
           if (t0 + base + k >= p.stats_start)
-            proc_accumulate(st, &sm.nav[s][(base + k) * 9], pe_max, pe_sum, pe_sq, pe_k, pe_cnt);
+            proc_accumulate<RF>(st, &sm.nav[s][(base + k) * 9], p.proc_pos_frame, pe_max, pe_sum, pe_sq,
+                                pe_k, pe_cnt);
         }
         // exact trigonometry again after every kResync-th sample (a rule in absolute time: the same for
         // every lane-group width)
@@ -621,7 +645,8 @@ mc_kernel(const __grid_constant__ McParams p) {
   // ---- per-run results -----------------------------------------------------
   if (PROC) {   // the last sample has no step after it: its error is accumulated here
     if (p.n - 1 >= p.stats_start)
-      proc_accumulate(st, p.ref_nav + (p.n - 1) * 9, pe_max, pe_sum, pe_sq, pe_k, pe_cnt);
+      proc_accumulate<RF>(st, p.ref_nav + (p.n - 1) * 9, p.proc_pos_frame, pe_max, pe_sum, pe_sq, pe_k,
+                          pe_cnt);
   }
   if (mr.active && j == 0) {
     put_end<true, true>(p, mr.run, st.yaw, st.pitch, st.roll, st.pos, st.vel);

@@ -11,6 +11,7 @@ import torch
 
 from . import _lib
 from ._lib import LAYOUT_RUN_MAJOR, LAYOUT_TIME_MAJOR, LAYOUT_CHANNEL_MAJOR  # noqa: F401
+from ._lib import POS_FRAME_LLA, POS_FRAME_NED, POS_FRAME_ECEF  # noqa: F401
 
 
 def _require_cuda():
@@ -147,8 +148,11 @@ class McResult:
 def make_mc_config(ref_frame, fs, n, runs, seed, gyro_err, accel_err, ini_sets, ini_rows,
                    earth_rot=True, run_offset=0, vib_gyro=None, vib_accel=None,
                    lanes_per_run=0, stats_start=-1, dump_runs=0, ini_offset=None,
-                   odo_err=None, ref_odo=None, dump_stride=1):
-    """odo_err {'scale','stdv'} + ref_odo (CUDA f64 [n]) select the odometer variant."""
+                   odo_err=None, ref_odo=None, dump_stride=1, proc_pos_frame=0):
+    """odo_err {'scale','stdv'} + ref_odo (CUDA f64 [n]) select the odometer variant.
+    proc_pos_frame (ref_frame 0): position columns of proc_stats as LLA differences (0), or as
+    NED (1) / ECEF (2) metres, the reference's extra_opt 'ned' / 'ecef'.  It is not a field of
+    b2ins_mc_config: mc_free_integration passes it to b2ins_mc_free_integration_ex_f64."""
     cfg = _lib.McConfig()
     cfg.ref_frame = int(ref_frame)
     cfg.earth_rot = int(bool(earth_rot))
@@ -169,6 +173,7 @@ def make_mc_config(ref_frame, fs, n, runs, seed, gyro_err, accel_err, ini_sets, 
     cfg.stats_start = int(stats_start)
     cfg.dump_runs = int(dump_runs)
     cfg.dump_stride = int(dump_stride)
+    cfg.proc_pos_frame = int(proc_pos_frame)      # a Python attribute beside the struct's fields
     cfg.algo = 0
     if odo_err is not None:
         assert ref_odo is not None and ref_odo.is_cuda and ref_odo.dtype == torch.float64
@@ -213,8 +218,9 @@ def mc_free_integration(cfg, ref_gyro, ref_accel, ref_nav, ini, want_state=False
         res.gyro = res.accel = res.odo = None
     cfg.dump_odo = res.odo.data_ptr() if res.odo is not None else None
     cfg.dump_quat = res.quat.data_ptr() if res.quat is not None else None
-    _lib.check(lib.b2ins_mc_free_integration_f64(
-        ctypes.byref(cfg), _ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ini),
+    _lib.check(lib.b2ins_mc_free_integration_ex_f64(
+        ctypes.byref(cfg), getattr(cfg, 'proc_pos_frame', POS_FRAME_LLA),
+        _ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ini),
         _ptr(res.end_err), _ptr(res.end_state), _ptr(res.proc_stats),
         _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.gyro), _ptr(res.accel), _stream()))
     return res

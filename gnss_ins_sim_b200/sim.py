@@ -106,6 +106,19 @@ def ecef_to_ned(lat, lon):
     return np.array([[-sl * co, -sl * so, cl], [-so, co, 0.0], [-cl * co, -cl * so, -sl]])
 
 
+def lla_error_metres(x, r, frame):
+    """array_error of LLA positions (ins_data_manager.py:543-552), vectorised over samples: x, r [n,3]
+    -> lla2ecef(x) - lla2ecef(r) [n,3] (frame 2, ECEF), rotated by ecef_to_ned of every row of r
+    (frame 1, NED)."""
+    d = lla2ecef(x) - lla2ecef(r)
+    if frame == 1:   # the rows of ecef_to_ned(r[i, 0], r[i, 1]) . d[i]
+        sl, cl, so, co = np.sin(r[:, 0]), np.cos(r[:, 0]), np.sin(r[:, 1]), np.cos(r[:, 1])
+        d = np.stack([-sl * co * d[:, 0] - sl * so * d[:, 1] + cl * d[:, 2],
+                      -so * d[:, 0] + co * d[:, 1],
+                      -cl * co * d[:, 0] - cl * so * d[:, 1] - sl * d[:, 2]], axis=1)
+    return d
+
+
 def euler2quat_zyx(att):
     """attitude.euler2quat 'zyx' (attitude.py:188-205), vectorised over rows: (n,3) -> (n,4)
     scalar-first.  The reference associates att_quat with every att_euler it holds
@@ -949,7 +962,14 @@ class Sim(object):
                 st = {'max': s[0, c0:c0 + 3].copy(), 'avg': s[1, c0:c0 + 3].copy(),
                       'std': s[2, c0:c0 + 3].copy()}
         else:
-            st = self._process_stats(algo_index, err_stats_start, c0)
+            # extra_opt 'ned' / 'ecef' in ref_frame 0: position error in metres (ignored in ref_frame 1, as in
+            # the reference).  The reference keeps the first option's error array per data name
+            # (ins_data_manager.py:427-431); here every call gets the option it asks for.
+            frame = {'ned': engine.POS_FRAME_NED, 'ecef': engine.POS_FRAME_ECEF}.get(extra_opt, 0) \
+                if self.ref_frame == 0 else 0
+            st = self._process_stats(algo_index, err_stats_start, c0, frame)
+            if data_name == 'pos' and frame:
+                units = out_units = ['m'] * 3
         if use_output_units:
             scale = np.array([R2D if (u == 'rad' and o == 'deg') else 1.0
                               for u, o in zip(units, out_units)])
@@ -976,8 +996,13 @@ class Sim(object):
             err = err.dot(ecef_to_ned(r[0], r[1]).T)
         return {'max': np.max(np.abs(err), 0), 'avg': np.average(err, 0), 'std': np.std(err, 0)}
 
-    def _process_stats(self, algo_index, start_s, c0):
-        key = ('proc', algo_index, float(start_s))
+    def _process_stats(self, algo_index, start_s, c0, frame=0):
+        """Per-run process statistics of columns c0:c0+3; frame: the position frame (engine.POS_FRAME_*).
+        One launch holds all nine columns: the attitude and velocity columns of any frame's launch serve."""
+        key = ('proc', algo_index, float(start_s), frame)
+        if c0 != 3:
+            key = next((k for k in (('proc', algo_index, float(start_s), f) for f in (frame, 0, 1, 2))
+                        if k in self._cache), key)
         if key not in self._cache:
             t = self.data['time']
             idx = np.where(t >= start_s)[0]
@@ -995,18 +1020,20 @@ class Sim(object):
                 ps = np.zeros((self.sim_count, 3, 9))
                 for r in range(self.sim_count):
                     k = '%s_%d' % (nm, r)
+                    pos, ref_pos = self.data['pos'][k], self._logged['ref_pos']
                     e = np.concatenate([
                         (self.data['att_euler'][k] - self._logged['ref_att_euler'] + math.pi) % (2.0 * math.pi)
                         - math.pi,
-                        self.data['pos'][k] - self._logged['ref_pos'],
+                        lla_error_metres(pos, ref_pos, frame) if frame else pos - ref_pos,
                         self.data['vel'][k] - self._logged['ref_vel']], axis=1)[start:]
                     ps[r] = np.stack([np.max(np.abs(e), 0), np.average(e, 0), np.std(e, 0)])
                 self._cache[key] = ps
-                return self._process_stats(algo_index, start_s, c0)
+                return self._process_stats(algo_index, start_s, c0, frame)
             d = self._dev
             ps = None
             if hi > lo:
                 cfg = self._mc_config(algo_index, hi - lo, lo, stats_start=start)
+                cfg.proc_pos_frame = frame
                 ps = engine.mc_free_integration(cfg, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
                                                 algo.ini_device()).proc_stats.reshape(hi - lo, 27)
             self._cache[key] = dist.gather_rows(ps, self.sim_count).reshape(-1, 3, 9)

@@ -111,6 +111,11 @@ typedef struct b2ins_mc_config {
                              att_euler it holds (ins_sim.py:729-794, attitude.euler2quat :188-205) */
 } b2ins_mc_config;
 
+/* frame of the position columns of proc_stats, b2ins_mc_free_integration_ex_f64 */
+#define B2INS_POS_FRAME_LLA 0   /* (lat, lon, alt) differences, as b2ins_mc_free_integration_f64 */
+#define B2INS_POS_FRAME_NED 1   /* metres: the reference's get_error_stats(extra_opt='ned') */
+#define B2INS_POS_FRAME_ECEF 2  /* metres: extra_opt='ecef' */
+
 /* ---- K1 + K4 fused: the Allan experiment without the series ------------------------------------
  * Replaces, for a whole Monte-Carlo Allan experiment, pathgen.acc_gen / gyro_gen (pathgen.py:441-594)
  * followed by allan.allan_var (allan.py:18-59) per run and channel (Allan.run, allan_analysis.py:29-49):
@@ -233,7 +238,8 @@ int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n,
  *   end_err [runs][9]: (att wrapped to [-pi,pi], pos, vel) error at sample n-1.
  *   end_state [runs][9] (nullable): att, pos, vel at sample n-1.
  *   proc_stats [runs][3][9] (nullable unless stats_start >= 0): per-run max|e|, mean, std
- *            (ddof 0) of the error over samples >= stats_start.
+ *            (ddof 0) of the error over samples >= stats_start; positions as (lat, lon, alt) differences
+ *            in ref_frame 0 (in metres: b2ins_mc_free_integration_ex_f64).
  *   dump_att/pos/vel, dump_gyro/accel (each nullable): [dump_runs][rows][3] histories, rows = n or
  *            ceil(n / cfg->dump_stride).
  * Asynchronous on `stream`. */
@@ -243,6 +249,19 @@ int b2ins_mc_free_integration_f64(const b2ins_mc_config* cfg,
                                   double* end_err, double* end_state, double* proc_stats,
                                   double* dump_att, double* dump_pos, double* dump_vel,
                                   double* dump_gyro, double* dump_accel, void* stream);
+/* The same with the frame of the position columns of proc_stats (ref_frame 0 only; the attitude and
+ * velocity columns and every other output are those of b2ins_mc_free_integration_f64):
+ *   B2INS_POS_FRAME_LLA   (lat, lon, alt) differences -- b2ins_mc_free_integration_f64;
+ *   B2INS_POS_FRAME_ECEF  metres, lla2ecef(x) - lla2ecef(truth) of every sample;
+ *   B2INS_POS_FRAME_NED   metres, that difference rotated by ecef_to_ned of the true position of the sample
+ * (array_error with extra_opt 'ned' / 'ecef', ins_data_manager.py:543-552).  NED and ECEF need
+ * cfg->ref_frame == 0: ref_frame 1 positions are metres already. */
+int b2ins_mc_free_integration_ex_f64(const b2ins_mc_config* cfg, int proc_pos_frame,
+                                     const double* ref_gyro, const double* ref_accel,
+                                     const double* ref_nav, const double* ini,
+                                     double* end_err, double* end_state, double* proc_stats,
+                                     double* dump_att, double* dump_pos, double* dump_vel,
+                                     double* dump_gyro, double* dump_accel, void* stream);
 /* Host-buffer convenience: copies ref/ini up, runs K12 + K3, copies end_err [runs][9] and
  * stats [3][9] back.  end_err may be NULL (stats only). */
 int b2ins_mc_free_integration_f64_host(const b2ins_mc_config* cfg,
