@@ -73,6 +73,7 @@ SIGNATURES = {
     'b2ins_imu_noise_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P, _P]),
     'b2ins_imu_noise_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
     'b2ins_gps_noise_f64': (_I, [_L, _L, _P, _P, _P, _I, _U64, _L, _P, _P]),
+    'b2ins_mag_noise_f64': (_I, [_L, _L, _P, _P, _P, _P, _U64, _L, _P, _P]),
     'b2ins_mc_free_integration_f64': (_I, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2ins_mc_free_integration_ex_f64': (_I, [_MC, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2ins_mc_free_integration_f64_host': (_I, [_MC, _P, _P, _P, _P, _P, _P]),
@@ -95,6 +96,7 @@ SIGNATURES = {
     'b2ins_psd_series_f64': (_I, [_D, _L, _L, _I, _I, _P, _P, _U64, _L, _P, _P, _P]),
     'b2ins_path_rows': (_L, [_P, _L, _D]),
     'b2ins_path_gen_host': (_L, [_P, _P, _L, _D, _D, _D, _D, _P, _I, _L, _P, _P, _P, c_int64_p, _P]),
+    'b2ins_path_gen_ex_host': (_L, [_P, _P, _L, _D, _D, _D, _D, _P, _I, _L, _P, _P, _P, c_int64_p, _P, _P, _P]),
     'b2ins_ins_loose_f64': (_I, [ctypes.POINTER(EkfConfig)] + [_P] * 15),
     'b2ins_diag_dfma_rate': (_I, [c_double_p]),
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),

@@ -15,6 +15,7 @@
 #include "pathgen_host.h"
 #include "psd_kernel.cuh"
 #include "gps_kernel.cuh"
+#include "mag_kernel.cuh"
 #include "ekf_kernel.cuh"
 #include "stats_kernel.cuh"
 
@@ -498,6 +499,38 @@ int b2ins_gps_noise_f64(int64_t runs, int64_t m, const double* ref_gps, const do
   const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
   if (blocks > cap) blocks = cap;
   gps_noise_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+int b2ins_mag_noise_f64(int64_t runs, int64_t n, const double* ref_mag, const double* si,
+                        const double* hi, const double* std, uint64_t seed, int64_t run_offset,
+                        double* mag, void* stream) {
+  ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
+  ARG_CHECK(si && hi && std, "null error model");
+  for (int i = 0; i < 3; ++i)
+    ARG_CHECK(std::isfinite(std[i]) && std[i] >= 0.0, "mag std must be finite and >= 0");
+  if (runs == 0 || n == 0) return B2INS_OK;
+  ARG_CHECK(ref_mag && mag, "null buffer");
+  ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
+  MagParams p;
+  p.n = n;
+  p.runs = runs;
+  p.run_offset = run_offset;
+  p.ref = ref_mag;
+  p.out = mag;
+  for (int i = 0; i < 9; ++i) p.si[i] = si[i];
+  for (int i = 0; i < 3; ++i) {
+    p.hi[i] = hi[i];
+    p.std[i] = std[i];
+  }
+  p.k0 = static_cast<uint32_t>(seed);
+  p.k1 = static_cast<uint32_t>(seed >> 32);
+  const int64_t total = runs * n;
+  int64_t blocks = (total + 255) / 256;
+  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
+  if (blocks > cap) blocks = cap;
+  mag_noise_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
@@ -1118,17 +1151,25 @@ int64_t b2ins_path_rows(const double* motion_def, int64_t segs, double fs) {
   return b2ins_host::path_rows(motion_def, segs, fs);
 }
 
-int64_t b2ins_path_gen_host(const double* ini, const double* motion_def, int64_t segs, double fs,
-                            double osr, double fs_gps, double fs_odo, const double* mobility,
-                            int ref_frame, int64_t cap, double* imu, double* nav, double* gps,
-                            int64_t* gps_rows, double* odo) {
+int64_t b2ins_path_gen_ex_host(const double* ini, const double* motion_def, int64_t segs, double fs,
+                               double osr, double fs_gps, double fs_odo, const double* mobility,
+                               int ref_frame, int64_t cap, double* imu, double* nav, double* gps,
+                               int64_t* gps_rows, double* odo, const double* geomag_n, double* mag) {
   if (!ini || !motion_def || !mobility || !imu || !nav || segs <= 0 || !(fs > 0.0) || !(osr >= 1.0) ||
-      (ref_frame != 0 && ref_frame != 1) || (gps && !(fs_gps > 0.0))) {
+      (ref_frame != 0 && ref_frame != 1) || (gps && !(fs_gps > 0.0)) || (geomag_n && !mag)) {
     fail(B2INS_ERR_ARG, "bad argument to b2ins_path_gen_host");
     return -1;
   }
   return b2ins_host::path_gen(ini, motion_def, segs, fs, osr, fs_gps, fs_odo, mobility, ref_frame,
-                              cap, imu, nav, gps, gps_rows, odo);
+                              cap, imu, nav, gps, gps_rows, odo, geomag_n, geomag_n ? mag : nullptr);
+}
+
+int64_t b2ins_path_gen_host(const double* ini, const double* motion_def, int64_t segs, double fs,
+                            double osr, double fs_gps, double fs_odo, const double* mobility,
+                            int ref_frame, int64_t cap, double* imu, double* nav, double* gps,
+                            int64_t* gps_rows, double* odo) {
+  return b2ins_path_gen_ex_host(ini, motion_def, segs, fs, osr, fs_gps, fs_odo, mobility, ref_frame,
+                                cap, imu, nav, gps, gps_rows, odo, nullptr, nullptr);
 }
 
 // ---------------------------------------------------------------- diag ------

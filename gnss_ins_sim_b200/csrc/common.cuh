@@ -34,6 +34,7 @@ constexpr uint32_t kDrawGyro = 3;   // +axis: (GM drive, white)
 constexpr uint32_t kDrawVib = 6;    // +axis: (accel random vib, gyro random vib)
 constexpr uint32_t kDrawPhase = 9;  // +axis, t = 0xFFFFFFFF: sinusoidal gyro-vib phase
 constexpr uint32_t kDrawOdo = 12;   // odometer white noise (z0)
+constexpr uint32_t kDrawMag = 13;   // magnetometer: 13 (x, y), 14 (z from z0)
 constexpr uint32_t kDrawPsd = 16;   // +3*sensor+axis, t = bin index: PSD random phases
 
 struct PhiloxOut {

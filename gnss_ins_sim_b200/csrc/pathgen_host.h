@@ -6,7 +6,8 @@
 // experiment and its result is shared by every Monte-Carlo run.  The reference spends ~40 us
 // per sample in Python on it (8.6 s for BASELINE config 3, ~10 min for config 4); this
 // restatement takes ~0.1 us per sample and removes the last runtime dependency on the
-// reference package.  Magnetometer output (geomag / WMM) is not generated.
+// reference package.  The geomagnetic field itself (WMM at the initial position) is an input:
+// gnss_ins_sim_b200/geomag.py evaluates it once on the host.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -159,11 +160,14 @@ inline int64_t path_rows(const double* motion_def, int64_t segs, double fs) {
 
 // pathgen.path_gen.  motion_def [segs][9] (angles already in rad, NaN already 0, durations in
 // seconds; NOT modified).  imu [cap][7], nav [cap][10], gps [cap][8] / odo [cap][5] (nullable).
+// geomag_n [3]: geomagnetic field in the navigation frame [uT] (null: no magnetometer); mag [cap][4]
+// gets (index, c_nb^T geomag_n) on every imu/nav row (pathgen.py:272-279).
 // Returns the number of imu/nav rows (<= cap), or a negative error; *gps_rows gets the gps count.
 inline int64_t path_gen(const double* ini, const double* motion_def, int64_t segs, double fs,
                         double osr, double fs_gps, double fs_odo, const double* mobility,
                         int ref_frame, int64_t cap, double* imu, double* nav, double* gps,
-                        int64_t* gps_rows, double* odo) {
+                        int64_t* gps_rows, double* odo, const double* geomag_n = nullptr,
+                        double* mag = nullptr) {
   const double sim_freq = osr * fs;
   const double dt = 1.0 / sim_freq;
   const double alpha = 0.9, fa = alpha, fb = 1 - alpha;
@@ -175,6 +179,7 @@ inline int64_t path_gen(const double* ini, const double* motion_def, int64_t seg
   if (rows == 0) return -3;
   if (rows > cap) return -4;
   const bool want_gps = gps != nullptr, want_odo = odo != nullptr;
+  const bool want_mag = geomag_n != nullptr && mag != nullptr;
   const double gps_period = want_gps ? osr * std::nearbyint(fs / fs_gps) : 0.0;
   (void)fs_odo;  // the reference computes an odometer period but writes odo at the IMU rate
 
@@ -256,6 +261,16 @@ inline int64_t path_gen(const double* ini, const double* motion_def, int64_t seg
           v[4 + k] = vel_n[k];
         }
         euler_range(att, v + 7);
+        if (want_mag) {
+          // c_nb^T geomag_n with the c_nb of this row's attitude.  The reference's c_nb.T.dot(geo_mag_n)
+          // is NumPy's BLAS dgemv on a C-contiguous 3x3 matrix; OpenBLAS's x86-64 kernel rounds each row
+          // as fma(a2, x2, fma(a0, x0, a1 x1)), and the same rounding here gives the same bits.
+          double* b = mag + hi * 4;
+          b[0] = sim_count;
+          for (int k = 0; k < 3; ++k)
+            b[1 + k] = std::fma(c_nb[2][k], geomag_n[2],
+                                std::fma(c_nb[0][k], geomag_n[0], c_nb[1][k] * geomag_n[1]));
+        }
         if (want_odo) {
           double* o = odo + hi * 5;
           o[0] = sim_count;

@@ -131,6 +131,21 @@ def gps_noise(runs, ref_gps, gps_err, gps_type, seed, run_offset=0):
     return out
 
 
+def mag_noise(runs, ref_mag, mag_err, seed, run_offset=0):
+    """K8: pathgen.mag_gen for `runs` runs.  ref_mag: CUDA f64 [n,3] (uT, body frame); mag_err
+    {'si' [3,3], 'hi' [3], 'std' [3]} (uT).  Returns [R,n,3]."""
+    _require_cuda()
+    lib = _lib.load()
+    n = ref_mag.shape[0]
+    out = torch.empty((runs, n, 3), dtype=torch.float64, device=ref_mag.device)
+    si = np.ascontiguousarray(np.asarray(mag_err['si'], dtype=np.float64).reshape(3, 3))
+    hi = np.ascontiguousarray(np.broadcast_to(np.asarray(mag_err['hi'], dtype=np.float64).reshape(-1), (3,)))
+    std = np.ascontiguousarray(np.broadcast_to(np.asarray(mag_err['std'], dtype=np.float64).reshape(-1), (3,)))
+    _lib.check(lib.b2ins_mag_noise_f64(runs, n, _ptr(ref_mag), _lib.host_ptr(si), _lib.host_ptr(hi),
+                                       _lib.host_ptr(std), int(seed), int(run_offset), _ptr(out), _stream()))
+    return out
+
+
 class McResult:
     """Device-side results of one fused Monte-Carlo launch."""
 

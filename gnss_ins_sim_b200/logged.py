@@ -153,11 +153,13 @@ OUTPUT_FORMAT = {
     'ref_gps': (['ref_gps_lat', 'ref_gps_lon', 'ref_gps_alt', 'ref_gps_vN', 'ref_gps_vE', 'ref_gps_vD'],
                 ['rad', 'rad', 'm', 'm/s', 'm/s', 'm/s'], ['deg', 'deg', 'm', 'm/s', 'm/s', 'm/s']),
     'ref_odo': (['ref_odo'], ['m/s'], ['m/s']),
+    'ref_mag': (['ref_mag_x', 'ref_mag_y', 'ref_mag_z'], ['uT'] * 3, ['uT'] * 3),
     'gyro': (['gyro_x', 'gyro_y', 'gyro_z'], ['rad/s'] * 3, ['deg/s'] * 3),
     'accel': (['accel_x', 'accel_y', 'accel_z'], ['m/s^2'] * 3, ['m/s^2'] * 3),
     'gps': (['gps_lat', 'gps_lon', 'gps_alt', 'gps_vN', 'gps_vE', 'gps_vD'],
             ['rad', 'rad', 'm', 'm/s', 'm/s', 'm/s'], ['deg', 'deg', 'm', 'm/s', 'm/s', 'm/s']),
     'odo': (['odo'], ['m/s'], ['m/s']),
+    'mag': (['mag_x', 'mag_y', 'mag_z'], ['uT'] * 3, ['uT'] * 3),
     'algo_time': (['algo_time'], ['sec'], ['sec']),
     'pos': (['pos_lat', 'pos_lon', 'pos_alt'], ['rad', 'rad', 'm'], ['deg', 'deg', 'm']),
     'vel': (['vel_x', 'vel_y', 'vel_z'], ['m/s'] * 3, ['m/s'] * 3),

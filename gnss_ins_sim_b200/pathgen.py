@@ -1,7 +1,7 @@
 """True-trajectory generation on the host -- the interface of gnss_ins_sim.pathgen.pathgen
 (`path_gen`, pathgen.py:26-329; `parse motion definition` as Sim.__parse_motion does,
 ins_sim.py:578-640), computed by the C++ restatement in csrc/pathgen_host.h through the C ABI
-(b2ins_path_gen_host).  CPU only: this is the one stage the north star keeps off the GPU."""
+(b2ins_path_gen_ex_host).  CPU only: this is the one stage the north star keeps off the GPU."""
 import ctypes
 import math
 import os
@@ -9,20 +9,22 @@ from io import StringIO
 
 import numpy as np
 
-from . import _lib
+from . import _lib, geomag
 
 D2R = math.pi / 180
 HIGH_MOBILITY = np.array([1.0, 0.5, 2.0])   # m/s^2, rad/s^2, rad/s (ins_sim.py:25)
 
 
-def path_gen(ini_pos_vel_att, motion_def, output_def, mobility, ref_frame=0, magnet=False):
+def path_gen(ini_pos_vel_att, motion_def, output_def, mobility, ref_frame=0, magnet=False,
+             wmm_file=None, wmm_date=None):
     """pathgen.path_gen: same arguments and the same result dictionary
-    ('status', 'imu' (n,7), 'nav' (n,10), 'gps' (m,8), 'odo' (n,5), 'mag' []).
-    Unlike the reference it does not modify motion_def / output_def in place."""
-    if magnet:
-        raise NotImplementedError('magnetometer output (geomag / WMM) is not generated here')
+    ('status', 'imu' (n,7), 'nav' (n,10), 'gps' (m,8), 'odo' (n,5), 'mag' (n,4) or []).
+    Unlike the reference it does not modify motion_def / output_def in place.
+    magnet: the field is the World Magnetic Model at the initial position (geomag.field_ned) from
+    wmm_file (default: the installed gnss_ins_sim's WMM.COF) on wmm_date (default: today)."""
     lib = _lib.load()
     ini = np.ascontiguousarray(ini_pos_vel_att, dtype=np.float64).reshape(-1)[:9].copy()
+    geo_mag_n = np.array(geomag.field_ned(ini, ref_frame, wmm_file, wmm_date)) if magnet else None
     md = np.ascontiguousarray(motion_def, dtype=np.float64)
     if md.ndim != 2 or md.shape[1] < 9:
         raise ValueError('motion_def must be (segments, 9)')
@@ -43,15 +45,16 @@ def path_gen(ini_pos_vel_att, motion_def, output_def, mobility, ref_frame=0, mag
     nav = np.zeros((rows, 10))
     gps = np.zeros((rows, 8)) if want_gps else None
     odo = np.zeros((rows, 5)) if want_odo else None
+    mag = np.zeros((rows, 4)) if magnet else None
     n_gps = ctypes.c_int64(0)
-    n = lib.b2ins_path_gen_host(_lib.host_ptr(ini), _lib.host_ptr(md), md.shape[0], fs, osr,
-                                float(od[1, 1]) if want_gps else 0.0, float(od[2, 1]) if want_odo else 0.0,
-                                _lib.host_ptr(mob), int(ref_frame), rows, _lib.host_ptr(imu),
-                                _lib.host_ptr(nav), _lib.host_ptr(gps), ctypes.byref(n_gps),
-                                _lib.host_ptr(odo))
+    n = lib.b2ins_path_gen_ex_host(_lib.host_ptr(ini), _lib.host_ptr(md), md.shape[0], fs, osr,
+                                   float(od[1, 1]) if want_gps else 0.0, float(od[2, 1]) if want_odo else 0.0,
+                                   _lib.host_ptr(mob), int(ref_frame), rows, _lib.host_ptr(imu),
+                                   _lib.host_ptr(nav), _lib.host_ptr(gps), ctypes.byref(n_gps),
+                                   _lib.host_ptr(odo), _lib.host_ptr(geo_mag_n), _lib.host_ptr(mag))
     if n < 0:
         raise ValueError('path_gen failed (%d): %s' % (n, lib.b2ins_last_error().decode()))
-    return {'status': True, 'imu': imu[:n], 'nav': nav[:n], 'mag': [],
+    return {'status': True, 'imu': imu[:n], 'nav': nav[:n], 'mag': mag[:n] if magnet else [],
             'gps': gps[:n_gps.value] if want_gps else [], 'odo': odo[:n] if want_odo else []}
 
 

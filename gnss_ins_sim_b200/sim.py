@@ -18,8 +18,9 @@ Dispatch on `algorithm`:
     lazily: counter-based Philox makes any run reproducible in isolation, so
     get_data(['pos'])[0]['algo0_7'] re-runs just run 7 with history output on.
   * gnss_ins_sim_b200 Allan            -> K1 (noise) + K4 (Allan variance) per run block.
-  * any other reference-style plugin   -> K1 generates gyro/accel on the device, the
-    plugin's own .run() is called per run on the host (compatibility path).
+  * any other reference-style plugin   -> K1 generates gyro/accel (K8 the magnetometer of a
+    9-axis IMU) on the device, the plugin's own .run() is called per run on the host
+    (compatibility path).
   * None                               -> sensor data only.
 Multi-GPU: runs are sharded by rank when torch.distributed is initialised (dist.py).
 """
@@ -168,6 +169,10 @@ def load_trajectory(src):
             raise ValueError('trajectory %s must be (n,3)' % k)
     if 'ref_odo' in src:
         out['ref_odo'] = np.ascontiguousarray(src['ref_odo'], dtype=np.float64).reshape(-1)
+    if 'ref_mag' in src:
+        out['ref_mag'] = np.ascontiguousarray(src['ref_mag'], dtype=np.float64)
+        if out['ref_mag'].shape != (n, 3):
+            raise ValueError('trajectory ref_mag must be (n,3)')
     if 'time' in src:
         out['time'] = np.asarray(src['time'], dtype=np.float64)
     if 'ini' in src:
@@ -179,7 +184,7 @@ def load_trajectory(src):
 
 
 def trajectory_from_motion_def(fs, motion_def, ref_frame, mode=None, magnetometer=False, odo=False,
-                               gps=False, fs_gps=0.0):
+                               gps=False, fs_gps=0.0, wmm_file=None, wmm_date=None):
     """Motion-definition csv/string -> trajectory dict, driven exactly as
     Sim.__gen_data_from_pathgen does (ins_sim.py:444-472): parse (ins_sim.py:578-640), then
     path_gen -- here the host-side restatement in csrc/pathgen_host.h (pathgen.py), ~200x faster
@@ -189,7 +194,7 @@ def trajectory_from_motion_def(fs, motion_def, ref_frame, mode=None, magnetomete
     mobility = pathgen.parse_mode(mode)
     output_def = np.array([[1.0, fs], [1.0 if gps else -1.0, fs_gps if gps else fs],
                            [1.0 if odo else -1.0, fs]])
-    rtn = pathgen.path_gen(ini_pva, cmd, output_def, mobility, ref_frame, magnetometer)
+    rtn = pathgen.path_gen(ini_pva, cmd, output_def, mobility, ref_frame, magnetometer, wmm_file, wmm_date)
     out = {'time': rtn['nav'][:, 0] / fs, 'ref_pos': np.ascontiguousarray(rtn['nav'][:, 1:4]),
            'ref_vel': np.ascontiguousarray(rtn['nav'][:, 4:7]),
            'ref_att': np.ascontiguousarray(rtn['nav'][:, 7:10]),
@@ -197,6 +202,8 @@ def trajectory_from_motion_def(fs, motion_def, ref_frame, mode=None, magnetomete
            'ref_gyro': np.ascontiguousarray(rtn['imu'][:, 4:7]), 'ini': ini_pva}
     if odo:
         out['ref_odo'] = np.ascontiguousarray(rtn['odo'][:, 2])
+    if magnetometer:
+        out['ref_mag'] = np.ascontiguousarray(rtn['mag'][:, 1:4])
     if gps:
         out['gps_time'] = rtn['gps'][:, 0] / fs
         out['ref_gps'] = np.ascontiguousarray(rtn['gps'][:, 1:7])
@@ -306,7 +313,8 @@ class Sim(object):
     '''
 
     def __init__(self, fs, motion_def, ref_frame=0, imu=None, mode=None, env=None,
-                 algorithm=None, seed=0, lanes_per_run=0, history_block=32, run_base=0):
+                 algorithm=None, seed=0, lanes_per_run=0, history_block=32, run_base=0,
+                 wmm_file=None, wmm_date=None):
         '''
         Args: as gnss_ins_sim.sim.ins_sim.Sim (ins_sim.py:31-124), plus
             seed: Philox key of the experiment (the reference is unseeded; here every
@@ -315,6 +323,9 @@ class Sim(object):
             history_block: runs materialised together on a lazy history access.
             run_base: Philox stream id of run 0 (run r draws stream run_base + r), so that
                 separate experiments can extend one ensemble without reusing streams.
+            wmm_file: World Magnetic Model coefficients (NOAA .COF) for a 9-axis IMU on a motion
+                definition; default: geoparams/WMM.COF of an installed gnss_ins_sim package.
+            wmm_date: datetime.date the field is evaluated at (default: today, as the reference).
         '''
         self.fs = list(fs) if isinstance(fs, (list, tuple, np.ndarray)) else [float(fs), 0.0, 0.0]
         self.imu = imu
@@ -325,6 +336,7 @@ class Sim(object):
         self.lanes_per_run = int(lanes_per_run)
         self.history_block = int(history_block)
         self.run_base = int(run_base)
+        self.wmm_file, self.wmm_date = wmm_file, wmm_date
         self.data_src = motion_def
         self.sim_count = 1
         self.sim_complete = False
@@ -367,7 +379,7 @@ class Sim(object):
                                               bool(self.imu and self.imu.magnetometer),
                                               bool(self.imu and self.imu.odo),
                                               bool(self.imu and self.imu.gps) and self.fs[1] > 0,
-                                              self.fs[1])
+                                              self.fs[1], self.wmm_file, self.wmm_date)
         else:
             raise TypeError('motion_def must be a trajectory dict, an .npz path or a motion '
                             'definition csv/string')
@@ -380,13 +392,14 @@ class Sim(object):
         d['ref_pos'], d['ref_vel'], d['ref_att_euler'] = traj['ref_pos'], traj['ref_vel'], traj['ref_att']
         d['ref_accel'], d['ref_gyro'] = traj['ref_accel'], traj['ref_gyro']
         d.defer('ref_att_quat', lambda: euler2quat_zyx(traj['ref_att']))   # built when first read
-        for k in ('ref_odo', 'gps_time', 'ref_gps', 'gps_visibility'):
+        for k in ('ref_odo', 'gps_time', 'ref_gps', 'gps_visibility', 'ref_mag'):
             if k in traj:
                 d[k] = traj[k]
         self._nav_end = np.concatenate([traj['ref_att'][-1], traj['ref_pos'][-1], traj['ref_vel'][-1]])
         self._nav_cache = None
         self._dev_cache = None
         self._ref_gps_dev = None
+        self._ref_mag_dev = None
 
     @property
     def _nav(self):
@@ -428,6 +441,8 @@ class Sim(object):
         self._vib_gyro = parse_env(self.env['gyro'], self.fs[0]) if self.env and 'gyro' in self.env else None
         self._psd_cache = {}
         R = self.sim_count
+        if getattr(self.imu, 'magnetometer', False) and 'ref_mag' not in self._traj:
+            raise ValueError('imu has a magnetometer (axis=9) but the trajectory has no ref_mag')
         self._shard = dist.shard(R)
         self.data['accel'] = LazyRuns(self, 'accel', R)
         self.data['gyro'] = LazyRuns(self, 'gyro', R)
@@ -437,6 +452,8 @@ class Sim(object):
             self.data['odo'] = LazyRuns(self, 'odo', R)
         if getattr(self.imu, 'gps', False) and 'ref_gps' in self._traj:
             self.data['gps'] = LazyRuns(self, 'gps', R)     # pathgen.gps_gen per run (ins_sim.py:497-500)
+        if getattr(self.imu, 'magnetometer', False):
+            self.data['mag'] = LazyRuns(self, 'mag', R)     # pathgen.mag_gen per run (ins_sim.py:501-503)
         if self.algo is not None:
             for i, a in enumerate(self.algo):
                 if isinstance(a, FreeIntegration):     # incl. the odometer variant
@@ -783,6 +800,8 @@ class Sim(object):
         for r in range(self.sim_count):
             gyro, accel = self._noise_block(r, r + 1)
             per_run = {'gyro': gyro[0].cpu().numpy(), 'accel': accel[0].cpu().numpy()}
+            if 'mag' in algo.input and 'mag' in self.data:
+                per_run['mag'] = self.data['mag'][r]     # the block get_data(['mag']) serves
             args = []
             for nm in algo.input:
                 if nm in per_run:
@@ -851,6 +870,11 @@ class Sim(object):
                     self._ref_gps_dev = engine.to_device(self._traj['ref_gps'])
                 hist['gps'] = engine.gps_noise(r1 - r0, self._ref_gps_dev, self.imu.gps_err, self.ref_frame,
                                                self.seed, run_offset=self.run_base + r0).cpu().numpy()
+            elif name == 'mag':
+                if getattr(self, '_ref_mag_dev', None) is None:
+                    self._ref_mag_dev = engine.to_device(self._traj['ref_mag'])
+                hist['mag'] = engine.mag_noise(r1 - r0, self._ref_mag_dev, self.imu.mag_err, self.seed,
+                                               run_offset=self.run_base + r0).cpu().numpy()
             else:
                 gyro, accel = self._noise_block(r0, r1)
                 hist.update({'gyro': gyro.cpu().numpy(), 'accel': accel.cpu().numpy()})

@@ -364,6 +364,18 @@ int b2ins_gps_noise_f64(int64_t runs, int64_t m, const double* ref_gps, const do
                         const double* stdv, int gps_type, uint64_t seed, int64_t run_offset,
                         double* gps, void* stream);
 
+/* ---- K8: magnetometer measurement generator ------------------------------------------
+ * Replaces pathgen.mag_gen (gnss_ins_sim/pathgen/pathgen.py:643-661) and its call in loop A
+ * (gnss_ins_sim/sim/ins_sim.py:501-503) for `runs` runs at once, at the IMU rate:
+ *   mag[r][k] = si (ref_mag[k] + hi) + std * N(0,1),
+ * Philox draws (k, 13, run_offset + r) -> (x, y) and z0 of (k, 14, run_offset + r) -> z.
+ * ref_mag [n][3] (device): true field in the body frame [uT], path_gen's 'mag' columns 1..3.
+ * si: host [9], soft-iron matrix, row-major; hi, std: host [3], hard iron and noise sigma [uT]
+ * (std finite and >= 0).  mag [runs][n][3] (device), run-major. */
+int b2ins_mag_noise_f64(int64_t runs, int64_t n, const double* ref_mag, const double* si,
+                        const double* hi, const double* std, uint64_t seed, int64_t run_offset,
+                        double* mag, void* stream);
+
 /* ---- host: true-trajectory generator -----------------------------------------------
  * Replaces pathgen.path_gen (gnss_ins_sim/pathgen/pathgen.py:26-329, with
  * calc_true_sensor_output :331-411 and parse_motion_def :413-439).  Plain CPU code (the
@@ -377,12 +389,20 @@ int b2ins_gps_noise_f64(int64_t runs, int64_t m, const double* ref_gps, const do
  *   imu [cap][7] (index, accel xyz, gyro xyz), nav [cap][10] (index, pos, vel NED, yaw pitch roll),
  *   gps [cap][8] (nullable), odo [cap][5] (nullable).  cap >= b2ins_path_rows(...).
  * Returns the number of imu/nav rows written, or < 0: -2 negative duration, -3 empty, -4 cap too
- * small, -5 unknown command type.  Magnetometer output is not generated. */
+ * small, -5 unknown command type.  b2ins_path_gen_host generates no magnetometer output; it is
+ * b2ins_path_gen_ex_host with a null geomag_n.
+ * b2ins_path_gen_ex_host: geomag_n [3] (nullable) is the geomagnetic field in the navigation frame
+ *   [uT] (WMM at the initial position, pathgen.py:164-171; gnss_ins_sim_b200/geomag.py evaluates
+ *   it); with it, mag [cap][4] gets (index, c_nb^T geomag_n) on every imu/nav row. */
 int64_t b2ins_path_rows(const double* motion_def, int64_t segs, double fs);
 int64_t b2ins_path_gen_host(const double* ini, const double* motion_def, int64_t segs, double fs,
                             double osr, double fs_gps, double fs_odo, const double* mobility,
                             int ref_frame, int64_t cap, double* imu, double* nav, double* gps,
                             int64_t* gps_rows, double* odo);
+int64_t b2ins_path_gen_ex_host(const double* ini, const double* motion_def, int64_t segs, double fs,
+                               double osr, double fs_gps, double fs_odo, const double* mobility,
+                               int ref_frame, int64_t cap, double* imu, double* nav, double* gps,
+                               int64_t* gps_rows, double* odo, const double* geomag_n, double* mag);
 
 /* ---- diagnostics ---------------------------------------------------------
  * Measured FP64 FMA issue rate of the current device [lane-FMA/s]: a ~10 ms dependent-chain

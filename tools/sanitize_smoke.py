@@ -74,6 +74,8 @@ def main():
     assert torch.isfinite(res.end_err).all() and torch.isfinite(res.consist).all()
     ref_gps = engine.to_device(np.tile(np.array([0.5, 2.0, 10.0, 1.0, 0.0, 0.0]), (50, 1)))
     engine.gps_noise(7, ref_gps, {'stdp': np.ones(3), 'stdv': np.ones(3)}, 0, 3)
+    ref_mag = engine.to_device(np.tile(np.array([20.0, -3.0, 40.0]), (51, 1)))
+    engine.mag_noise(9, ref_mag, {'si': np.eye(3), 'hi': np.ones(3), 'std': np.full(3, 0.5)}, 5, 3)
     torch.cuda.synchronize()
     print('sanitize smoke ok')
 
