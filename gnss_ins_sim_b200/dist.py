@@ -1,12 +1,12 @@
 """Multi-GPU plumbing: Monte-Carlo runs shard embarrassingly across ranks (one process
 per GPU, torch.distributed); the only data-path collectives are one broadcast of the
-CPU-generated trajectory and the all-reduces of the final error statistics
+CPU-generated trajectory and the exchange of the final error statistics
 (SURVEY 8e).  Works un-initialised (single process) and with the gloo backend (CPU
 tests of the host logic); on GPUs the backend is NCCL over NVLink.
 
-Statistics are combined exactly like np.std's two passes:
-  phase 1  all-reduce SUM(sum e, count), MAX(max|e|)  -> mean
-  phase 2  all-reduce SUM(sum (e-mean)^2)             -> std (ddof 0)
+Statistics are combined from each rank's (count, max|e|, mean, std) by Chan's pairwise update
+(merge_stats), as robust as np.std's two passes: inside K3x through NVLink peer memory
+(P2PStats), or after ONE all_gather (StatsMerger, combine_local_stats).
 """
 import numpy as np
 import torch
@@ -53,24 +53,6 @@ def all_reduce(t, op):
     if buf is not t:
         t.copy_(buf)
     return t
-
-
-def combine_phase1(partial, local_runs, ncomp):
-    """partial [2*ncomp] = (sum e, max|e|) of this rank (zeros if it owns no runs).
-    Returns (mean [ncomp], max [ncomp], total_runs) after the all-reduces."""
-    sums = torch.cat([partial[:ncomp], partial.new_tensor([float(local_runs)])])
-    mx = partial[ncomp:2 * ncomp].clone()
-    all_reduce(sums, td.ReduceOp.SUM)
-    all_reduce(mx, td.ReduceOp.MAX)
-    total = float(sums[ncomp].item())
-    return sums[:ncomp] / total, mx, int(round(total))
-
-
-def combine_phase2(partial2, total_runs):
-    """partial2 [ncomp] = sum (e - mean)^2 of this rank -> std [ncomp]."""
-    p = partial2.clone()
-    all_reduce(p, td.ReduceOp.SUM)
-    return torch.sqrt(p / float(total_runs))
 
 
 def merge_stats(blocks):
@@ -215,28 +197,6 @@ class P2PStats:
 
     def reset_timeout(self):
         self.flag.zero_()
-
-
-def ensemble_stats(end_err, total_runs):
-    """[3, ncomp] numpy = max|e|, mean, std over ALL ranks' runs.
-    end_err: this rank's CUDA [R_local, ncomp] (or None if it owns no runs)."""
-    from . import engine
-    ncomp = 9 if end_err is None else end_err.shape[1]
-    dev = end_err.device if end_err is not None else _comm_device()
-    if end_err is not None and end_err.shape[0] > 0:
-        partial = engine.error_partial(end_err)
-        local = end_err.shape[0]
-    else:
-        partial = torch.zeros(2 * ncomp, dtype=torch.float64, device=dev)
-        local = 0
-    mean, mx, total = combine_phase1(partial, local, ncomp)
-    assert total == total_runs, (total, total_runs)
-    if local:
-        partial2 = engine.error_partial2(end_err, mean)
-    else:
-        partial2 = torch.zeros(ncomp, dtype=torch.float64, device=dev)
-    std = combine_phase2(partial2, total)
-    return torch.stack([mx, mean, std]).cpu().numpy()
 
 
 def gather_rows(local, total_runs):

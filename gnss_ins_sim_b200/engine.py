@@ -30,6 +30,13 @@ def _ptr(t):
     return ctypes.c_void_p(t.data_ptr())
 
 
+def _reuse(cur, shape, dev):
+    """cur if it is a buffer of this shape (results handed back through `out=`), else a new f64 one on dev."""
+    if cur is not None and tuple(cur.shape) == tuple(shape):
+        return cur
+    return torch.empty(shape, dtype=torch.float64, device=dev)
+
+
 def to_device(a, device=None):
     """numpy / tensor -> contiguous float64 CUDA tensor (H2D copy if needed)."""
     if isinstance(a, torch.Tensor):
@@ -211,24 +218,18 @@ def mc_free_integration(cfg, ref_gyro, ref_accel, ref_nav, ini, want_state=False
     R, n, D = cfg.runs, cfg.n, cfg.dump_runs
     rows = -(-n // max(1, cfg.dump_stride))          # histories keep every dump_stride-th sample
     res = out or McResult()
-
-    def buf(cur, shape):
-        if cur is not None and tuple(cur.shape) == tuple(shape):
-            return cur
-        return torch.empty(shape, dtype=torch.float64, device=dev)
-
-    res.end_err = buf(res.end_err, (R, 9))
-    res.end_state = buf(res.end_state, (R, 9)) if want_state else None
-    res.proc_stats = buf(res.proc_stats, (R, 3, 9)) if cfg.stats_start >= 0 else None
+    res.end_err = _reuse(res.end_err, (R, 9), dev)
+    res.end_state = _reuse(res.end_state, (R, 9), dev) if want_state else None
+    res.proc_stats = _reuse(res.proc_stats, (R, 3, 9), dev) if cfg.stats_start >= 0 else None
     if dump_nav and D > 0:
-        res.att, res.pos, res.vel = (buf(res.att, (D, rows, 3)), buf(res.pos, (D, rows, 3)),
-                                     buf(res.vel, (D, rows, 3)))
-        res.quat = buf(res.quat, (D, rows, 4)) if dump_quat else None
+        res.att, res.pos, res.vel = (_reuse(res.att, (D, rows, 3), dev), _reuse(res.pos, (D, rows, 3), dev),
+                                     _reuse(res.vel, (D, rows, 3), dev))
+        res.quat = _reuse(res.quat, (D, rows, 4), dev) if dump_quat else None
     else:
         res.att = res.pos = res.vel = res.quat = None
     if dump_imu and D > 0:
-        res.gyro, res.accel = buf(res.gyro, (D, rows, 3)), buf(res.accel, (D, rows, 3))
-        res.odo = buf(res.odo, (D, rows)) if cfg.algo == 1 else None
+        res.gyro, res.accel = _reuse(res.gyro, (D, rows, 3), dev), _reuse(res.accel, (D, rows, 3), dev)
+        res.odo = _reuse(res.odo, (D, rows), dev) if cfg.algo == 1 else None
     else:
         res.gyro = res.accel = res.odo = None
     cfg.dump_odo = res.odo.data_ptr() if res.odo is not None else None
@@ -324,26 +325,6 @@ def error_stats(err):
     _lib.check(lib.b2ins_error_stats_f64(R, nc, _ptr(err), _ptr(stats),
                                          _ptr(_stats_ws(nc, err.device)), _stream()))
     return stats
-
-
-def error_partial(err):
-    """K3 phase 1: [2*ncomp] = (sum e, max|e|) of this shard."""
-    lib = _lib.load()
-    R, nc = err.shape
-    out = torch.empty(2 * nc, dtype=torch.float64, device=err.device)
-    _lib.check(lib.b2ins_error_partial_f64(R, nc, _ptr(err), _ptr(out),
-                                           _ptr(_stats_ws(nc, err.device)), _stream()))
-    return out
-
-
-def error_partial2(err, mean):
-    """K3 phase 2: [ncomp] = sum (e - mean)^2 of this shard."""
-    lib = _lib.load()
-    R, nc = err.shape
-    out = torch.empty(nc, dtype=torch.float64, device=err.device)
-    _lib.check(lib.b2ins_error_partial2_f64(R, nc, _ptr(err), _ptr(mean.contiguous()), _ptr(out),
-                                            _ptr(_stats_ws(nc, err.device)), _stream()))
-    return out
 
 
 def psd_series(fs, n, runs, sensor, vib_def, seed, run_offset=0):
@@ -472,17 +453,12 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     cfg.earth_rot = int(bool(earth_rot))
     cfg.vel_rw, cfg.att_rw = float(vel_rw), float(att_rw)
     res = out or EkfResult()
-
-    def buf(cur, shape):
-        if cur is not None and tuple(cur.shape) == tuple(shape):
-            return cur
-        return torch.empty(shape, dtype=torch.float64, device=dev)
-    res.end_err = buf(res.end_err, (runs, 9))
-    res.end_bias = buf(res.end_bias, (runs, 6))
-    res.consist = buf(res.consist, (runs, 19))
+    res.end_err = _reuse(res.end_err, (runs, 9), dev)
+    res.end_bias = _reuse(res.end_bias, (runs, 6), dev)
+    res.consist = _reuse(res.consist, (runs, 19), dev)
     if dump_runs > 0:
         rows = -(-n // max(1, int(dump_stride)))
-        res.att, res.pos, res.vel, res.wb, res.ab = (buf(getattr(res, k), (dump_runs, rows, 3))
+        res.att, res.pos, res.vel, res.wb, res.ab = (_reuse(getattr(res, k), (dump_runs, rows, 3), dev)
                                                      for k in ('att', 'pos', 'vel', 'wb', 'ab'))
     else:
         res.att = res.pos = res.vel = res.wb = res.ab = None

@@ -24,6 +24,7 @@ Dispatch on `algorithm`:
   * None                               -> sensor data only.
 Multi-GPU: runs are sharded by rank when torch.distributed is initialised (dist.py).
 """
+import copy
 import math
 import os
 import weakref
@@ -232,8 +233,16 @@ class _DataDict(dict):
         return self[key] if key in self else default
 
 
+def _keyed(name, per_run):
+    """{'<name>_<r>': per_run[r]}: an algorithm's per-run outputs under the reference's run keys."""
+    return {'%s_%d' % (name, r): v for r, v in enumerate(per_run)}
+
+
 class _LazyDevice(dict):
-    """{'ref_gyro', 'ref_accel', 'ref_nav'} -> CUDA tensors, uploaded when first asked for."""
+    """The trajectory on the device, each array uploaded when first asked for: ref_gyro, ref_accel, ref_odo,
+    ref_gps, ref_mag, ref_nav ([n][9] att, pos, vel), and for the filter gps_idx (the IMU sample of each GPS
+    row) and gps_vis (visibility).  The single-GPU run() goes through a plan that stages the host arrays
+    itself; the Allan path never needs the navigation rows."""
 
     def __init__(self, sim):
         super().__init__()
@@ -241,8 +250,13 @@ class _LazyDevice(dict):
 
     def __missing__(self, key):
         sim = self._sim()
-        src = sim._nav if key == 'ref_nav' else sim._traj[key]
-        self[key] = engine.to_device(src)
+        t = sim._traj
+        if key == 'gps_idx':
+            self[key] = torch.from_numpy(np.rint(np.asarray(t['gps_time']) * sim.fs[0]).astype(np.int64)).cuda()
+        elif key == 'ref_nav':
+            self[key] = engine.to_device(np.concatenate([t['ref_att'], t['ref_pos'], t['ref_vel']], axis=1))
+        else:
+            self[key] = engine.to_device(t['gps_visibility' if key == 'gps_vis' else key])
         return self[key]
 
 
@@ -357,8 +371,7 @@ class Sim(object):
         self.err_stats = {}     # end-point ensemble statistics of the last run()
         self._traj = None
         self._logged = None      # data read from a logged-data directory (no sensor model)
-        self._dev_cache = None
-        self._cache = {}
+        self._dev = None         # _LazyDevice of the trajectory
 
     # ---- names ------------------------------------------------------------
     def algo_name(self, i):
@@ -396,28 +409,7 @@ class Sim(object):
             if k in traj:
                 d[k] = traj[k]
         self._nav_end = np.concatenate([traj['ref_att'][-1], traj['ref_pos'][-1], traj['ref_vel'][-1]])
-        self._nav_cache = None
-        self._dev_cache = None
-        self._ref_gps_dev = None
-        self._ref_mag_dev = None
-
-    @property
-    def _nav(self):
-        """[n][9] att,pos,vel of the true trajectory (built on first use)."""
-        if self._nav_cache is None:
-            t = self._traj
-            self._nav_cache = np.ascontiguousarray(
-                np.concatenate([t['ref_att'], t['ref_pos'], t['ref_vel']], axis=1))
-        return self._nav_cache
-
-    @property
-    def _dev(self):
-        """The trajectory on the device, each array uploaded on first use (the single-GPU run()
-        goes through a plan that stages the host arrays itself; the Allan path never needs the
-        [n][9] navigation rows)."""
-        if self._dev_cache is None:
-            self._dev_cache = _LazyDevice(self)
-        return self._dev_cache
+        self._dev = _LazyDevice(self)
 
     # ---- run ----------------------------------------------------------------
     def run(self, num_times=1):
@@ -433,8 +425,9 @@ class Sim(object):
             return self._run_logged()
         if self.imu is None:
             raise ValueError('imu must be an IMU model when data are generated from a trajectory')
-        self._cache = {}
-        self._all_hist = None
+        self._blocks = {}        # (block, name) -> [runs of the block, ...] host histories (_history)
+        self._proc = {}          # (algo index, start [s], position frame) -> [R, 3, 9] process statistics
+        self._all_hist = None    # (algo index, first run, arrays) of the last histories() with stride 1
         self.err_stats = {}
         self._mc = {}
         self._vib_acc = parse_env(self.env['acc'], self.fs[0]) if self.env and 'acc' in self.env else None
@@ -444,6 +437,9 @@ class Sim(object):
         if getattr(self.imu, 'magnetometer', False) and 'ref_mag' not in self._traj:
             raise ValueError('imu has a magnetometer (axis=9) but the trajectory has no ref_mag')
         self._shard = dist.shard(R)
+        for a in self.algo or []:      # outputs start afresh: a _Merged view holds the plugins of this run only
+            for o in a.output:
+                self.data.pop(o, None)
         self.data['accel'] = LazyRuns(self, 'accel', R)
         self.data['gyro'] = LazyRuns(self, 'gyro', R)
         if getattr(self.imu, 'odo', False):
@@ -463,7 +459,7 @@ class Sim(object):
                 elif isinstance(a, InsLoose):
                     self._run_ins_loose(i, a)
                 else:
-                    self._run_foreign(i, a)
+                    self._run_plugin(i, a, self._generated_inputs)
         self.sim_complete = True
 
     # ---- logged data (ins_sim.py:415-451: data from files instead of pathgen) -------------------
@@ -498,10 +494,8 @@ class Sim(object):
         """Algorithms on the logged sets 0 .. sim_count-1 (InsAlgoMgr.run_algo over the keys,
         ins_algo_manager.py:73-95): one batched launch per algorithm, outputs keyed
         '<algo>_<key>'; end-point error statistics if the directory has the reference files."""
-        import copy
-        self._cache, self.err_stats, self._mc = {}, {}, {}
-        R = self.sim_count
-        self._shard = (0, R)
+        self._proc, self.err_stats, self._mc = {}, {}, {}
+        self._shard = (0, self.sim_count)
         d = self._logged
         for i, a in enumerate(self.algo or []):
             name = self.algo_name(i)
@@ -515,7 +509,7 @@ class Sim(object):
                                                 self._logged_sets('accel'))
                 for out, arr in (('att_euler', att), ('pos', pos), ('vel', vel)):
                     self.data[out] = dict(self.data[out]) if isinstance(self.data.get(out), dict) else {}
-                    self.data[out].update({'%s_%d' % (name, r): arr[r] for r in range(R)})
+                    self.data[out].update(_keyed(name, arr))
                 self.data['att_quat'] = DerivedRuns(self.data['att_euler'], euler2quat_zyx)
                 if all(k in d for k in ('ref_att_euler', 'ref_pos', 'ref_vel')):
                     err = np.concatenate([
@@ -524,34 +518,42 @@ class Sim(object):
                     self._mc[i]['end_err'] = err
                     self.err_stats[name] = engine.error_stats(engine.to_device(err)).cpu().numpy()
             elif isinstance(a, Allan):
-                tau, ad_a, ad_g = a.run_batch(self.fs[0], self._logged_sets('accel'), self._logged_sets('gyro'))
-                self.data['algo_time'] = {'%s_%d' % (name, r): tau for r in range(R)}
-                self.data['ad_accel'] = {'%s_%d' % (name, r): ad_a[r] for r in range(R)}
-                self.data['ad_gyro'] = {'%s_%d' % (name, r): ad_g[r] for r in range(R)}
+                self._publish_allan(name, *a.run_batch(self.fs[0], self._logged_sets('accel'),
+                                                       self._logged_sets('gyro')))
             else:
-                outs = {o: {} for o in a.output}
-                for r in range(R):
-                    args = []
-                    for nm in a.input:
-                        v = self.data[nm] if nm in self.data else None
-                        if isinstance(v, dict):
-                            v = v.get(r)
-                        if v is None:
-                            raise ValueError('algorithm input %r is not in the data directory' % nm)
-                        args.append(v)
-                    a.reset()
-                    a.run(copy.deepcopy(args))
-                    for o, v in zip(a.output, a.get_results()):
-                        outs[o]['%s_%d' % (name, r)] = v
-                for o in a.output:
-                    self.data[o] = outs[o]
+                self._run_plugin(i, a, self._logged_inputs)
         self.sim_complete = True
 
-    def _mc_config(self, ai, runs, r0, stats_start=-1, dump_runs=0):
-        """Config for experiment runs [r0, r0+runs) of algorithm ai.  Philox streams are
-        named by the experiment run index (all algorithms see the same sensor data, as in
-        the reference where loop A runs once); the initial-state rule counts the plugin's
-        own run_times."""
+    def _logged_inputs(self, algo, r):
+        """Inputs of run r of a foreign plugin on logged data: set r of per-run data, everything else as is."""
+        args = []
+        for nm in algo.input:
+            v = self.data.get(nm)
+            if isinstance(v, dict):
+                v = v.get(r)
+            if v is None:
+                raise ValueError('algorithm input %r is not in the data directory' % nm)
+            args.append(v)
+        return args
+
+    def _run_plugin(self, i, algo, inputs):
+        """A reference-style plugin run on the host (the per-run protocol of InsAlgoMgr.run_algo,
+        ins_algo_manager.py:73-95); inputs(algo, r): its input list for run r."""
+        name = self.algo_name(i)
+        outs = {o: {} for o in algo.output}
+        for r in range(self.sim_count):
+            args = inputs(algo, r)
+            algo.reset()
+            algo.run(copy.deepcopy(args))
+            for o, v in zip(algo.output, algo.get_results()):
+                outs[o]['%s_%d' % (name, r)] = v
+        self.data.update(outs)
+
+    def _mc_config(self, ai, r0, runs, **kw):
+        """Config for experiment runs [r0, r0+runs) of algorithm ai; kw: make_mc_config's stats_start,
+        dump_runs, dump_stride, proc_pos_frame.  Philox streams are named by the experiment run index (all
+        algorithms see the same sensor data, as in the reference where loop A runs once); the
+        initial-state rule counts the plugin's own run_times."""
         algo = self.algo[ai]
         n = self._traj['ref_gyro'].shape[0]
         vib_gyro, vib_acc = self._vib_pair(runs, r0)
@@ -560,8 +562,16 @@ class Sim(object):
             algo.ini_sets.shape[0], algo.ini_sets.shape[1], earth_rot=algo.earth_rot,
             run_offset=self.run_base + r0, ini_offset=self._mc[ai]['base'] + r0,
             vib_gyro=vib_gyro, vib_accel=vib_acc,
-            lanes_per_run=self.lanes_per_run or algo.lanes_per_run, stats_start=stats_start,
-            dump_runs=dump_runs, **self._odo_args(algo))
+            lanes_per_run=self.lanes_per_run or algo.lanes_per_run, **kw, **self._odo_args(algo))
+
+    def _mc_launch(self, ai, r0, runs, stats_start=-1, dump_runs=0, dump_stride=1, proc_pos_frame=0, **kw):
+        """K12 for experiment runs [r0, r0+runs) of algorithm ai on the device trajectory; kw: what
+        engine.mc_free_integration outputs beside the end-point errors."""
+        cfg = self._mc_config(ai, r0, runs, stats_start=stats_start, dump_runs=dump_runs, dump_stride=dump_stride,
+                              proc_pos_frame=proc_pos_frame)
+        d = self._dev
+        return engine.mc_free_integration(cfg, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
+                                          self.algo[ai].ini_device(), **kw)
 
     def _odo_args(self, algo):
         """Odometer variant: noise model (imu.odo_err) and the true forward speed on the device."""
@@ -569,9 +579,7 @@ class Sim(object):
             return {}
         if not getattr(self.imu, 'odo', False) or 'ref_odo' not in self._traj:
             raise ValueError('free_integration_odo needs IMU(odo=True) and a trajectory with ref_odo')
-        if getattr(self, '_ref_odo_dev', None) is None:
-            self._ref_odo_dev = engine.to_device(self._traj['ref_odo'])
-        return {'odo_err': self.imu.odo_err, 'ref_odo': self._ref_odo_dev}
+        return {'odo_err': self.imu.odo_err, 'ref_odo': self._dev['ref_odo']}
 
     def _vib_pair(self, runs, r0):
         """(vib_gyro, vib_accel) arguments for experiment runs [r0, r0+runs): parsed dicts, or
@@ -601,17 +609,17 @@ class Sim(object):
         name = self.algo_name(i)
         lo, hi = self._shard
         self._mc[i] = {'base': algo.run_times, 'end_err': None}   # plugin's run counter at run 0
+        err, stats = np.zeros((0, 9)), np.zeros((3, 9))
         if not isinstance(algo, FreeIntegrationOdo):
             # the plan path on this rank's shard (pinned staging, one H2D, K12, K3, one D2H);
             # with several ranks the [3][9] shard statistics are merged by one all_gather
-            err, stats = np.zeros((0, 9)), np.zeros((3, 9))
             # the exchange path is chosen from the LARGEST shard, a rank-independent quantity (shards
             # differ by one run; every rank must take the same collective)
             w = dist.world()
             p2p = dist.fused_exchange(9) if w > 1 and -(-self.sim_count // w) * 9 <= (1 << 17) else None
             plan = None
             if hi > lo:
-                cfg = self._mc_config(i, hi - lo, lo)
+                cfg = self._mc_config(i, lo, hi - lo)
                 t = self._traj
                 plan = engine.get_plan(cfg.n, cfg.runs, cfg.ini_sets, cfg.ini_rows)
                 if self._uses_psd():
@@ -633,23 +641,19 @@ class Sim(object):
             else:
                 self.err_stats[name] = dist.combine_local_stats(stats, hi - lo)
         else:
-            d = self._dev
-            err, stats = np.zeros((0, 9)), np.zeros((3, 9))
             if hi > lo:
-                cfg = self._mc_config(i, hi - lo, lo)
-                res = engine.mc_free_integration(cfg, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
-                                                 algo.ini_device())
+                res = self._mc_launch(i, lo, hi - lo)
                 stats = engine.error_stats(res.end_err).cpu().numpy()
                 err = res.end_err.cpu().numpy()
             self._mc[i]['end_err'] = err
             self.err_stats[name] = dist.combine_local_stats(stats, hi - lo)
         algo.run_times += self.sim_count
-        for out in ('att_euler', 'pos', 'vel'):
+        for out in ('att_euler', 'pos', 'vel'):     # several free-integration plugins: one view over all
             prev = self.data.get(out)
             lazy = LazyRuns(self, (i, out), self.sim_count, prefix=name)
             if isinstance(prev, _Merged):
                 prev.add(lazy)
-            elif isinstance(prev, LazyRuns) and prev._name[0] != i:
+            elif isinstance(prev, LazyRuns):
                 self.data[out] = _Merged([prev, lazy])
             else:
                 self.data[out] = lazy
@@ -665,71 +669,94 @@ class Sim(object):
                                 run_offset=self.run_base + r0, vib_gyro=vib_gyro,
                                 vib_accel=vib_acc, layout=layout)
 
-    def _run_allan(self, i, algo):
-        """K1 (channel-major) + K4 for this rank's shard of the runs, in blocks sized to the free
-        device memory; the [R, ntau, 3] deviations of all ranks are gathered (a few hundred KB)."""
-        name = self.algo_name(i)
-        R = self.sim_count
+    def _generated_inputs(self, algo, r):
+        """Inputs of run r of a foreign plugin: gyro and accel from K1 (one launch per run), mag from the
+        history block get_data(['mag']) serves, everything else from self.data."""
+        gyro, accel = self._noise_block(r, r + 1)
+        per_run = {'gyro': gyro[0].cpu().numpy(), 'accel': accel[0].cpu().numpy()}
+        if 'mag' in algo.input and 'mag' in self.data:
+            per_run['mag'] = self.data['mag'][r]
+        args = []
+        for nm in algo.input:
+            v = per_run[nm] if nm in per_run else self.data.get(nm)
+            if v is None or isinstance(v, Mapping):
+                raise ValueError('algorithm input %r is not generated by this engine' % nm)
+            args.append(v)
+        return args
+
+    # ---- Allan variance (K1 + K4, or K1 fused into K4) ------------------------------------------
+    def _allan_block(self, bytes_per_sample, share):
+        """Runs per Allan block of this rank's shard: `bytes_per_sample` of device memory per run-sample, in
+        at most 1/share of the free device memory (free on the device + cached by torch's allocator but
+        unused)."""
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
-        if self._vib_acc is None and self._vib_gyro is None and n > 5040 and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0':
-            return self._run_allan_fused(i, name, R, lo, hi, n)
-        # runs per block: K1 materialises 48 B and K4 needs ~2 B of workspace per run-sample;
-        # use up to a third of the free device memory
-        if torch.cuda.is_available():    # free on the device + cached by torch's allocator but unused
+        if torch.cuda.is_available():
             free_b = (torch.cuda.mem_get_info()[0] + torch.cuda.memory_reserved()
                       - torch.cuda.memory_allocated())
         else:
             free_b = 2 ** 31
-        block = max(1, min(max(hi - lo, 1), int(free_b / 3 // (n * 64)) or 1))
-        tau_all, acc_blocks, gyr_blocks = None, [], []
+        return max(1, min(max(hi - lo, 1), int(free_b / share // (n * bytes_per_sample)) or 1))
+
+    def _publish_allan(self, name, tau, ad_accel, ad_gyro):
+        """algo_time (the same tau for every run), ad_accel, ad_gyro [R, ntau, 3] under run keys."""
+        self.data['algo_time'] = _keyed(name, [tau] * len(ad_accel))
+        self.data['ad_accel'] = _keyed(name, ad_accel)
+        self.data['ad_gyro'] = _keyed(name, ad_gyro)
+
+    def _run_allan(self, i, algo):
+        """The Allan deviations of this rank's shard of the runs, in run blocks sized to the free device
+        memory; the [R, ntau, 6] deviations of all ranks are gathered (a few hundred KB).  Without a vibration
+        model and with series longer than one chunk, K1 is fused into K4's first level (engine.allan_mc) and
+        the only device memory is the decade-sum workspace (about 2 B per run-sample), so run blocks are
+        rarely needed; otherwise K1 materialises the series (48 B per run-sample) for K4 (~2 B of workspace)."""
+        lo, hi = self._shard
+        n = self._traj['ref_gyro'].shape[0]
+        fused = (self._vib_acc is None and self._vib_gyro is None and n > 5040
+                 and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
+        tau = engine.allan_taus(n, self.fs[0])
+        block = self._allan_block(6 * 2, 2) if fused else self._allan_block(64, 3)
+        parts = []      # [runs, ntau, 6]: accel, gyro
         for r0 in range(lo, hi, block):
             r1 = min(hi, r0 + block)
-            # every channel a contiguous series: K4 then streams them with bulk copies
-            gyro, accel = self._noise_block(r0, r1, engine.LAYOUT_CHANNEL_MAJOR)
-            tau, a, g = algo.run_batch(self.fs[0], accel, gyro, channel_major=True)
-            acc_blocks.append(a)
-            gyr_blocks.append(g)
-            tau_all = tau
-        if tau_all is None:      # a rank without runs still needs tau for the gather below
-            tau_all = engine.allan_taus(n, self.fs[0])
-        ntau = len(tau_all)
-        a = np.concatenate(acc_blocks) if acc_blocks else np.zeros((0, ntau, 3))
-        g = np.concatenate(gyr_blocks) if gyr_blocks else np.zeros((0, ntau, 3))
+            if fused:
+                d = self._dev
+                avar, _ = engine.allan_mc(self.fs[0], r1 - r0, d['ref_gyro'], d['ref_accel'], self.imu.gyro_err,
+                                          self.imu.accel_err, self.seed, run_offset=self.run_base + r0)
+                parts.append(torch.sqrt(avar).permute(0, 2, 1).contiguous().cpu().numpy())
+            else:
+                # every channel a contiguous series: K4 then streams them with bulk copies
+                gyro, accel = self._noise_block(r0, r1, engine.LAYOUT_CHANNEL_MAJOR)
+                tau, a, g = algo.run_batch(self.fs[0], accel, gyro, channel_major=True)
+                parts.append(np.concatenate([a, g], axis=2))
+        both = np.concatenate(parts) if parts else np.zeros((0, len(tau), 6))
         if dist.world() > 1:
-            both = np.concatenate([a.reshape(hi - lo, -1), g.reshape(hi - lo, -1)], axis=1)
-            both = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(both)), R)
-            a = both[:, :ntau * 3].reshape(R, ntau, 3)
-            g = both[:, ntau * 3:].reshape(R, ntau, 3)
-        self.data['algo_time'] = {'%s_%d' % (name, r): tau_all for r in range(R)}
-        self.data['ad_accel'] = {'%s_%d' % (name, r): a[r] for r in range(R)}
-        self.data['ad_gyro'] = {'%s_%d' % (name, r): g[r] for r in range(R)}
+            both = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(both.reshape(hi - lo, -1))),
+                                    self.sim_count).reshape(self.sim_count, len(tau), 6)
+        self._publish_allan(self.algo_name(i), tau, both[:, :, 0:3], both[:, :, 3:6])
 
     # ---- loosely-coupled GNSS/INS filter (K7) -------------------------------------------------
     def _ekf_inputs(self):
         """Device copies of what K7 reads beside the IMU truth: GPS truth rows, their IMU sample
         indices, visibility."""
-        if getattr(self, '_ekf_dev', None) is None:
-            t = self._traj
-            if self.ref_frame != 0:
-                raise ValueError('ins_loose works in ref_frame 0 (LLA positions, NED velocities)')
-            if not (getattr(self.imu, 'gps', False) and 'ref_gps' in t and self.fs[1] > 0):
-                raise ValueError('ins_loose needs IMU(gps=True), fs = [fs_imu, fs_gps, ...] and a trajectory '
-                                 'with ref_gps / gps_time / gps_visibility')
-            idx = np.rint(np.asarray(t['gps_time']) * self.fs[0]).astype(np.int64)
-            self._ekf_dev = {'ref_gps': engine.to_device(t['ref_gps']),
-                             'gps_idx': torch.from_numpy(np.ascontiguousarray(idx)).cuda(),
-                             'gps_vis': engine.to_device(np.asarray(t['gps_visibility'], dtype=np.float64))}
-        return self._ekf_dev
+        t = self._traj
+        if self.ref_frame != 0:
+            raise ValueError('ins_loose works in ref_frame 0 (LLA positions, NED velocities)')
+        if not (getattr(self.imu, 'gps', False) and 'ref_gps' in t and self.fs[1] > 0):
+            raise ValueError('ins_loose needs IMU(gps=True), fs = [fs_imu, fs_gps, ...] and a trajectory '
+                             'with ref_gps / gps_time / gps_visibility')
+        d = self._dev
+        return d['ref_gps'], d['gps_idx'], d['gps_vis']
 
     def _ekf_launch(self, algo, r0, runs, stats_start=0, dump_runs=0, dump_stride=1):
-        d, e = self._dev, self._ekf_inputs()
+        gps = self._ekf_inputs()
+        d = self._dev
         ini = algo.ini if algo.ini is not None else self._traj.get('ini')
         if ini is None:
             raise ValueError('InsLoose needs ini_pos_vel_att (the trajectory carries no initial state)')
         return engine.ins_loose(self.fs[0], runs, self.seed, self.imu.gyro_err, self.imu.accel_err,
                                 self.imu.gps_err, ini, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
-                                e['ref_gps'], e['gps_idx'], e['gps_vis'], run_offset=self.run_base + r0,
+                                *gps, run_offset=self.run_base + r0,
                                 ini_att_std=algo.ini_att_std, earth_rot=algo.earth_rot,
                                 stats_start=stats_start, dump_runs=dump_runs, dump_stride=dump_stride,
                                 vel_rw=algo.vel_model_std, att_rw=algo.att_model_std)
@@ -764,121 +791,52 @@ class Sim(object):
         return {'nees': c[:, 0:3] / ep, 'inside3': c[:, 3:18] / ep, 'epochs': int(c[0, 18]) if len(c) else 0,
                 'end_bias': self._mc[algo_index]['end_bias']}
 
-    def _run_allan_fused(self, i, name, R, lo, hi, n):
-        """The Allan experiment without the series: K1 fused into K4's first level (engine.allan_mc).
-        Used when no vibration model is set and the series is longer than one chunk; the only device
-        memory is the decade-sum workspace (about 2 B per run-sample), so run blocks are rarely needed."""
-        d = self._dev
-        tau_all = engine.allan_taus(n, self.fs[0])
-        ntau = len(tau_all)
-        if torch.cuda.is_available():
-            free_b = (torch.cuda.mem_get_info()[0] + torch.cuda.memory_reserved() - torch.cuda.memory_allocated())
-        else:
-            free_b = 2 ** 31
-        block = max(1, min(max(hi - lo, 1), int(free_b / 2 // (n * 6 * 2)) or 1))
-        parts = []
-        for r0 in range(lo, hi, block):
-            r1 = min(hi, r0 + block)
-            avar, _ = engine.allan_mc(self.fs[0], r1 - r0, d['ref_gyro'], d['ref_accel'], self.imu.gyro_err,
-                                      self.imu.accel_err, self.seed, run_offset=self.run_base + r0)
-            parts.append(torch.sqrt(avar).permute(0, 2, 1).contiguous().cpu().numpy())     # [r, ntau, 6]
-        both = np.concatenate(parts) if parts else np.zeros((0, ntau, 6))
-        if dist.world() > 1:
-            both = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(both.reshape(hi - lo, -1))), R)
-            both = both.reshape(R, ntau, 6)
-        self.data['algo_time'] = {'%s_%d' % (name, r): tau_all for r in range(R)}
-        self.data['ad_accel'] = {'%s_%d' % (name, r): both[r, :, 0:3] for r in range(R)}
-        self.data['ad_gyro'] = {'%s_%d' % (name, r): both[r, :, 3:6] for r in range(R)}
-
-    def _run_foreign(self, i, algo):
-        """Reference-style plugin run on the host, sensor data from K1
-        (the per-run protocol of InsAlgoMgr.run_algo, ins_algo_manager.py:73-95)."""
-        import copy
-        name = self.algo_name(i)
-        outs = {o: {} for o in algo.output}
-        static = {'fs': self.fs[0], 'ref_frame': self.ref_frame, 'time': self.data['time']}
-        for r in range(self.sim_count):
-            gyro, accel = self._noise_block(r, r + 1)
-            per_run = {'gyro': gyro[0].cpu().numpy(), 'accel': accel[0].cpu().numpy()}
-            if 'mag' in algo.input and 'mag' in self.data:
-                per_run['mag'] = self.data['mag'][r]     # the block get_data(['mag']) serves
-            args = []
-            for nm in algo.input:
-                if nm in per_run:
-                    args.append(per_run[nm])
-                elif nm in static:
-                    args.append(static[nm])
-                elif nm in self.data and not isinstance(self.data[nm], (dict, Mapping)):
-                    args.append(self.data[nm])
-                else:
-                    raise ValueError('algorithm input %r is not generated by this engine' % nm)
-            algo.reset()
-            algo.run(copy.deepcopy(args))
-            res = algo.get_results()
-            for o, v in zip(algo.output, res):
-                outs[o]['%s_%d' % (name, r)] = v
-        for o in algo.output:
-            self.data[o] = outs[o]
-
     # ---- lazy histories -------------------------------------------------------
     def _history(self, name, run):
-        """(n,3) history of one run; materialises a block of neighbouring runs at once."""
-        blk = run // self.history_block
-        whole = getattr(self, '_all_hist', None)      # histories() has pulled every run already
-        if whole is not None:
-            ai_w, lo_w, arrs = whole
+        """(n,3) history of one run: from the histories() arrays if they hold it, else from the history block
+        of neighbouring runs that one launch of name's source fills.  name: a sensor name, or
+        (algo index, output name)."""
+        if self._all_hist is not None:
+            ai_w, lo_w, arrs = self._all_hist
             key_w = name[1] if isinstance(name, tuple) and name[0] == ai_w else name
             if isinstance(key_w, str) and key_w in arrs and 0 <= run - lo_w < arrs[key_w].shape[0]:
                 return arrs[key_w][run - lo_w]
-        if isinstance(name, tuple):      # algorithm output (algo index, data name)
-            ai, out = name
-            key = ('nav', ai, blk)
-            if key not in self._cache and isinstance(self.algo[ai], InsLoose):
-                r0 = blk * self.history_block
-                r1 = min(self.sim_count, r0 + self.history_block)
-                res = self._ekf_launch(self.algo[ai], r0, r1 - r0, dump_runs=r1 - r0)
-                self._cache[key] = {'att_euler': res.att.cpu().numpy(), 'pos': res.pos.cpu().numpy(),
-                                    'vel': res.vel.cpu().numpy(), 'wb': res.wb.cpu().numpy(),
-                                    'ab': res.ab.cpu().numpy()}
-            if key not in self._cache:
-                algo = self.algo[ai]
-                r0 = blk * self.history_block
-                r1 = min(self.sim_count, r0 + self.history_block)
-                cfg = self._mc_config(ai, r1 - r0, r0, dump_runs=r1 - r0)
-                d = self._dev
-                res = engine.mc_free_integration(cfg, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
-                                                 algo.ini_device(), dump_nav=True, dump_imu=True)
-                self._cache[key] = {'att_euler': res.att.cpu().numpy(), 'pos': res.pos.cpu().numpy(),
-                                    'vel': res.vel.cpu().numpy()}
-                imu_hist = {'gyro': res.gyro.cpu().numpy(), 'accel': res.accel.cpu().numpy()}
-                if res.odo is not None:
-                    imu_hist['odo'] = res.odo.cpu().numpy()
-                self._cache.setdefault(('imu', blk), {}).update(imu_hist)
-            return self._cache[key][out][run - blk * self.history_block]
-        key = ('imu', blk)
-        if key not in self._cache or name not in self._cache[key]:
+        blk, i = divmod(run, self.history_block)
+        if (blk, name) not in self._blocks:
             r0 = blk * self.history_block
-            r1 = min(self.sim_count, r0 + self.history_block)
-            hist = self._cache.setdefault(key, {})
-            if name == 'odo':      # pathgen.odo_gen stream: a zero-length odometer experiment
-                ai = [i for i, a in enumerate(self.algo or []) if isinstance(a, FreeIntegrationOdo)]
-                if not ai:
-                    raise KeyError('odo histories are produced with the free_integration_odo plugin')
-                self._history((ai[0], 'pos'), run)
-            elif name == 'gps':
-                if getattr(self, '_ref_gps_dev', None) is None:
-                    self._ref_gps_dev = engine.to_device(self._traj['ref_gps'])
-                hist['gps'] = engine.gps_noise(r1 - r0, self._ref_gps_dev, self.imu.gps_err, self.ref_frame,
-                                               self.seed, run_offset=self.run_base + r0).cpu().numpy()
-            elif name == 'mag':
-                if getattr(self, '_ref_mag_dev', None) is None:
-                    self._ref_mag_dev = engine.to_device(self._traj['ref_mag'])
-                hist['mag'] = engine.mag_noise(r1 - r0, self._ref_mag_dev, self.imu.mag_err, self.seed,
-                                               run_offset=self.run_base + r0).cpu().numpy()
-            else:
-                gyro, accel = self._noise_block(r0, r1)
-                hist.update({'gyro': gyro.cpu().numpy(), 'accel': accel.cpu().numpy()})
-        return self._cache[key][name][run - blk * self.history_block]
+            filled = self._history_block(name, r0, min(self.sim_count, r0 + self.history_block) - r0)
+            self._blocks.update({(blk, k): v for k, v in filled.items()})
+        return self._blocks[(blk, name)][i]
+
+    def _history_block(self, name, r0, runs):
+        """One launch of what produces `name` for runs [r0, r0+runs): {name: [runs, ...] host array} of every
+        history that launch makes.  A K12 block also holds the IMU samples of its runs (and the odometer's,
+        for the odometer variant); odo histories come from the odometer plugin's K12 block."""
+        if name == 'odo':      # pathgen.odo_gen stream: a zero-length odometer experiment
+            ai = [i for i, a in enumerate(self.algo or []) if isinstance(a, FreeIntegrationOdo)]
+            if not ai:
+                raise KeyError('odo histories are produced with the free_integration_odo plugin')
+            name = (ai[0], 'pos')
+        if isinstance(name, tuple) and isinstance(self.algo[name[0]], InsLoose):
+            res = self._ekf_launch(self.algo[name[0]], r0, runs, dump_runs=runs)
+            return {(name[0], k): v.cpu().numpy() for k, v in (('att_euler', res.att), ('pos', res.pos),
+                                                               ('vel', res.vel), ('wb', res.wb), ('ab', res.ab))}
+        if isinstance(name, tuple):
+            res = self._mc_launch(name[0], r0, runs, dump_runs=runs, dump_nav=True, dump_imu=True)
+            out = {(name[0], k): v.cpu().numpy() for k, v in (('att_euler', res.att), ('pos', res.pos),
+                                                              ('vel', res.vel))}
+            out.update({'gyro': res.gyro.cpu().numpy(), 'accel': res.accel.cpu().numpy()})
+            if res.odo is not None:
+                out['odo'] = res.odo.cpu().numpy()
+            return out
+        if name == 'gps':
+            return {'gps': engine.gps_noise(runs, self._dev['ref_gps'], self.imu.gps_err, self.ref_frame,
+                                            self.seed, run_offset=self.run_base + r0).cpu().numpy()}
+        if name == 'mag':
+            return {'mag': engine.mag_noise(runs, self._dev['ref_mag'], self.imu.mag_err, self.seed,
+                                            run_offset=self.run_base + r0).cpu().numpy()}
+        gyro, accel = self._noise_block(r0, r0 + runs)
+        return {'gyro': gyro.cpu().numpy(), 'accel': accel.cpu().numpy()}
 
     def histories(self, algo_index=0, imu=False, stride=1, quat=False):
         '''
@@ -895,16 +853,13 @@ class Sim(object):
         if not isinstance(algo, FreeIntegration) or self._logged is not None:
             raise ValueError('histories() is for the fused free-integration experiment')
         runs = hi - lo
-        n = self._traj['ref_gyro'].shape[0]
-        out = {}
         if runs == 0:
+            n = self._traj['ref_gyro'].shape[0]
             return {k: np.zeros((0, n, 3)) for k in ('att_euler', 'pos', 'vel')}
-        cfg = self._mc_config(algo_index, runs, lo, dump_runs=runs)
-        cfg.dump_stride = max(1, int(stride))
-        d = self._dev
+        stride = max(1, int(stride))
         pool = _hist_pool(self)      # device + pinned buffers: this Sim's, or a dead Sim's (never a live one's)
-        res = engine.mc_free_integration(cfg, d['ref_gyro'], d['ref_accel'], d['ref_nav'], algo.ini_device(),
-                                         dump_nav=True, dump_imu=imu, out=pool.get('res'), dump_quat=quat)
+        res = self._mc_launch(algo_index, lo, runs, dump_runs=runs, dump_stride=stride, dump_nav=True,
+                              dump_imu=imu, out=pool.get('res'), dump_quat=quat)
         pool['res'] = res
         pinned = pool.setdefault('pinned', {})
         names = [('att_euler', res.att), ('pos', res.pos), ('vel', res.vel)]
@@ -919,10 +874,10 @@ class Sim(object):
             pinned[k].copy_(t, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         out = {k: pinned[k].numpy() for k, _ in names}
-        if cfg.dump_stride == 1:
+        if stride == 1:
             self._all_hist = (algo_index, lo, out)
         else:
-            out['time'] = self.data['time'][::cfg.dump_stride]
+            out['time'] = self.data['time'][::stride]
         return out
 
     # ---- results --------------------------------------------------------------
@@ -1011,8 +966,7 @@ class Sim(object):
         """'ned' / 'ecef' position error of LLA results, ins_data_manager.py:543-552."""
         err = self._mc[algo_index]['end_err']
         if dist.world() > 1:
-            import torch as _t
-            err = dist.gather_rows(_t.from_numpy(err), self.sim_count)
+            err = dist.gather_rows(torch.from_numpy(err), self.sim_count)
         r = self._traj['ref_pos'][-1]
         x = err[:, 3:6] + r            # end position = error + truth
         err = lla2ecef(x) - lla2ecef(r)[0]
@@ -1023,20 +977,17 @@ class Sim(object):
     def _process_stats(self, algo_index, start_s, c0, frame=0):
         """Per-run process statistics of columns c0:c0+3; frame: the position frame (engine.POS_FRAME_*).
         One launch holds all nine columns: the attitude and velocity columns of any frame's launch serve."""
-        key = ('proc', algo_index, float(start_s), frame)
+        key = (algo_index, float(start_s), frame)
         if c0 != 3:
-            key = next((k for k in (('proc', algo_index, float(start_s), f) for f in (frame, 0, 1, 2))
-                        if k in self._cache), key)
-        if key not in self._cache:
-            t = self.data['time']
-            idx = np.where(t >= start_s)[0]
+            key = next((k for k in ((algo_index, float(start_s), f) for f in (frame, 0, 1, 2))
+                        if k in self._proc), key)
+        if key not in self._proc:
+            idx = np.where(self.data['time'] >= start_s)[0]
             if idx.shape[0] == 0:
                 print('err_stats_start exceeds max data points.')
                 start = 0
             else:
                 start = int(idx[0])
-            algo = self.algo[algo_index]
-            lo, hi = self._shard
             if self._logged is not None:
                 # the histories are on the host already (array_error + __array_stats,
                 # ins_data_manager.py:512-541, :797-808)
@@ -1051,25 +1002,17 @@ class Sim(object):
                         lla_error_metres(pos, ref_pos, frame) if frame else pos - ref_pos,
                         self.data['vel'][k] - self._logged['ref_vel']], axis=1)[start:]
                     ps[r] = np.stack([np.max(np.abs(e), 0), np.average(e, 0), np.std(e, 0)])
-                self._cache[key] = ps
-                return self._process_stats(algo_index, start_s, c0, frame)
-            d = self._dev
-            ps = None
-            if hi > lo:
-                cfg = self._mc_config(algo_index, hi - lo, lo, stats_start=start)
-                cfg.proc_pos_frame = frame
-                ps = engine.mc_free_integration(cfg, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
-                                                algo.ini_device()).proc_stats.reshape(hi - lo, 27)
-            self._cache[key] = dist.gather_rows(ps, self.sim_count).reshape(-1, 3, 9)
-        ps = self._cache[key]
+            else:
+                lo, hi = self._shard
+                ps = None
+                if hi > lo:
+                    ps = self._mc_launch(algo_index, lo, hi - lo, stats_start=start,
+                                         proc_pos_frame=frame).proc_stats.reshape(hi - lo, 27)
+                ps = dist.gather_rows(ps, self.sim_count).reshape(-1, 3, 9)
+            self._proc[key] = ps
+        ps = self._proc[key]
         name = self.algo_name(algo_index)
-        out = {'max': {}, 'avg': {}, 'std': {}}
-        for r in range(self.sim_count):
-            k = '%s_%d' % (name, r)
-            out['max'][k] = ps[r, 0, c0:c0 + 3].copy()
-            out['avg'][k] = ps[r, 1, c0:c0 + 3].copy()
-            out['std'][k] = ps[r, 2, c0:c0 + 3].copy()
-        return out
+        return {s: _keyed(name, ps[:, k, c0:c0 + 3].copy()) for k, s in enumerate(('max', 'avg', 'std'))}
 
     def results(self, data_dir=None, err_stats_start=0, gen_kml=False, extra_opt=''):
         '''
@@ -1088,7 +1031,7 @@ class Sim(object):
         s += 'Reference frame: %s\n' % str(self.ref_frame)
         s += 'Simulation time duration: %s s\n' % str(len(self.data['time']) / self.fs[0])
         s += 'Simulation runs: %s\n' % str(self.sim_count)
-        has_mc = bool(getattr(self, '_mc', None)) and bool(self.err_stats)   # logged data may lack references
+        has_mc = bool(self._mc) and bool(self.err_stats)   # logged data may lack references
         if has_mc:
             s += '\n------------------------------------------------------------\n'
             s += 'The following are error statistics.'
@@ -1130,7 +1073,6 @@ _HIST_POOLS = []      # [weakref to the owning Sim or None, dict]
 
 
 def _hist_pool(sim):
-    import weakref
     for entry in _HIST_POOLS:
         if entry[0] is not None and entry[0]() is sim:
             return entry[1]

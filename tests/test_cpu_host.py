@@ -291,10 +291,6 @@ def _gloo_worker(rank, world, port, tmp):
     err = rng.randn(total, 9) * np.logspace(-4, 2, 9) + 0.3
     lo, hi = dist.shard(total)
     mine = torch.from_numpy(err[lo:hi])
-    # what K3 phase 1 / 2 compute on each rank (numpy stands in for the kernels here)
-    partial = torch.cat([mine.sum(0), mine.abs().max(0).values])
-    mean, mx, tot = dist.combine_phase1(partial, hi - lo, 9)
-    std = dist.combine_phase2(((mine - mean) ** 2).sum(0), tot)
     loc = mine.numpy()
     merged = dist.combine_local_stats(np.stack([np.abs(loc).max(0), loc.mean(0), loc.std(0)]), hi - lo)
     rows = dist.gather_rows(mine, total)
@@ -302,12 +298,11 @@ def _gloo_worker(rank, world, port, tmp):
     if rank == 0:
         traj = {k: rng.randn(50, 3) for k in ('ref_pos', 'ref_vel', 'ref_att', 'ref_accel', 'ref_gyro')}
     got = dist.broadcast_trajectory(traj)
-    np.savez(os.path.join(tmp, 'r%d.npz' % rank), mean=mean.numpy(), mx=mx.numpy(), std=std.numpy(),
-             tot=tot, rows=rows, gyro=got['ref_gyro'], lo=lo, hi=hi, merged=merged)
+    np.savez(os.path.join(tmp, 'r%d.npz' % rank), rows=rows, gyro=got['ref_gyro'], lo=lo, hi=hi, merged=merged)
     td.destroy_process_group()
 
 
-def test_two_rank_statistics_over_gloo(tmp_path):
+def test_two_rank_merge_gather_and_broadcast_over_gloo(tmp_path):
     import torch.multiprocessing as mp
     port = 29500 + (os.getpid() % 2000)
     mp.spawn(_gloo_worker, args=(2, port, str(tmp_path)), nprocs=2, join=True)
@@ -316,10 +311,6 @@ def test_two_rank_statistics_over_gloo(tmp_path):
     gyro0 = None
     for r in range(2):
         z = np.load(os.path.join(str(tmp_path), 'r%d.npz' % r))
-        assert int(z['tot']) == 1001
-        assert_close(z['mean'], err.mean(0), 1e-12, 1e-12, 'mean')
-        assert_close(z['mx'], np.abs(err).max(0), 0.0, 0.0, 'max')
-        assert_close(z['std'], err.std(0), 1e-12, 0.0, 'std')
         assert np.array_equal(z['rows'], err)
         assert_close(z['merged'], np.stack([np.abs(err).max(0), err.mean(0), err.std(0)]), 1e-12, 1e-12,
                      'one-collective merge')
