@@ -18,6 +18,7 @@
 #include "mag_kernel.cuh"
 #include "ekf_kernel.cuh"
 #include "stats_kernel.cuh"
+#include "sensor_stats_kernel.cuh"
 
 #ifdef B2INS_SINGLE_TU
 #define B2_RF 0
@@ -243,6 +244,77 @@ struct Stream {
   cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
 };
 
+// K1's parameters and time segmentation, shared by K1 and K9; with segments, pass 1 and the carry chain are
+// launched here and *scratch holds their buffers (freed by the caller after its pass-0 launch).
+int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
+                  const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
+                  const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, cudaStream_t s, NoiseParams* out,
+                  double** out_scratch) {
+  NoiseParams& p = *out;
+  std::memset(&p, 0, sizeof(p));
+  p.n = n;
+  p.runs = runs;
+  p.run_offset = run_offset;
+  p.dt = 1.0 / fs;
+  p.k0 = static_cast<uint32_t>(seed);
+  p.k1 = static_cast<uint32_t>(seed >> 32);
+  int rc = digest_triad(gyro_err, vib_gyro, fs, &p.gyro);
+  if (rc != B2INS_OK) return rc;
+  rc = digest_triad(accel_err, vib_accel, fs, &p.accel);
+  if (rc != B2INS_OK) return rc;
+  p.ref_gyro = ref_gyro;
+  p.ref_accel = ref_accel;
+  // Few runs and a long series (the Allan configuration): split the time axis into segments so
+  // that every SM has work.  The Gauss-Markov state at a segment start needs the draws before it:
+  // pass 1 reduces every segment to its zero-state end value, a tiny serial kernel chains them,
+  // pass 0 regenerates (counter-based Philox: nothing is stored) and writes.  Costs the noise
+  // twice, so it is only used when one CTA per run would leave most of the GPU idle.
+  int nseg = 1;
+  const int64_t want_ctas = static_cast<int64_t>(sm_count()) * 2;
+  if (runs < want_ctas && n >= (int64_t(1) << 18)) {
+    nseg = static_cast<int>((want_ctas + runs - 1) / runs);
+    const int64_t max_seg = n / (int64_t(1) << 16);
+    if (nseg > max_seg) nseg = static_cast<int>(max_seg);
+    if (nseg < 1) nseg = 1;
+  }
+  p.nseg = nseg;
+  p.seg_len = n;
+  p.pass = 0;
+  p.seg_carry = nullptr;
+  p.seg_end = nullptr;
+  double* scratch = nullptr;
+  if (nseg > 1) {
+    int64_t len = (n + nseg - 1) / nseg;
+    len = (len + kNoiseTile - 1) / kNoiseTile * kNoiseTile;   // whole tiles per segment
+    p.seg_len = len;
+    p.nseg = static_cast<int>((n + len - 1) / len);
+    CU_CHECK(cudaMallocAsync(&scratch, sizeof(double) * runs * p.nseg * 12, s));
+    *out_scratch = scratch;        // the caller frees it, also when a launch below fails
+    p.seg_end = scratch;
+    p.seg_carry = scratch + runs * p.nseg * 6;
+    // pass 1 only needs the drives that still matter at the segment end: a^L < 1e-20
+    int64_t keep = 1;
+    for (int c = 0; c < 6; ++c) {
+      const double a = (c < 3) ? p.accel.gm_a[c] : p.gyro.gm_a[c - 3];
+      if (a >= 1.0) {
+        keep = len;
+      } else if (a > 0.0) {
+        const double need = std::ceil(std::log(1e-20) / std::log(a));
+        if (need > static_cast<double>(keep)) keep = need >= static_cast<double>(len) ? len : static_cast<int64_t>(need);
+      }
+    }
+    keep = (keep + kNoiseTile - 1) / kNoiseTile * kNoiseTile;
+    p.pass1_len = keep < len ? keep : len;
+    p.pass = 1;
+    if (p.nseg > 1)
+      imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
+    noise_carry_kernel<<<static_cast<unsigned>((runs * 6 + 127) / 128), 128, 0, s>>>(p);
+    p.pass = 0;
+  }
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -403,72 +475,79 @@ int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n, const double* ref_gy
   ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && gyro && accel, "null buffer");
   ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
   NoiseParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.n = n;
-  p.runs = runs;
-  p.run_offset = run_offset;
-  p.dt = 1.0 / fs;
-  p.k0 = static_cast<uint32_t>(seed);
-  p.k1 = static_cast<uint32_t>(seed >> 32);
-  int rc = digest_triad(gyro_err, vib_gyro, fs, &p.gyro);
-  if (rc != B2INS_OK) return rc;
-  rc = digest_triad(accel_err, vib_accel, fs, &p.accel);
-  if (rc != B2INS_OK) return rc;
-  p.ref_gyro = ref_gyro;
-  p.ref_accel = ref_accel;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  double* scratch = nullptr;
+  int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset,
+                         s, &p, &scratch);
+  if (rc != B2INS_OK) {
+    if (scratch) cudaFreeAsync(scratch, s);
+    return rc;
+  }
   p.out_gyro = gyro;
   p.out_accel = accel;
   layout_strides(layout, runs, n, &p.osr, &p.ost, &p.osc);
   p.z_dump = z_dump;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // Few runs and a long series (the Allan configuration): split the time axis into segments so
-  // that every SM has work.  The Gauss-Markov state at a segment start needs the draws before it:
-  // pass 1 reduces every segment to its zero-state end value, a tiny serial kernel chains them,
-  // pass 0 regenerates (counter-based Philox: nothing is stored) and writes.  Costs the noise
-  // twice, so it is only used when one CTA per run would leave most of the GPU idle.
-  int nseg = 1;
-  const int64_t want_ctas = static_cast<int64_t>(sm_count()) * 2;
-  if (runs < want_ctas && n >= (int64_t(1) << 18)) {
-    nseg = static_cast<int>((want_ctas + runs - 1) / runs);
-    const int64_t max_seg = n / (int64_t(1) << 16);
-    if (nseg > max_seg) nseg = static_cast<int>(max_seg);
-    if (nseg < 1) nseg = 1;
-  }
-  p.nseg = nseg;
-  p.seg_len = n;
-  p.pass = 0;
-  p.seg_carry = nullptr;
-  p.seg_end = nullptr;
-  double* scratch = nullptr;
-  if (nseg > 1) {
-    int64_t len = (n + nseg - 1) / nseg;
-    len = (len + kNoiseTile - 1) / kNoiseTile * kNoiseTile;   // whole tiles per segment
-    p.seg_len = len;
-    p.nseg = static_cast<int>((n + len - 1) / len);
-    CU_CHECK(cudaMallocAsync(&scratch, sizeof(double) * runs * p.nseg * 12, s));
-    p.seg_end = scratch;
-    p.seg_carry = scratch + runs * p.nseg * 6;
-    // pass 1 only needs the drives that still matter at the segment end: a^L < 1e-20
-    int64_t keep = 1;
-    for (int c = 0; c < 6; ++c) {
-      const double a = (c < 3) ? p.accel.gm_a[c] : p.gyro.gm_a[c - 3];
-      if (a >= 1.0) {
-        keep = len;
-      } else if (a > 0.0) {
-        const double need = std::ceil(std::log(1e-20) / std::log(a));
-        if (need > static_cast<double>(keep)) keep = need >= static_cast<double>(len) ? len : static_cast<int64_t>(need);
-      }
-    }
-    keep = (keep + kNoiseTile - 1) / kNoiseTile * kNoiseTile;
-    p.pass1_len = keep < len ? keep : len;
-    p.pass = 1;
-    if (p.nseg > 1)
-      imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
-    noise_carry_kernel<<<static_cast<unsigned>((runs * 6 + 127) / 128), 128, 0, s>>>(p);
-    p.pass = 0;
-  }
   imu_noise_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p);
   if (scratch) CU_CHECK(cudaFreeAsync(scratch, s));
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+// ---------------------------------------------------------------- K9 --------
+int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
+                            const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                            const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
+                            int64_t stats_start, double* end_err, double* proc_stats, void* stream) {
+  ARG_CHECK(fs > 0.0, "fs must be positive");
+  ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
+  ARG_CHECK(stats_start < n || n == 0, "stats_start must be < n");
+  if (runs == 0 || n == 0) return B2INS_OK;
+  ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && end_err, "null buffer");
+  ARG_CHECK(stats_start < 0 || proc_stats, "stats_start >= 0 needs proc_stats");
+  ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
+  ErrStatsParams P;
+  std::memset(&P, 0, sizeof(P));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  double* scratch = nullptr;
+  int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset,
+                         s, &P.np, &scratch);
+  if (rc != B2INS_OK) {
+    if (scratch) cudaFreeAsync(scratch, s);
+    return rc;
+  }
+  P.stats_start = stats_start;
+  P.end_err = end_err;
+  P.proc_stats = proc_stats;
+  double* partial = nullptr;
+  if (P.np.nseg > 1 && stats_start >= 0) {
+    const cudaError_t e = cudaMallocAsync(&partial, sizeof(double) * runs * P.np.nseg * kErrPartial, s);
+    if (e != cudaSuccess) {
+      if (scratch) cudaFreeAsync(scratch, s);
+      return fail(B2INS_ERR_CUDA, "cudaMallocAsync of the segment partials: %s", cudaGetErrorString(e));
+    }
+    P.partial = partial;
+  }
+  imu_err_stats_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P);
+  if (partial) {
+    err_stats_fold_kernel<<<static_cast<unsigned>((runs * kErrCh + 127) / 128), 128, 0, s>>>(P);
+    CU_CHECK(cudaFreeAsync(partial, s));
+  }
+  if (scratch) CU_CHECK(cudaFreeAsync(scratch, s));
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+// ---------------------------------------------------------------- K3p -------
+int b2ins_proc_stats_f64(int64_t runs, int64_t m, int ncomp, const double* x, const double* ref, int64_t start,
+                         double* end_err, double* proc_stats, void* stream) {
+  ARG_CHECK(runs >= 0 && m >= 0, "runs and m must be non-negative");
+  ARG_CHECK(ncomp >= 1 && ncomp <= kProcMaxComp, "ncomp must be in 1..%d, got %d", kProcMaxComp, ncomp);
+  ARG_CHECK(start >= 0 && (start < m || m == 0), "start must be in [0, m)");
+  if (runs == 0 || m == 0) return B2INS_OK;
+  ARG_CHECK(x && ref && end_err && proc_stats, "null buffer");
+  ARG_CHECK(runs < (int64_t(1) << 31), "runs must be < 2^31");
+  proc_stats_kernel<<<static_cast<unsigned>(runs), kProcThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      m, ncomp, x, ref, start, end_err, proc_stats);
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }

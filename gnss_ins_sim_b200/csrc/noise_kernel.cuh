@@ -7,7 +7,8 @@
 // an affine scan over the 128 threads of a tile -- shuffles within a warp, four warp totals through
 // shared memory: ONE exchange per kNoisePer samples instead of one per sample -- after which every
 // thread adds a^q S to its samples and the tile leaves shared memory in the caller's layout with
-// coalesced stores.
+// coalesced stores.  imu_err_stats_kernel (K9, sensor_stats_kernel.cuh) repeats this kernel's tile loop
+// (generation, affine scan, carry) with the store replaced by a reduction: a change here goes there too.
 #pragma once
 #include "mc_kernel.cuh"
 

@@ -153,6 +153,40 @@ def mag_noise(runs, ref_mag, mag_err, seed, run_offset=0):
     return out
 
 
+def imu_err_stats(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0,
+                  vib_gyro=None, vib_accel=None, stats_start=-1):
+    """K9: error statistics of the measurements imu_noise would make, reduced inside the generator.
+    Returns end_err [R,6] (e = meas - ref at the last sample; accel x y z, gyro x y z) and, if
+    stats_start >= 0, proc_stats [R,3,6] (max|e|, mean, std over samples >= stats_start), else None."""
+    _require_cuda()
+    lib = _lib.load()
+    n = ref_gyro.shape[0]
+    dev = ref_gyro.device
+    end_err = torch.empty((runs, 6), dtype=torch.float64, device=dev)
+    proc = torch.empty((runs, 3, 6), dtype=torch.float64, device=dev) if stats_start >= 0 else None
+    ge, ae = _lib.sensor_err(gyro_err, 'arw'), _lib.sensor_err(accel_err, 'vrw')
+    vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
+    va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
+    _lib.check(lib.b2ins_imu_err_stats_f64(
+        float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
+        ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
+        _ptr(end_err), _ptr(proc), _stream()))
+    return end_err, proc
+
+
+def proc_stats(x, ref, start):
+    """K3p: x CUDA f64 [R,m,C], ref [m,C] -> end_err [R,C] (x - ref at row m-1) and proc_stats
+    [R,3,C] (max|e|, mean, std over rows >= start)."""
+    _require_cuda()
+    lib = _lib.load()
+    R, m, C = x.shape
+    end_err = torch.empty((R, C), dtype=torch.float64, device=x.device)
+    proc = torch.empty((R, 3, C), dtype=torch.float64, device=x.device)
+    _lib.check(lib.b2ins_proc_stats_f64(R, m, C, _ptr(x), _ptr(ref), int(start), _ptr(end_err), _ptr(proc),
+                                        _stream()))
+    return end_err, proc
+
+
 class McResult:
     """Device-side results of one fused Monte-Carlo launch."""
 

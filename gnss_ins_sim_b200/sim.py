@@ -321,6 +321,30 @@ _UNITS = {  # name -> (description, units, output units)   ins_data_manager.py:8
 }
 
 
+_SENSOR_UNITS = {  # sensor data with a ref_ counterpart -> (units, output units), ins_data_manager.py:96-143
+    'gyro': (['rad/s'] * 3, ['deg/s'] * 3),
+    'accel': (['m/s^2'] * 3, ['m/s^2'] * 3),
+    'mag': (['uT'] * 3, ['uT'] * 3),
+    'gps': (['rad', 'rad', 'm', 'm/s', 'm/s', 'm/s'], ['deg', 'deg', 'm', 'm/s', 'm/s', 'm/s']),
+}
+_REF_OF = {'att_euler': 'ref_att', 'pos': 'ref_pos', 'vel': 'ref_vel'}   # trajectory key of an output's truth
+
+
+def _first_at(t, start_s):
+    """Index of the first time >= start_s; past the end: the reference's message and 0
+    (ins_data_manager.py:774-782)."""
+    idx = np.where(np.asarray(t) >= start_s)[0]
+    if idx.shape[0] == 0:
+        print('err_stats_start exceeds max data points.')
+        return 0
+    return int(idx[0])
+
+
+def _host_stats(e):
+    """InsDataMgr.__array_stats (ins_data_manager.py:797-808) over axis 0."""
+    return np.stack([np.max(np.abs(e), 0), np.average(e, 0), np.std(e, 0)])
+
+
 class Sim(object):
     '''
     INS Monte-Carlo simulation engine (device-backed).
@@ -427,6 +451,7 @@ class Sim(object):
             raise ValueError('imu must be an IMU model when data are generated from a trajectory')
         self._blocks = {}        # (block, name) -> [runs of the block, ...] host histories (_history)
         self._proc = {}          # (algo index, start [s], position frame) -> [R, 3, 9] process statistics
+        self._sens = {}          # (source, first row) -> sensor error statistics (_sensor_launch)
         self._all_hist = None    # (algo index, first run, arrays) of the last histories() with stride 1
         self.err_stats = {}
         self._mc = {}
@@ -494,7 +519,7 @@ class Sim(object):
         """Algorithms on the logged sets 0 .. sim_count-1 (InsAlgoMgr.run_algo over the keys,
         ins_algo_manager.py:73-95): one batched launch per algorithm, outputs keyed
         '<algo>_<key>'; end-point error statistics if the directory has the reference files."""
-        self._proc, self.err_stats, self._mc = {}, {}, {}
+        self._proc, self.err_stats, self._mc, self._sens = {}, {}, {}, {}
         self._shard = (0, self.sim_count)
         d = self._logged
         for i, a in enumerate(self.algo or []):
@@ -921,36 +946,61 @@ class Sim(object):
     def get_error_stats(self, data_name, err_stats_start=-1, angle=False, use_output_units=False,
                         extra_opt='', algo_index=0):
         '''
-        InsDataMgr.get_error_stats (ins_data_manager.py:385-452) for att_euler / pos / vel.
-        err_stats_start == -1: end-point statistics over runs {'max','avg','std'} (3,).
-        otherwise: per-run process statistics from that time [s]: dicts keyed by run key.
+        InsDataMgr.get_error_stats (ins_data_manager.py:385-452) for att_euler / pos / vel of an algorithm and
+        for the sensor data gyro / accel / mag / gps.
+        err_stats_start == -1: end-point statistics over runs {'max','avg','std'} (3,) (sensor data: (3,) or
+        (6,)).  Otherwise: per-run process statistics from that time [s]: dicts keyed by run key ('<algo>_<r>'
+        for algorithm outputs, the run index for sensor data).  GPS process statistics start at the first
+        GPS sample at or after that time.
         '''
+        if data_name == 'odo':
+            raise ValueError('odo has no error statistics: the odometer history is one column per run, and the '
+                             "reference's own end-point statistics index it as a 2-D array "
+                             '(ins_data_manager.py:737), so there is no defined result')
+        if data_name in _SENSOR_UNITS:
+            units, out_units = _SENSOR_UNITS[data_name]
+            if data_name == 'gps' and self.ref_frame == 1:      # ins_data_manager.py:221-230
+                units = out_units = ['m', 'm', 'm', 'm/s', 'm/s', 'm/s']
+            st = self._sensor_stats(data_name, err_stats_start)
+            return self._with_units(st, units, out_units, use_output_units)
         if data_name not in _UNITS:
-            raise ValueError('error statistics exist for att_euler, pos and vel')
+            raise ValueError('error statistics exist for att_euler, pos, vel, gyro, accel, mag and gps')
         c0 = {'att_euler': 0, 'pos': 3, 'vel': 6}[data_name]
         desc, units, out_units = _UNITS[data_name]
         if data_name == 'pos' and self.ref_frame == 1:
             units, out_units = ['m'] * 3, ['m'] * 3
         name = self.algo_name(algo_index)
-        if err_stats_start == -1:
-            if data_name == 'pos' and self.ref_frame == 0 and extra_opt in ('ned', 'ecef'):
+        # extra_opt 'ned' / 'ecef' in ref_frame 0: position error in metres (ignored in ref_frame 1, as in
+        # the reference).  The reference keeps the first option's error array per data name
+        # (ins_data_manager.py:427-431); here every call gets the option it asks for.
+        frame = {'ned': engine.POS_FRAME_NED, 'ecef': engine.POS_FRAME_ECEF}.get(extra_opt, 0) \
+            if self.ref_frame == 0 else 0
+        if data_name == 'pos' and frame:
+            units = out_units = ['m'] * 3
+        if algo_index not in self._mc:
+            # a reference-style plugin: its outputs are on the host
+            errs, starts = zip(*(self._host_error(algo_index, r, data_name, frame) for r in range(self.sim_count)))
+            if err_stats_start == -1:
+                st = dict(zip(('max', 'avg', 'std'), _host_stats(np.stack([e[-1] for e in errs]))))
+            else:
+                ps = [_host_stats(e[_first_at(t, err_stats_start):]) for e, t in zip(errs, starts)]
+                st = {s: _keyed(name, [p[k] for p in ps]) for k, s in enumerate(('max', 'avg', 'std'))}
+        elif err_stats_start == -1:
+            if frame:
                 st = self._end_point_pos_stats(extra_opt, algo_index)
-                units = out_units = ['m'] * 3
             else:
                 s = self.err_stats[name]
                 st = {'max': s[0, c0:c0 + 3].copy(), 'avg': s[1, c0:c0 + 3].copy(),
                       'std': s[2, c0:c0 + 3].copy()}
         else:
-            # extra_opt 'ned' / 'ecef' in ref_frame 0: position error in metres (ignored in ref_frame 1, as in
-            # the reference).  The reference keeps the first option's error array per data name
-            # (ins_data_manager.py:427-431); here every call gets the option it asks for.
-            frame = {'ned': engine.POS_FRAME_NED, 'ecef': engine.POS_FRAME_ECEF}.get(extra_opt, 0) \
-                if self.ref_frame == 0 else 0
             st = self._process_stats(algo_index, err_stats_start, c0, frame)
-            if data_name == 'pos' and frame:
-                units = out_units = ['m'] * 3
+        return self._with_units(st, units, out_units, use_output_units)
+
+    @staticmethod
+    def _with_units(st, units, out_units, use_output_units):
+        """The statistics in output units on request (sim_data.convert_unit: rad -> deg), with the units string."""
         if use_output_units:
-            scale = np.array([R2D if (u == 'rad' and o == 'deg') else 1.0
+            scale = np.array([R2D if (u, o) in (('rad', 'deg'), ('rad/s', 'deg/s')) else 1.0
                               for u, o in zip(units, out_units)])
             for k in ('max', 'avg', 'std'):
                 if isinstance(st[k], dict):
@@ -961,6 +1011,110 @@ class Sim(object):
         else:
             st['units'] = str(units)
         return st
+
+    def _host_error(self, ai, r, data_name, frame=0):
+        """(e, t) of run r of a host-held output of algorithm ai (logged-data results, reference-style plugins):
+        e = x - truth as calc_data_err / array_error make it (ins_data_manager.py:454-553) -- att_euler wrapped
+        to [-pi, pi], pos in NED / ECEF metres for frame 1 / 2, the truth interpolated to the plugin's algo_time
+        when the row counts differ (:497-506) -- and the times of its rows (algo_time if the plugin outputs it,
+        :774-777)."""
+        key = '%s_%d' % (self.algo_name(ai), r)
+        x = np.asarray(self.data[data_name][key], dtype=np.float64)
+        ref = self._traj[_REF_OF[data_name]]
+        at = self.data.get('algo_time')
+        t = np.asarray(at[key], dtype=np.float64) if isinstance(at, Mapping) and key in at else None
+        if ref.shape[0] != x.shape[0]:
+            if t is None:
+                raise ValueError('%s of %s has %d rows and its truth %d: interpolating needs algo_time'
+                                 % (data_name, key, x.shape[0], ref.shape[0]))
+            ref = np.stack([np.interp(t, self.data['time'], ref[:, i]) for i in range(ref.shape[1])], axis=1)
+        if data_name == 'att_euler':
+            e = (x - ref + math.pi) % (2.0 * math.pi) - math.pi
+        elif data_name == 'pos' and frame:
+            e = lla_error_metres(x, ref, frame)
+        else:
+            e = x - ref
+        return e, (self.data['time'] if t is None else t)
+
+    # ---- sensor-data error statistics (K9 for gyro / accel, K8 / K6 + K3p for mag / gps) ------------
+    def _sensor_stats(self, name, start_s):
+        """get_error_stats of gyro / accel / mag / gps: end-point statistics over runs (start_s == -1) or
+        per-run process statistics keyed by run index."""
+        if name not in self.data:
+            raise ValueError('%s is not available in this simulation' % name)
+        if self._logged is not None:
+            return self._logged_sensor_stats(name, start_s)
+        src, cols = {'gyro': ('imu', slice(3, 6)), 'accel': ('imu', slice(0, 3)),
+                     'mag': ('mag', slice(0, 3)), 'gps': ('gps', slice(0, 6))}[name]
+        if start_s == -1:
+            hit = next((v for k, v in self._sens.items() if k[0] == src), None)
+            end_err, _ = hit if hit is not None else self._sensor_launch(src, -1)
+            lo, hi = self._shard
+            stats = np.zeros((3, cols.stop - cols.start))
+            if hi > lo:
+                stats = engine.error_stats(engine.to_device(end_err[:, cols])).cpu().numpy()
+            stats = dist.combine_local_stats(stats, hi - lo)
+            return {'max': stats[0], 'avg': stats[1], 'std': stats[2]}
+        t = self._traj['gps_time'] if name == 'gps' else self.data['time']
+        start = _first_at(t, start_s)
+        if (src, start) not in self._sens:
+            self._sensor_launch(src, start)
+        ps = self._sens[(src, start)][1][:, :, cols]
+        return {s: {r: ps[r, k].copy() for r in range(ps.shape[0])} for k, s in enumerate(('max', 'avg', 'std'))}
+
+    def _sensor_launch(self, src, start):
+        """This rank's runs of one source ('imu', 'mag', 'gps') reduced from row `start` (-1: end points only):
+        caches and returns (end_err [R_local, C], process statistics [R, 3, C] of all ranks or None).  The IMU
+        is one K9 launch (in run blocks only with PSD vibration, whose series K5 materialises); mag and gps
+        are materialised by K8 / K6 in run blocks sized to the free device memory and reduced by K3p."""
+        lo, hi = self._shard
+        d = self._dev
+        C = {'imu': 6, 'mag': 3, 'gps': 6}[src]
+        if src == 'imu':
+            block = self._allan_block(48, 3) if self._uses_psd() else max(hi - lo, 1)
+        else:
+            block = self._allan_block(8 * C, 3)
+        ends, procs = [], []
+        for r0 in range(lo, hi, block):
+            runs = min(hi, r0 + block) - r0
+            if src == 'imu':
+                vib_gyro, vib_acc = self._vib_pair(runs, r0)
+                e, p = engine.imu_err_stats(self.fs[0], runs, d['ref_gyro'], d['ref_accel'], self.imu.gyro_err,
+                                            self.imu.accel_err, self.seed, run_offset=self.run_base + r0,
+                                            vib_gyro=vib_gyro, vib_accel=vib_acc, stats_start=start)
+            else:
+                ref = d['ref_mag'] if src == 'mag' else d['ref_gps']
+                if src == 'mag':
+                    x = engine.mag_noise(runs, ref, self.imu.mag_err, self.seed, run_offset=self.run_base + r0)
+                else:
+                    x = engine.gps_noise(runs, ref, self.imu.gps_err, self.ref_frame, self.seed,
+                                         run_offset=self.run_base + r0)
+                e, p = engine.proc_stats(x, ref, max(start, 0))
+                del x
+            ends.append(e)
+            procs.append(p)
+        end_err = torch.cat(ends).cpu().numpy() if ends else np.zeros((0, C))
+        proc = None
+        if start >= 0:
+            local = torch.cat(procs).reshape(hi - lo, 3 * C) if procs else None
+            proc = dist.gather_rows(local, self.sim_count).reshape(-1, 3, C)
+        self._sens[(src, start)] = (end_err, proc)
+        return self._sens[(src, start)]
+
+    def _logged_sensor_stats(self, name, start_s):
+        """The statistics of a logged directory's <name>-<key>.csv sets against ref_<name>.csv, on the host."""
+        ref = self._logged.get('ref_' + name)
+        if ref is None:
+            raise ValueError('the data directory holds no ref_%s.csv' % name)
+        x = self._logged_sets(name)
+        e = x - ref[None]
+        if start_s == -1:
+            return dict(zip(('max', 'avg', 'std'), _host_stats(e[:, -1])))
+        t = self._logged.get('gps_time') if name == 'gps' else self.data['time']
+        if t is None:
+            raise ValueError('the data directory holds no gps_time.csv')
+        ps = [_host_stats(er[_first_at(t, start_s):]) for er in e]
+        return {s: {r: p[k] for r, p in enumerate(ps)} for k, s in enumerate(('max', 'avg', 'std'))}
 
     def _end_point_pos_stats(self, opt, algo_index):
         """'ned' / 'ecef' position error of LLA results, ins_data_manager.py:543-552."""
@@ -982,26 +1136,15 @@ class Sim(object):
             key = next((k for k in ((algo_index, float(start_s), f) for f in (frame, 0, 1, 2))
                         if k in self._proc), key)
         if key not in self._proc:
-            idx = np.where(self.data['time'] >= start_s)[0]
-            if idx.shape[0] == 0:
-                print('err_stats_start exceeds max data points.')
-                start = 0
-            else:
-                start = int(idx[0])
+            start = _first_at(self.data['time'], start_s)
             if self._logged is not None:
                 # the histories are on the host already (array_error + __array_stats,
                 # ins_data_manager.py:512-541, :797-808)
-                nm = self.algo_name(algo_index)
                 ps = np.zeros((self.sim_count, 3, 9))
                 for r in range(self.sim_count):
-                    k = '%s_%d' % (nm, r)
-                    pos, ref_pos = self.data['pos'][k], self._logged['ref_pos']
-                    e = np.concatenate([
-                        (self.data['att_euler'][k] - self._logged['ref_att_euler'] + math.pi) % (2.0 * math.pi)
-                        - math.pi,
-                        lla_error_metres(pos, ref_pos, frame) if frame else pos - ref_pos,
-                        self.data['vel'][k] - self._logged['ref_vel']], axis=1)[start:]
-                    ps[r] = np.stack([np.max(np.abs(e), 0), np.average(e, 0), np.std(e, 0)])
+                    e = np.concatenate([self._host_error(algo_index, r, dn, frame)[0]
+                                        for dn in ('att_euler', 'pos', 'vel')], axis=1)[start:]
+                    ps[r] = _host_stats(e)
             else:
                 lo, hi = self._shard
                 ps = None
@@ -1031,12 +1174,19 @@ class Sim(object):
         s += 'Reference frame: %s\n' % str(self.ref_frame)
         s += 'Simulation time duration: %s s\n' % str(len(self.data['time']) / self.fs[0])
         s += 'Simulation runs: %s\n' % str(self.sim_count)
-        has_mc = bool(self._mc) and bool(self.err_stats)   # logged data may lack references
-        if has_mc:
+        names = []
+        if self._mc and self.err_stats:      # logged data may lack references
+            ai, names = sorted(self._mc.keys())[0], ['att_euler', 'pos', 'vel']
+        else:   # reference-style plugins only: the first one that outputs att_euler / pos / vel with a truth
+            for i, a in enumerate(self.algo or []):
+                got = [dn for dn in _REF_OF if dn in a.output and _REF_OF[dn] in (self._traj or {})]
+                if i not in self._mc and got:
+                    ai, names = i, got
+                    break
+        if names:
             s += '\n------------------------------------------------------------\n'
             s += 'The following are error statistics.'
-            ai = sorted(self._mc.keys())[0]
-            for dn in ('att_euler', 'pos', 'vel'):
+            for dn in names:
                 st = self.get_error_stats(dn, err_stats_start=err_stats_start,
                                           angle=(dn == 'att_euler'), use_output_units=True,
                                           extra_opt=extra_opt, algo_index=ai)

@@ -376,6 +376,30 @@ int b2ins_mag_noise_f64(int64_t runs, int64_t n, const double* ref_mag, const do
                         const double* hi, const double* std, uint64_t seed, int64_t run_offset,
                         double* mag, void* stream);
 
+/* ---- K9: IMU error statistics, reduced inside the noise generator ---------------------
+ * InsDataMgr.get_error_stats('gyro' | 'accel') (ins_data_manager.py:385-452, :524-541, :717-808) for
+ * `runs` runs without materialising them: the measurements of b2ins_imu_noise_f64 (same arguments, same
+ * Philox draws, the same values) minus the truth, e = meas - ref, reduced per run.
+ *   end_err [runs][6] (device): e at sample n-1; columns accel x, y, z, then gyro x, y, z.
+ *   proc_stats [runs][3][6] (device; may be NULL when stats_start < 0): max|e|, mean and std (ddof 0)
+ *       over samples >= stats_start, same columns.
+ * stats_start < 0: end_err only; otherwise stats_start < n.  Deterministic (fixed-order reductions, no
+ * floating-point atomics).  Asynchronous on `stream`. */
+int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n,
+                            const double* ref_gyro, const double* ref_accel,
+                            const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                            const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                            uint64_t seed, int64_t run_offset, int64_t stats_start,
+                            double* end_err, double* proc_stats, void* stream);
+
+/* ---- K3p: per-run error statistics of a device array ----------------------------------
+ * x [runs][m][ncomp] against the shared ref [m][ncomp] (device), e = x - ref:
+ *   end_err [runs][ncomp]: e at row m-1;
+ *   proc_stats [runs][3][ncomp]: max|e|, mean and std (ddof 0) over rows >= start (0 <= start < m).
+ * 1 <= ncomp <= 8.  Deterministic.  Asynchronous on `stream`. */
+int b2ins_proc_stats_f64(int64_t runs, int64_t m, int ncomp, const double* x, const double* ref,
+                         int64_t start, double* end_err, double* proc_stats, void* stream);
+
 /* ---- host: true-trajectory generator -----------------------------------------------
  * Replaces pathgen.path_gen (gnss_ins_sim/pathgen/pathgen.py:26-329, with
  * calc_true_sensor_output :331-411 and parse_motion_def :413-439).  Plain CPU code (the

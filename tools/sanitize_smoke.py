@@ -75,7 +75,12 @@ def main():
     ref_gps = engine.to_device(np.tile(np.array([0.5, 2.0, 10.0, 1.0, 0.0, 0.0]), (50, 1)))
     engine.gps_noise(7, ref_gps, {'stdp': np.ones(3), 'stdv': np.ones(3)}, 0, 3)
     ref_mag = engine.to_device(np.tile(np.array([20.0, -3.0, 40.0]), (51, 1)))
-    engine.mag_noise(9, ref_mag, {'si': np.eye(3), 'hi': np.ones(3), 'std': np.full(3, 0.5)}, 5, 3)
+    mag = engine.mag_noise(9, ref_mag, {'si': np.eye(3), 'hi': np.ones(3), 'std': np.full(3, 0.5)}, 5, 3)
+    # K9 (plain, end points only, time-segmented) and K3p
+    engine.imu_err_stats(100.0, 5, rg, ra, MID_G, MID_A, 1, stats_start=250)
+    engine.imu_err_stats(100.0, 5, rg, ra, MID_G, MID_A, 1)
+    engine.imu_err_stats(100.0, 1, long_g, long_g, MID_G, MID_A, 1, stats_start=1000)
+    engine.proc_stats(mag, ref_mag, 7)
     torch.cuda.synchronize()
     print('sanitize smoke ok')
 
