@@ -900,6 +900,15 @@ int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, con
                         const double* gps_vis, double* end_err, double* end_bias, double* consist,
                         double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb,
                         double* dump_ab, void* stream) {
+  return b2ins_ins_loose_ex_f64(cfg, nullptr, nullptr, ref_gyro, ref_accel, ref_nav, ref_gps, gps_idx, gps_vis,
+                                end_err, end_bias, consist, dump_att, dump_pos, dump_vel, dump_wb, dump_ab, stream);
+}
+
+int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                           const double* ref_gyro, const double* ref_accel, const double* ref_nav,
+                           const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
+                           double* end_bias, double* consist, double* dump_att, double* dump_pos,
+                           double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
   ARG_CHECK(cfg, "cfg is null");
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
@@ -922,9 +931,9 @@ int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, con
   p.earth_rot = cfg->earth_rot;
   p.k0 = static_cast<uint32_t>(cfg->seed);
   p.k1 = static_cast<uint32_t>(cfg->seed >> 32);
-  int rc = digest_triad(&cfg->gyro_err, nullptr, cfg->fs, &p.gyro);
+  int rc = digest_triad(&cfg->gyro_err, vib_gyro, cfg->fs, &p.gyro);
   if (rc != B2INS_OK) return rc;
-  rc = digest_triad(&cfg->accel_err, nullptr, cfg->fs, &p.accel);
+  rc = digest_triad(&cfg->accel_err, vib_accel, cfg->fs, &p.accel);
   if (rc != B2INS_OK) return rc;
   p.ref_gyro = ref_gyro;
   p.ref_accel = ref_accel;
@@ -966,7 +975,10 @@ int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, con
   p.dump_stride = cfg->dump_stride > 1 ? cfg->dump_stride : 1;
   p.dump_rows = (cfg->n + p.dump_stride - 1) / p.dump_stride;
   const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
-  ekf_kernel<<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  if (p.gyro.vib_type == B2INS_VIB_NONE && p.accel.vib_type == B2INS_VIB_NONE)
+    ekf_kernel<false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  else
+    ekf_kernel<true><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }

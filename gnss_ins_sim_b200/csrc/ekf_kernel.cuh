@@ -118,6 +118,10 @@ __device__ __forceinline__ int ekf_own(int q, int m) {
   return (q < 3) ? 3 * blk + q : ((m < 3) ? 9 + m : 9);
 }
 
+// VIB: the vibration models of p.accel / p.gyro (vib_term's, added last to each measurement) are compiled
+// in; the launch picks ekf_kernel<false> when both vib_types are B2INS_VIB_NONE, so that instantiation is
+// the filter without any vibration code.
+template <bool VIB>
 __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant__ EkfParams p) {
   __shared__ double Psm[kEkfN * kEkfN * kEkfRuns];      // 14.4 KB
   const int lane = threadIdx.x;
@@ -191,6 +195,21 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   model(c0, &b0, &w0, &wd0, &ga0, &gb0);
   model(two ? c1 : c0, &b1, &w1, &wd1, &ga1, &gb1);
   double carry0 = 0.0, carry1 = 0.0;                              // d[i] of the lane's channels
+  // vibration (VIB only) of the lane's accelerometer channel (axis q, lanes 0..2) and gyro channel (c0 of
+  // lane 3: x; c1 of lanes 0 and 1: y, z; lane 2 computes axis z and drops it): amplitude, the PSD model's
+  // row of the series, the sinusoidal model's random gyro phase
+  const int vax = q < 3 ? q : 0, vgx = q == 3 ? 0 : (q < 2 ? q + 1 : 2);
+  double vamp_a = 0.0, vamp_g = 0.0, vphase = 0.0;
+  const double* vser_a = nullptr;
+  const double* vser_g = nullptr;
+  if constexpr (VIB) {
+    vamp_a = p.accel.vib_amp[vax];
+    vamp_g = p.gyro.vib_amp[vgx];
+    if (p.accel.vib_type == 3) vser_a = p.accel.series + (run * 3 + vax) * p.accel.series_len;
+    if (p.gyro.vib_type == 3) vser_g = p.gyro.series + (run * 3 + vgx) * p.gyro.series_len;
+    if (p.gyro.vib_type == 2)
+      vphase = (uniform01(0xFFFFFFFFu, kDrawPhase + vgx, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
+  }
   double nees[3] = {0.0, 0.0, 0.0};
   int inside[kEkfN];
 #pragma unroll
@@ -349,6 +368,26 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
       const Normal2 z1 = normal_pair(t, static_cast<uint32_t>(cc), run_lo, run_hi, p.k0, p.k1);
       m1 = ((ref1[0] + b1) + w1 * z1.z1) + (carry1 + wd1 * z1.z0);
       carry1 = two ? fma(ga1, carry1, gb1 * z1.z0) : 0.0;
+      if constexpr (VIB) {
+        // vib_term's models (1 random, 2 sinusoidal, 3 series), added last as in oracle_np.sensor_gen.
+        // Random: lane q < 3 draws pair kDrawVib + q, whose z0 is its own accelerometer axis and whose z1
+        // (gyro axis q) belongs to lane (q + 3) & 3 -- one quad shuffle from lane (q + 1) & 3; lane 3's
+        // draw is dropped
+        const int ta = p.accel.vib_type, tg = p.gyro.vib_type;
+        double va = 0.0, vg = 0.0;
+        if ((ta == 1) | (tg == 1)) {
+          const Normal2 zv = normal_pair(t, kDrawVib + vax, run_lo, run_hi, p.k0, p.k1);
+          const double zvg = quad(zv.z1, (q + 1) & 3);
+          if (ta == 1) va = vamp_a * zv.z0;
+          if (tg == 1) vg = vamp_g * zvg;
+        }
+        if (ta == 2) va = vamp_a * sin(p.accel.vib_w * static_cast<double>(t) + 0.0);
+        if (tg == 2) vg = vamp_g * sin(p.gyro.vib_w * static_cast<double>(t) + vphase);
+        if (ta == 3) va = vser_a[t % static_cast<uint32_t>(p.accel.series_len)];
+        if (tg == 3) vg = vser_g[t % static_cast<uint32_t>(p.gyro.series_len)];
+        m0 += (q < 3) ? va : vg;
+        m1 += vg;
+      }
     }
     const Vec3 f{quad(m0, 0) - ba[0], quad(m0, 1) - ba[1], quad(m0, 2) - ba[2]};
     const Vec3 w{quad(m0, 3) - bg[0], quad(m1, 0) - bg[1], quad(m1, 1) - bg[2]};

@@ -460,11 +460,15 @@ class EkfResult:
 
 def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_accel, ref_nav, ref_gps,
               gps_idx, gps_vis, run_offset=0, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True,
-              stats_start=0, dump_runs=0, dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0):
+              stats_start=0, dump_runs=0, dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0,
+              vib_gyro=None, vib_accel=None):
     """K7: Monte-Carlo loosely-coupled GNSS/INS filter (the spec: DESIGN.md section 11; csrc/ekf_kernel.cuh).
     ref_gyro, ref_accel [n,3], ref_nav [n,9], ref_gps [m,6], gps_vis [m]: CUDA f64; gps_idx [m]: CUDA
     int64 (IMU sample index of every GPS row).  ini: the 9 true initial values (LLA, body velocity, Euler
-    angles).  Asynchronous on the current stream."""
+    angles).  vib_gyro / vib_accel: the vibration of the measurements the filter sees, as imu_noise takes
+    them (a parsed dict, or a Vib such as vib_series over K5 series of exactly these runs); the filter
+    model does not include it (vel_rw / att_rw, DESIGN.md section 11).  Asynchronous on the current
+    stream."""
     _require_cuda()
     lib = _lib.load()
     n, m = ref_gyro.shape[0], ref_gps.shape[0]
@@ -486,6 +490,9 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     cfg.stats_start, cfg.dump_runs, cfg.dump_stride = int(stats_start), int(dump_runs), int(dump_stride)
     cfg.earth_rot = int(bool(earth_rot))
     cfg.vel_rw, cfg.att_rw = float(vel_rw), float(att_rw)
+    # Vib structs are passed by pointer; a VIB_SERIES Vib keeps its series tensor alive through the call
+    vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
+    va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
     res = out or EkfResult()
     res.end_err = _reuse(res.end_err, (runs, 9), dev)
     res.end_bias = _reuse(res.end_bias, (runs, 6), dev)
@@ -496,8 +503,8 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
                                                      for k in ('att', 'pos', 'vel', 'wb', 'ab'))
     else:
         res.att = res.pos = res.vel = res.wb = res.ab = None
-    _lib.check(lib.b2ins_ins_loose_f64(
-        ctypes.byref(cfg), _ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps),
+    _lib.check(lib.b2ins_ins_loose_ex_f64(
+        ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), _ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps),
         ctypes.c_void_p(gps_idx.data_ptr()), _ptr(gps_vis), _ptr(res.end_err), _ptr(res.end_bias),
         _ptr(res.consist), _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream()))
     return res

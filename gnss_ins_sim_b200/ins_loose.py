@@ -35,6 +35,14 @@ class InsLoose(object):
                 random walks of the filter model.  The reference's truth generator and its first-order
                 mechanization disagree slightly (noise-free free integration of motion_def-ins.csv ends
                 0.37 m/s off); 0.02 m/s/sqrt(s) covers that and keeps the filter consistent.
+
+        Vibration: the measurements carry the Sim's env vibration (random, sinusoidal or PSD), as
+        get_data(['accel']) / get_data(['gyro']) do, but the filter model does not know about it.  Tell
+        it through these two random walks.  For white (random) vibration of 1-sigma sa [m/s^2] on the
+        accelerometer and sg [rad/s] on the gyro, sampled at dt = 1 / fs:
+            vel_model_std = sqrt(0.02**2 + sa**2 * dt),   att_model_std = sg * sqrt(dt)
+        (plus any att_model_std of its own, in quadrature).  With the default model the velocity and
+        attitude blocks become overconfident (DESIGN.md section 11 has the figures).
         '''
         self.input = ['fs', 'gyro', 'accel', 'time', 'gps_time', 'gps']   # ins_loose.py:31
         self.output = ['pos', 'vel', 'att_euler', 'wb', 'ab']             # ins_loose.py:32

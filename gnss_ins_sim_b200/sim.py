@@ -779,15 +779,18 @@ class Sim(object):
         ini = algo.ini if algo.ini is not None else self._traj.get('ini')
         if ini is None:
             raise ValueError('InsLoose needs ini_pos_vel_att (the trajectory carries no initial state)')
+        vib_gyro, vib_acc = self._vib_pair(runs, r0)       # K5 (PSD) runs on the stream K7 runs on
         return engine.ins_loose(self.fs[0], runs, self.seed, self.imu.gyro_err, self.imu.accel_err,
                                 self.imu.gps_err, ini, d['ref_gyro'], d['ref_accel'], d['ref_nav'],
                                 *gps, run_offset=self.run_base + r0,
                                 ini_att_std=algo.ini_att_std, earth_rot=algo.earth_rot,
                                 stats_start=stats_start, dump_runs=dump_runs, dump_stride=dump_stride,
-                                vel_rw=algo.vel_model_std, att_rw=algo.att_model_std)
+                                vel_rw=algo.vel_model_std, att_rw=algo.att_model_std,
+                                vib_gyro=vib_gyro, vib_accel=vib_acc)
 
     def _run_ins_loose(self, i, algo):
-        """demo_ins_loose.py semantics, all runs of this rank in one K7 launch: end-point errors and their
+        """demo_ins_loose.py semantics, all runs of this rank in one K7 launch (in run blocks sized to the free
+        device memory with PSD vibration, whose series K5 materialises, as for K9): end-point errors and their
         ensemble statistics (as for free integration), bias estimates, the consistency record."""
         name = self.algo_name(i)
         lo, hi = self._shard
@@ -795,9 +798,19 @@ class Sim(object):
         err, stats, con, bias = np.zeros((0, 9)), np.zeros((3, 9)), np.zeros((0, 19)), np.zeros((0, 6))
         if hi > lo:
             start = int(round(min(30.0, 0.1 * len(self.data['time']) / self.fs[0]) * self.fs[0]))
-            res = self._ekf_launch(algo, lo, hi - lo, stats_start=start)
-            stats = engine.error_stats(res.end_err).cpu().numpy()
-            err, con, bias = res.end_err.cpu().numpy(), res.consist.cpu().numpy(), res.end_bias.cpu().numpy()
+            block = self._allan_block(48, 3) if self._uses_psd() else hi - lo
+            parts = []
+            for r0 in range(lo, hi, block):
+                runs = min(hi, r0 + block) - r0
+                parts.append(self._ekf_launch(algo, r0, runs, stats_start=start))
+                if block < hi - lo:     # the next block's series take the memory of this block's
+                    for sensor in (0, 1):
+                        self._psd_cache.pop((sensor, runs, r0), None)
+            end_err = torch.cat([r.end_err for r in parts])
+            stats = engine.error_stats(end_err).cpu().numpy()
+            err = end_err.cpu().numpy()
+            con = torch.cat([r.consist for r in parts]).cpu().numpy()
+            bias = torch.cat([r.end_bias for r in parts]).cpu().numpy()
         self._mc[i].update({'end_err': err, 'consist': con, 'end_bias': bias})
         self.err_stats[name] = dist.combine_local_stats(stats, hi - lo)
         algo.run_times += self.sim_count

@@ -174,6 +174,19 @@ int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, con
                         double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb,
                         double* dump_ab, void* stream);
 
+/* b2ins_ins_loose_f64 on vibrating sensors: every run's accelerometer and gyro samples carry the
+ * vibration of vib_accel / vib_gyro (each nullable = none), added last, as b2ins_imu_noise_f64 adds it
+ * (pathgen.py:477-493, :540-555): the filter sees the measurements K1 makes for the same runs.
+ * VIB_SERIES: series [runs][3][series_len] on the device, for exactly the runs of this call (local run r
+ * reads row r), e.g. from b2ins_psd_series_f64 with the same run_offset, ordered before this call on
+ * `stream`.  The filter model itself knows nothing of the vibration (DESIGN.md section 11: raise vel_rw /
+ * att_rw by sigma sqrt(dt) for random vibration).  b2ins_ins_loose_f64 is the NULL / NULL case. */
+int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                           const double* ref_gyro, const double* ref_accel, const double* ref_nav,
+                           const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
+                           double* end_bias, double* consist, double* dump_att, double* dump_pos,
+                           double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
+
 /* ---- housekeeping ------------------------------------------------------ */
 int b2ins_version(void);
 const char* b2ins_last_error(void);

@@ -72,7 +72,21 @@ def main():
                            engine.to_device(nav0), engine.to_device(gp['ref_gps']), idx,
                            torch.ones(len(idx), dtype=torch.float64, device='cuda'), dump_runs=2, dump_stride=10)
     assert torch.isfinite(res.end_err).all() and torch.isfinite(res.consist).all()
-    ref_gps = engine.to_device(np.tile(np.array([0.5, 2.0, 10.0, 1.0, 0.0, 0.0]), (50, 1)))
+    # K7 with each vibration model (PSD: K5 series of exactly these 40 runs)
+    n0 = g0['ref_gyro'].shape[0]
+    sa, na = engine.psd_series(100.0, n0, 40, 0, vib, 1)
+    sg, ng = engine.psd_series(100.0, n0, 40, 1, vib, 1)
+    for vg, va in (({'type': 'random', 'x': 0.01, 'y': 0.02, 'z': 0.03}, {'type': 'random', 'x': 0.5, 'y': 0.5, 'z': 0.5}),
+                   ({'type': 'sinusoidal', 'freq': 3.0, 'x': 0.01, 'y': 0.02, 'z': 0.03},
+                    {'type': 'sinusoidal', 'freq': 7.5, 'x': 0.5, 'y': 0.5, 'z': 0.5}),
+                   (engine.vib_series(sg * 1e-3, ng), engine.vib_series(sa, na))):
+        res = engine.ins_loose(100.0, 40, 1, MID_G, MID_A, {'stdp': np.array([5.0, 5.0, 7.0]), 'stdv': np.full(3, 0.05)},
+                               g0['ini'], engine.to_device(g0['ref_gyro']), engine.to_device(g0['ref_accel']),
+                               engine.to_device(nav0), engine.to_device(gp['ref_gps']), idx,
+                               torch.ones(len(idx), dtype=torch.float64, device='cuda'), dump_runs=2, dump_stride=10,
+                               vib_gyro=vg, vib_accel=va)
+        assert torch.isfinite(res.end_err).all() and torch.isfinite(res.consist).all()
+    ref_gps =engine.to_device(np.tile(np.array([0.5, 2.0, 10.0, 1.0, 0.0, 0.0]), (50, 1)))
     engine.gps_noise(7, ref_gps, {'stdp': np.ones(3), 'stdv': np.ones(3)}, 0, 3)
     ref_mag = engine.to_device(np.tile(np.array([20.0, -3.0, 40.0]), (51, 1)))
     mag = engine.mag_noise(9, ref_mag, {'si': np.eye(3), 'hi': np.ones(3), 'std': np.full(3, 0.5)}, 5, 3)
