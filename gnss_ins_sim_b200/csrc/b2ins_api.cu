@@ -895,6 +895,9 @@ double* b2ins_mc_plan_err_device(b2ins_mc_plan* plan) { return plan ? plan->d_ou
 void* b2ins_mc_plan_stream(b2ins_mc_plan* plan) { return plan ? plan->stream : nullptr; }
 
 // ---------------------------------------------------------------- K7 --------
+static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                      int ndump, EkfParams* out);
+
 int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, const double* ref_accel,
                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx,
                         const double* gps_vis, double* end_err, double* end_bias, double* consist,
@@ -922,6 +925,78 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
   ARG_CHECK(ndump == 0 || ndump == 5, "dump_att/pos/vel/wb/ab must be given together");
   ARG_CHECK(cfg->dump_stride >= 0, "dump_stride must be >= 0");
   EkfParams p;
+  int rc = ekf_params(cfg, vib_gyro, vib_accel, ndump, &p);
+  if (rc != B2INS_OK) return rc;
+  p.ref_gyro = ref_gyro;
+  p.ref_accel = ref_accel;
+  p.ref_nav = ref_nav;
+  p.ref_gps = ref_gps;
+  p.gps_idx = gps_idx;
+  p.gps_vis = gps_vis;
+  p.stats_start = cfg->stats_start;
+  p.end_err = end_err;
+  p.end_bias = end_bias;
+  p.consist = consist;
+  p.out_att = dump_att;
+  p.out_pos = dump_pos;
+  p.out_vel = dump_vel;
+  p.out_wb = dump_wb;
+  p.out_ab = dump_ab;
+  const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
+  if (p.gyro.vib_type == B2INS_VIB_NONE && p.accel.vib_type == B2INS_VIB_NONE)
+    ekf_kernel<false, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  else
+    ekf_kernel<true, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const double* gyro, const double* accel,
+                            const double* gps, const int64_t* gps_idx, const double* gps_vis,
+                            const double* ref_nav, double* end_err, double* end_bias, double* dump_att,
+                            double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+  ARG_CHECK(cfg, "cfg is null");
+  ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
+  ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
+  ARG_CHECK(ini_draw == 0 || ini_draw == 1, "ini_draw must be 0 or 1");
+  ARG_CHECK((end_err == nullptr) == (ref_nav == nullptr), "end_err and ref_nav must be given together");
+  if (cfg->runs == 0 || cfg->n == 0) return B2INS_OK;
+  ARG_CHECK(cfg->n < (int64_t(1) << 32), "n must be < 2^32");
+  ARG_CHECK(gyro && accel, "null buffer: gyro and accel are required");
+  ARG_CHECK(cfg->m == 0 || (gps && gps_idx && gps_vis), "m > 0 needs gps, gps_idx and gps_vis");
+  ARG_CHECK(cfg->dump_runs >= 0 && cfg->dump_runs <= cfg->runs, "dump_runs out of range");
+  const int ndump = (dump_att != nullptr) + (dump_pos != nullptr) + (dump_vel != nullptr) + (dump_wb != nullptr) +
+                    (dump_ab != nullptr);
+  ARG_CHECK(ndump == 0 || ndump == 5, "dump_att/pos/vel/wb/ab must be given together");
+  ARG_CHECK(cfg->dump_stride >= 0, "dump_stride must be >= 0");
+  EkfParams p;
+  int rc = ekf_params(cfg, nullptr, nullptr, ndump, &p);
+  if (rc != B2INS_OK) return rc;
+  p.ref_nav = ref_nav;
+  p.gps_idx = gps_idx;
+  p.gps_vis = gps_vis;
+  p.fed_gyro = gyro;
+  p.fed_accel = accel;
+  p.fed_gps = gps;
+  p.ini_draw = ini_draw;
+  p.end_err = end_err;
+  p.end_bias = end_bias;
+  p.out_att = dump_att;
+  p.out_pos = dump_pos;
+  p.out_vel = dump_vel;
+  p.out_wb = dump_wb;
+  p.out_ab = dump_ab;
+  const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
+  ekf_kernel<false, true><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+// The filter model of cfg (Q, R, P0, bias model, initial state) and the launch geometry of K7; the
+// caller sets the buffers.  vib_*: the generator's vibration (NULL for supplied measurements).
+static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                      int ndump, EkfParams* out) {
+  EkfParams& p = *out;
   std::memset(&p, 0, sizeof(p));
   p.n = cfg->n;
   p.runs = cfg->runs;
@@ -935,12 +1010,6 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
   if (rc != B2INS_OK) return rc;
   rc = digest_triad(&cfg->accel_err, vib_accel, cfg->fs, &p.accel);
   if (rc != B2INS_OK) return rc;
-  p.ref_gyro = ref_gyro;
-  p.ref_accel = ref_accel;
-  p.ref_nav = ref_nav;
-  p.ref_gps = ref_gps;
-  p.gps_idx = gps_idx;
-  p.gps_vis = gps_vis;
   for (int c = 0; c < 3; ++c) {
     p.stdp[c] = cfg->gps_stdp[c];
     p.stdv[c] = cfg->gps_stdv[c];
@@ -962,24 +1031,9 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
   ARG_CHECK(cfg->vel_rw >= 0.0 && cfg->att_rw >= 0.0, "vel_rw and att_rw must be >= 0");
   p.qv_extra = cfg->vel_rw * cfg->vel_rw * p.dt;
   p.qphi_extra = cfg->att_rw * cfg->att_rw * p.dt;
-  p.stats_start = cfg->stats_start;
-  p.end_err = end_err;
-  p.end_bias = end_bias;
-  p.consist = consist;
-  p.out_att = dump_att;
-  p.out_pos = dump_pos;
-  p.out_vel = dump_vel;
-  p.out_wb = dump_wb;
-  p.out_ab = dump_ab;
   p.dump_runs = ndump ? cfg->dump_runs : 0;
   p.dump_stride = cfg->dump_stride > 1 ? cfg->dump_stride : 1;
   p.dump_rows = (cfg->n + p.dump_stride - 1) / p.dump_stride;
-  const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
-  if (p.gyro.vib_type == B2INS_VIB_NONE && p.accel.vib_type == B2INS_VIB_NONE)
-    ekf_kernel<false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  else
-    ekf_kernel<true><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
 

@@ -55,6 +55,11 @@ struct EkfParams {
   double* out_wb;
   double* out_ab;
   int64_t dump_runs, dump_stride, dump_rows;
+  // supplied measurements (ekf_kernel<false, true>), run-major: gyro, accel [runs][n][3], gps [runs][m][6]
+  const double* fed_gyro;
+  const double* fed_accel;
+  const double* fed_gps;
+  int ini_draw;                    // 1: the initial state is ini + the P0 draw of the run; 0: ini itself
 };
 
 // 3 x 3 symmetric-positive NEES  e^T A^-1 e  via the adjugate
@@ -121,8 +126,14 @@ __device__ __forceinline__ int ekf_own(int q, int m) {
 // VIB: the vibration models of p.accel / p.gyro (vib_term's, added last to each measurement) are compiled
 // in; the launch picks ekf_kernel<false> when both vib_types are B2INS_VIB_NONE, so that instantiation is
 // the filter without any vibration code.
-template <bool VIB>
+// FED: the filter runs on supplied measurements (p.fed_gyro / fed_accel / fed_gps) instead of generating
+// them: no Philox draws besides the optional initial-state draw, no Gauss-Markov carry, no vibration (it is
+// in the data).  Lane q reads the channels it would generate, so the quad shuffles that build f and w are
+// the same; sample i + 1 and the next GPS row are loaded a step / an epoch before they are used.  The
+// consistency record needs the true biases and is compiled out; end_err is written when ref_nav is given.
+template <bool VIB, bool FED>
 __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant__ EkfParams p) {
+  static_assert(!(VIB && FED), "supplied measurements carry their vibration already");
   __shared__ double Psm[kEkfN * kEkfN * kEkfRuns];      // 14.4 KB
   const int lane = threadIdx.x;
   // lane = q * 8 + rs: the eight runs of a quad index are neighbours, so a warp's 64-bit accesses to
@@ -142,7 +153,7 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   // GPS noise of the generator: horizontal sigmas in radians with the radii at the FIRST reference
   // sample, as pathgen.gps_gen does (pathgen.py:617-620)
   double sdp0 = p.stdp[0], sdp1 = p.stdp[1];
-  if (p.m > 0) {
+  if (!FED && p.m > 0) {
     const GeoParam gp = geo_param(p.ref_gps[0], p.ref_gps[2]);
     sdp0 = div_nr(sdp0, gp.rm);
     sdp1 = div_nr(div_nr(sdp1, gp.rn), gp.cl);
@@ -157,7 +168,8 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   double e0[10];
 #pragma unroll
   for (int j = 0; j < 5; ++j) {
-    const Normal2 z = normal_pair(0xFFFFFFFEu, kDrawIni + j, run_lo, run_hi, p.k0, p.k1);
+    Normal2 z{0.0, 0.0};        // FED without ini_draw: a zero draw through the same code
+    if (!FED || p.ini_draw) z = normal_pair(0xFFFFFFFEu, kDrawIni + j, run_lo, run_hi, p.k0, p.k1);
     e0[2 * j] = z.z0;
     e0[2 * j + 1] = z.z1;
   }
@@ -217,31 +229,58 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   int epochs = 0;
   int64_t jg = 0;                          // next GPS row
   int64_t next_gps = p.m > 0 ? p.gps_idx[0] : -1;
+  // FED: the lane's two channels of its run (lanes 2 and 3 read c0 twice and drop the second) and the run's
+  // GPS rows; nx0 / nx1 hold sample i + 1 during step i, ng the next GPS row
+  const double* fch0 = nullptr;
+  const double* fch1 = nullptr;
+  const double* fgps = nullptr;
+  double nx0 = 0.0, nx1 = 0.0, ng[6];
+  if constexpr (FED) {
+    const int cc = two ? c1 : c0;
+    fch0 = (c0 < 3) ? p.fed_accel + run * p.n * 3 + c0 : p.fed_gyro + run * p.n * 3 + (c0 - 3);
+    fch1 = (cc < 3) ? p.fed_accel + run * p.n * 3 + cc : p.fed_gyro + run * p.n * 3 + (cc - 3);
+    fgps = p.fed_gps + run * p.m * 6;
+    nx0 = fch0[0];
+    nx1 = fch1[0];
+#pragma unroll
+    for (int k = 0; k < 6; ++k) ng[k] = p.m > 0 ? fgps[k] : 0.0;
+  }
   __syncwarp();
 
   for (int64_t i = 0; i < p.n; ++i) {
     // ================= GPS sample of IMU sample i: update, then the consistency record ==========
     if (i == next_gps) {
       if (p.gps_vis[jg] > 0.0) {
-        // the three GPS pairs: lane q < 3 makes pair q, the quad shares them
-        Normal2 zz{0.0, 0.0};
-        if (q < 3) zz = normal_pair(static_cast<uint32_t>(jg), kPairGps + q, run_lo, run_hi, p.k0, p.k1);
         double zn[6];
+        if constexpr (!FED) {
+          // the three GPS pairs: lane q < 3 makes pair q, the quad shares them
+          Normal2 zz{0.0, 0.0};
+          if (q < 3) zz = normal_pair(static_cast<uint32_t>(jg), kPairGps + q, run_lo, run_hi, p.k0, p.k1);
 #pragma unroll
-        for (int j = 0; j < 3; ++j) {
-          zn[2 * j] = quad(zz.z0, j);
-          zn[2 * j + 1] = quad(zz.z1, j);
+          for (int j = 0; j < 3; ++j) {
+            zn[2 * j] = quad(zz.z0, j);
+            zn[2 * j + 1] = quad(zz.z1, j);
+          }
         }
         const double* rg = p.ref_gps + jg * 6;
         const GeoParam gp = geo_param_sc(st.sl, st.cl, st.pos.z);
         const double rmh = gp.rm + st.pos.z, rnh = (gp.rn + st.pos.z) * gp.cl;
         double zm[6];
-        zm[0] = (st.pos.x - (rg[0] + sdp0 * zn[0])) * rmh;
-        zm[1] = (st.pos.y - (rg[1] + sdp1 * zn[1])) * rnh;
-        zm[2] = -(st.pos.z - (rg[2] + p.stdp[2] * zn[2]));
-        zm[3] = st.vel.x - (rg[3] + p.stdv[0] * zn[3]);
-        zm[4] = st.vel.y - (rg[4] + p.stdv[1] * zn[4]);
-        zm[5] = st.vel.z - (rg[5] + p.stdv[2] * zn[5]);
+        if constexpr (FED) {
+          zm[0] = (st.pos.x - ng[0]) * rmh;
+          zm[1] = (st.pos.y - ng[1]) * rnh;
+          zm[2] = -(st.pos.z - ng[2]);
+          zm[3] = st.vel.x - ng[3];
+          zm[4] = st.vel.y - ng[4];
+          zm[5] = st.vel.z - ng[5];
+        } else {
+          zm[0] = (st.pos.x - (rg[0] + sdp0 * zn[0])) * rmh;
+          zm[1] = (st.pos.y - (rg[1] + sdp1 * zn[1])) * rnh;
+          zm[2] = -(st.pos.z - (rg[2] + p.stdp[2] * zn[2]));
+          zm[3] = st.vel.x - (rg[3] + p.stdv[0] * zn[3]);
+          zm[4] = st.vel.y - (rg[4] + p.stdv[1] * zn[4]);
+          zm[5] = st.vel.z - (rg[5] + p.stdv[2] * zn[5]);
+        }
         double x[kEkfN];
 #pragma unroll
         for (int c = 0; c < kEkfN; ++c) x[c] = 0.0;
@@ -292,7 +331,7 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
           ba[c3] -= x[12 + c3];
         }
       }
-      if (i >= p.stats_start) {
+      if (!FED && i >= p.stats_start) {
         // the generator's drift d[i] of every channel, from its owner
         double dch[6];
         dch[0] = quad(carry0, 0); dch[1] = quad(carry0, 1); dch[2] = quad(carry0, 2); dch[3] = quad(carry0, 3);
@@ -338,6 +377,12 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
       }
       ++jg;
       next_gps = jg < p.m ? p.gps_idx[jg] : -1;
+      if constexpr (FED) {
+        if (jg < p.m) {
+#pragma unroll
+          for (int k = 0; k < 6; ++k) ng[k] = fgps[jg * 6 + k];
+        }
+      }
     }
     // ================= histories ==================================================================
     int64_t row;
@@ -355,7 +400,13 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
     if (i == p.n - 1) break;
     // ================= the measurements of sample i (the K12 generator, shared out over the quad) ==
     double m0, m1 = 0.0;
-    {
+    if constexpr (FED) {
+      // sample i was loaded during step i - 1; sample i + 1 <= n - 1 is loaded now, a step before its use
+      m0 = nx0;
+      m1 = nx1;
+      nx0 = fch0[(i + 1) * 3];
+      nx1 = fch1[(i + 1) * 3];
+    } else {
       const uint32_t t = static_cast<uint32_t>(i);
       const double* ref0 = (c0 < 3) ? p.ref_accel + i * 3 + c0 : p.ref_gyro + i * 3 + (c0 - 3);
       const Normal2 z0 = normal_pair(t, static_cast<uint32_t>(c0), run_lo, run_hi, p.k0, p.k1);
@@ -492,17 +543,19 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   }
 
   if (active && q == 0) {
-    const double* r = p.ref_nav + (p.n - 1) * 9;
-    double* e = p.end_err + run * 9;
-    e[0] = angle_range_pi(st.yaw - r[0]);
-    e[1] = angle_range_pi(st.pitch - r[1]);
-    e[2] = angle_range_pi(st.roll - r[2]);
-    e[3] = st.pos.x - r[3];
-    e[4] = st.pos.y - r[4];
-    e[5] = st.pos.z - r[5];
-    e[6] = st.vel.x - r[6];
-    e[7] = st.vel.y - r[7];
-    e[8] = st.vel.z - r[8];
+    if (!FED || p.end_err) {
+      const double* r = p.ref_nav + (p.n - 1) * 9;
+      double* e = p.end_err + run * 9;
+      e[0] = angle_range_pi(st.yaw - r[0]);
+      e[1] = angle_range_pi(st.pitch - r[1]);
+      e[2] = angle_range_pi(st.roll - r[2]);
+      e[3] = st.pos.x - r[3];
+      e[4] = st.pos.y - r[4];
+      e[5] = st.pos.z - r[5];
+      e[6] = st.vel.x - r[6];
+      e[7] = st.vel.y - r[7];
+      e[8] = st.vel.z - r[8];
+    }
     if (p.end_bias) {
 #pragma unroll
       for (int c3 = 0; c3 < 3; ++c3) {
@@ -510,7 +563,7 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
         p.end_bias[run * 6 + 3 + c3] = ba[c3];
       }
     }
-    if (p.consist) {
+    if (!FED && p.consist) {
       double* o = p.consist + run * 19;
       o[0] = nees[0]; o[1] = nees[1]; o[2] = nees[2];
 #pragma unroll

@@ -448,6 +448,42 @@ def allan_mc(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offse
     return avar, tau
 
 
+def _ekf_config(fs, n, runs, m, seed, gyro_err, accel_err, gps_err, ini, run_offset, ini_att_std, earth_rot,
+                stats_start, dump_runs, dump_stride, vel_rw, att_rw):
+    """b2ins_ekf_config of one K7 launch."""
+    cfg = _lib.EkfConfig()
+    cfg.fs, cfg.n, cfg.runs, cfg.run_offset, cfg.m = float(fs), int(n), int(runs), int(run_offset), int(m)
+    cfg.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    cfg.gyro_err = _lib.sensor_err(gyro_err, 'arw')
+    cfg.accel_err = _lib.sensor_err(accel_err, 'vrw')
+    stdp = np.broadcast_to(np.asarray(gps_err['stdp'], dtype=np.float64), (3,))
+    stdv = np.broadcast_to(np.asarray(gps_err['stdv'], dtype=np.float64), (3,))
+    ini = np.asarray(ini, dtype=np.float64).reshape(-1)
+    for c in range(3):
+        cfg.gps_stdp[c], cfg.gps_stdv[c] = float(stdp[c]), float(stdv[c])
+        cfg.ini_att_std[c] = float(ini_att_std[c])
+    for c in range(9):
+        cfg.ini[c] = float(ini[c])
+    cfg.stats_start, cfg.dump_runs, cfg.dump_stride = int(stats_start), int(dump_runs), int(dump_stride)
+    cfg.earth_rot = int(bool(earth_rot))
+    cfg.vel_rw, cfg.att_rw = float(vel_rw), float(att_rw)
+    return cfg
+
+
+def _ekf_result(out, runs, n, dump_runs, dump_stride, dev, end_err):
+    """The EkfResult buffers of one K7 launch (those of `out` where they fit); consist is the caller's."""
+    res = out or EkfResult()
+    res.end_err = _reuse(res.end_err, (runs, 9), dev) if end_err else None
+    res.end_bias = _reuse(res.end_bias, (runs, 6), dev)
+    if dump_runs > 0:
+        rows = -(-n // max(1, int(dump_stride)))
+        res.att, res.pos, res.vel, res.wb, res.ab = (_reuse(getattr(res, k), (dump_runs, rows, 3), dev)
+                                                     for k in ('att', 'pos', 'vel', 'wb', 'ab'))
+    else:
+        res.att = res.pos = res.vel = res.wb = res.ab = None
+    return res
+
+
 class EkfResult:
     """Device-side results of one loosely-coupled-filter launch (K7)."""
 
@@ -474,37 +510,48 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     n, m = ref_gyro.shape[0], ref_gps.shape[0]
     dev = ref_gyro.device
     assert gps_idx.dtype == torch.int64 and gps_idx.is_cuda and gps_idx.is_contiguous()
-    cfg = _lib.EkfConfig()
-    cfg.fs, cfg.n, cfg.runs, cfg.run_offset, cfg.m = float(fs), int(n), int(runs), int(run_offset), int(m)
-    cfg.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    cfg.gyro_err = _lib.sensor_err(gyro_err, 'arw')
-    cfg.accel_err = _lib.sensor_err(accel_err, 'vrw')
-    stdp = np.broadcast_to(np.asarray(gps_err['stdp'], dtype=np.float64), (3,))
-    stdv = np.broadcast_to(np.asarray(gps_err['stdv'], dtype=np.float64), (3,))
-    ini = np.asarray(ini, dtype=np.float64).reshape(-1)
-    for c in range(3):
-        cfg.gps_stdp[c], cfg.gps_stdv[c] = float(stdp[c]), float(stdv[c])
-        cfg.ini_att_std[c] = float(ini_att_std[c])
-    for c in range(9):
-        cfg.ini[c] = float(ini[c])
-    cfg.stats_start, cfg.dump_runs, cfg.dump_stride = int(stats_start), int(dump_runs), int(dump_stride)
-    cfg.earth_rot = int(bool(earth_rot))
-    cfg.vel_rw, cfg.att_rw = float(vel_rw), float(att_rw)
+    cfg = _ekf_config(fs, n, runs, m, seed, gyro_err, accel_err, gps_err, ini, run_offset, ini_att_std, earth_rot,
+                      stats_start, dump_runs, dump_stride, vel_rw, att_rw)
     # Vib structs are passed by pointer; a VIB_SERIES Vib keeps its series tensor alive through the call
     vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
-    res = out or EkfResult()
-    res.end_err = _reuse(res.end_err, (runs, 9), dev)
-    res.end_bias = _reuse(res.end_bias, (runs, 6), dev)
+    res = _ekf_result(out, runs, n, dump_runs, dump_stride, dev, end_err=True)
     res.consist = _reuse(res.consist, (runs, 19), dev)
-    if dump_runs > 0:
-        rows = -(-n // max(1, int(dump_stride)))
-        res.att, res.pos, res.vel, res.wb, res.ab = (_reuse(getattr(res, k), (dump_runs, rows, 3), dev)
-                                                     for k in ('att', 'pos', 'vel', 'wb', 'ab'))
-    else:
-        res.att = res.pos = res.vel = res.wb = res.ab = None
     _lib.check(lib.b2ins_ins_loose_ex_f64(
         ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), _ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps),
         ctypes.c_void_p(gps_idx.data_ptr()), _ptr(gps_vis), _ptr(res.end_err), _ptr(res.end_bias),
         _ptr(res.consist), _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream()))
+    return res
+
+
+def ins_loose_fed(fs, gyro, accel, gps, gps_idx, gps_vis, gyro_err, accel_err, gps_err, ini, seed=0, ini_draw=False,
+                  run_offset=0, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True, ref_nav=None, dump_runs=0,
+                  dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0):
+    """K7 on supplied measurements (b2ins_ins_loose_fed_f64): gyro, accel [R,n,3] and gps [R,m,6] (LLA rad, m;
+    NED m/s) CUDA f64, run-major; gps_idx [m] CUDA int64, strictly ascending IMU sample indices of the GPS rows;
+    gps_vis [m] CUDA f64.  gyro_err / accel_err / gps_err are the filter's model (Q, R, P0) only.  Every run
+    starts at ini, plus with ini_draw the P0 draw of global run run_offset + r under seed (the generated
+    experiment's draw).  ref_nav [n,9] (optional): end_err as engine.ins_loose makes it.  Returns an
+    EkfResult without consist (and without end_err when ref_nav is None).  Asynchronous on the current
+    stream."""
+    _require_cuda()
+    lib = _lib.load()
+    R, n, three = gyro.shape
+    m = gps.shape[1]
+    if three != 3 or tuple(accel.shape) != (R, n, 3) or tuple(gps.shape) != (R, m, 6):
+        raise ValueError('gyro, accel must be [R, n, 3] and gps [R, m, 6]; got %s, %s, %s'
+                         % (tuple(gyro.shape), tuple(accel.shape), tuple(gps.shape)))
+    if tuple(gps_idx.shape) != (m,) or tuple(gps_vis.shape) != (m,):
+        raise ValueError('gps_idx and gps_vis need one entry per GPS row (%d)' % m)
+    if ref_nav is not None and tuple(ref_nav.shape) != (n, 9):
+        raise ValueError('ref_nav must be [n, 9]')
+    assert gps_idx.dtype == torch.int64 and gps_idx.is_cuda and gps_idx.is_contiguous()
+    cfg = _ekf_config(fs, n, R, m, seed, gyro_err, accel_err, gps_err, ini, run_offset, ini_att_std, earth_rot,
+                      -1, dump_runs, dump_stride, vel_rw, att_rw)
+    res = _ekf_result(out, R, n, dump_runs, dump_stride, gyro.device, end_err=ref_nav is not None)
+    res.consist = None
+    _lib.check(lib.b2ins_ins_loose_fed_f64(
+        ctypes.byref(cfg), int(bool(ini_draw)), _ptr(gyro), _ptr(accel), _ptr(gps), ctypes.c_void_p(gps_idx.data_ptr()),
+        _ptr(gps_vis), _ptr(ref_nav), _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.att), _ptr(res.pos),
+        _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream()))
     return res

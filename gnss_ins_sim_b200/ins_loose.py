@@ -10,11 +10,44 @@ IMU and GPS measurements from the shared true trajectory (the reference's sensor
 streams), filters them, and leaves end-point errors, bias estimates and a consistency record (NEES,
 3-sigma containment).  Parity with the reference is unpinnable; the filter is validated statistically.
 
-It is driven by gnss_ins_sim_b200.sim.Sim (ref_frame 0, IMU(gps=True), fs = [fs_imu, fs_gps, 0]); the
-per-run .run(set_of_input) of the reference protocol would need the measurements on the host and a
-CPU filter, which this package does not have (no CPU fallback): it raises.
+It is driven by gnss_ins_sim_b200.sim.Sim (ref_frame 0, IMU(gps=True), fs = [fs_imu, fs_gps, 0]).  The same
+filter also runs on SUPPLIED measurements (a drive log, another simulator, a saved experiment): run_batch() for
+R runs in one launch, the reference's per-run .run(set_of_input), and Sim on a logged-data directory.  There it
+needs its noise model, InsLoose(imu=IMU(..., gps=True)), and an initial state.
 """
 import numpy as np
+import torch
+
+from . import engine
+
+
+class ModelMissing(ValueError, NotImplementedError):
+    """The filter has no noise model (InsLoose(imu=...)) for measurements it did not generate."""
+
+
+def gps_sample_index(fs, time, gps_time):
+    """IMU sample of every GPS row: the sample nearest to gps_time[j] by time, ties to the earlier one
+    (rint(gps_time * fs) for the simulator's own data).  Raises ValueError for a row outside the series, a row
+    more than half a sample (0.5 / fs) from every IMU sample (a gap in time), and rows that do not land on
+    strictly increasing samples: the filter applies at most one GPS row per sample, in order."""
+    time = np.asarray(time, dtype=np.float64).reshape(-1)
+    gt = np.asarray(gps_time, dtype=np.float64).reshape(-1)
+    n = time.size
+    if n < 2 or not np.all(np.diff(time) > 0.0):
+        raise ValueError('time must hold at least two strictly increasing IMU sample times')
+    half = 0.5 / float(fs)
+    tol = 1e-9 * half           # times read back from text files may be an ulp off the grid
+    for j, t in enumerate(gt):
+        if not (time[0] - half - tol <= t <= time[-1] + half + tol):
+            raise ValueError('gps_time[%d] = %r s lies outside the IMU series [%r, %r] s' % (j, t, time[0], time[-1]))
+    k = np.clip(np.searchsorted(time, gt, side='left'), 1, n - 1)
+    idx = np.where(gt - time[k - 1] <= time[k] - gt, k - 1, k)
+    for j in np.nonzero(np.abs(gt - time[idx]) > half + tol)[0]:
+        raise ValueError('gps_time[%d] = %r s lies more than half a sample from every IMU sample' % (j, gt[j]))
+    for j in np.nonzero(np.diff(idx) <= 0)[0]:
+        raise ValueError('gps rows %d and %d (%r s, %r s) land on IMU samples %d and %d: every row needs a later '
+                         'sample than the row before' % (j, j + 1, gt[j], gt[j + 1], idx[j], idx[j + 1]))
+    return idx.astype(np.int64)
 
 
 class InsLoose(object):
@@ -23,18 +56,23 @@ class InsLoose(object):
     '''
 
     def __init__(self, ini_pos_vel_att=None, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True,
-                 vel_model_std=0.02, att_model_std=0.0):
+                 vel_model_std=0.02, att_model_std=0.0, imu=None):
         '''
         Args:
             ini_pos_vel_att: (9,) true initial LLA [rad, rad, m], body velocity, ZYX Euler angles; None:
-                the initial state of the motion definition the Sim was given.  Every run starts from
-                this state plus a draw from the initial covariance.
+                the initial state of the motion definition the Sim was given (on a logged-data directory: its
+                first reference row).  Every run of a Sim starts from this state plus a draw from the initial
+                covariance; run_batch() / run() need it given here.
             ini_att_std: 1-sigma of the initial misalignment about N, E, D [rad].
             earth_rot: consider the Earth rotation in the mechanization.
             vel_model_std, att_model_std: extra velocity [m/s/sqrt(s)] and misalignment [rad/sqrt(s)]
                 random walks of the filter model.  The reference's truth generator and its first-order
                 mechanization disagree slightly (noise-free free integration of motion_def-ins.csv ends
                 0.37 m/s off); 0.02 m/s/sqrt(s) covers that and keeps the filter consistent.
+            imu: the filter's noise model on supplied measurements, an imu_model.IMU with gps=True (its gyro,
+                accelerometer and GPS errors set Q, R and P0).  Needed by run_batch() / run(); a Sim on a
+                logged-data directory falls back to its own imu.  A generating Sim filters with the IMU that
+                makes its data: any other model there is an error.
 
         Vibration: the measurements carry the Sim's env vibration (random, sinusoidal or PSD), as
         get_data(['accel']) / get_data(['gyro']) do, but the filter model does not know about it.  Tell
@@ -53,14 +91,75 @@ class InsLoose(object):
         self.earth_rot = bool(earth_rot)
         self.vel_model_std, self.att_model_std = float(vel_model_std), float(att_model_std)
         self.run_times = 0
+        if imu is not None and not getattr(imu, 'gps', False):
+            raise ValueError('InsLoose(imu=...) needs an IMU with gps=True: its GPS errors are the filter\'s R')
+        self.imu = imu
 
     def run(self, set_of_input):
-        raise NotImplementedError(
-            'InsLoose runs as one fused Monte-Carlo kernel through gnss_ins_sim_b200.sim.Sim (measurement '
-            'generation + filter on the device); there is no per-run host filter (no CPU fallback)')
+        '''
+        One run of the reference protocol: set_of_input = [fs, gyro (n,3) rad/s, accel (n,3) m/s^2, time (n,)
+        s, gps_time (m,) s, gps (m,6) LLA rad, m, NED m/s].  Every GPS row is used; the run starts at ini.
+        '''
+        fs, gyro, accel, time, gps_time, gps = set_of_input
+        out = self.run_batch(fs, np.asarray(gyro, dtype=np.float64)[None], np.asarray(accel, dtype=np.float64)[None],
+                             time, gps_time, np.asarray(gps, dtype=np.float64)[None])
+        self.results = [o[0] for o in out]
 
     def get_results(self):
-        return [self.results]
+        '''
+        [pos, vel, att_euler, wb, ab] of the last run(), in self.output order.
+        '''
+        return self.results
 
     def reset(self):
         pass
+
+    def run_batch(self, fs, gyro, accel, time, gps_time, gps, gps_visibility=None, seed=None, to_host=True):
+        '''
+        R runs of supplied measurements in one launch.  gyro, accel [R, n, 3] (rad/s, m/s^2); time [n] s;
+        gps_time [m] s; gps [R, m, 6] (LLA rad, m; NED m/s); gps_visibility [m] (None: every row is used).  GPS
+        row j is applied at the IMU sample nearest to gps_time[j] (gps_sample_index).  seed None: every run
+        starts at ini; an integer: ini plus the initial-covariance draw of run run_times + r under that seed,
+        as a generated experiment draws it.  Returns pos, vel, att_euler, wb, ab [R, n, 3] (numpy, or CUDA
+        tensors if not to_host).
+        '''
+        imu = self.model()
+        g, a, gp = engine.to_device(gyro), engine.to_device(accel), engine.to_device(gps)
+        if g.dim() != 3 or g.shape[2] != 3 or a.shape != g.shape:
+            raise ValueError('gyro and accel must both be [R, n, 3]')
+        if gp.dim() != 3 or gp.shape[0] != g.shape[0] or gp.shape[2] != 6:
+            raise ValueError('gps must be [R, m, 6] with the R of gyro / accel')
+        if np.asarray(time).reshape(-1).size != g.shape[1]:
+            raise ValueError('time needs one entry per IMU sample (%d)' % g.shape[1])
+        if np.asarray(gps_time).reshape(-1).size != gp.shape[1]:
+            raise ValueError('gps_time needs one entry per GPS row (%d)' % gp.shape[1])
+        vis = np.ones(gp.shape[1]) if gps_visibility is None else np.asarray(gps_visibility, dtype=np.float64).reshape(-1)
+        if vis.size != gp.shape[1]:
+            raise ValueError('gps_visibility needs one entry per GPS row (%d)' % gp.shape[1])
+        res = self.launch(fs, g, a, gp, gps_sample_index(fs, time, gps_time), vis, imu, self.ini,
+                          0 if seed is None else seed, seed is not None, self.run_times)
+        self.run_times += g.shape[0]
+        out = (res.pos, res.vel, res.att, res.wb, res.ab)
+        return tuple(o.cpu().numpy() for o in out) if to_host else out
+
+    def model(self, fallback=None):
+        """The filter's noise model: imu, else fallback; ModelMissing if neither."""
+        imu = self.imu if self.imu is not None else fallback
+        if imu is None:
+            raise ModelMissing('InsLoose on supplied measurements needs its noise model: InsLoose(imu=IMU(..., '
+                               'gps=True)).  (Inside gnss_ins_sim_b200.sim.Sim the filter generates its own data.)')
+        if not getattr(imu, 'gps', False):
+            raise ValueError('the filter model must be an IMU with gps=True')
+        return imu
+
+    def launch(self, fs, gyro, accel, gps, gps_idx, gps_vis, imu, ini, seed, ini_draw, run_offset, ref_nav=None):
+        """engine.ins_loose_fed with this filter's options and histories of every run: gyro, accel [R,n,3], gps
+        [R,m,6], ref_nav [n,9] (optional) CUDA; gps_idx, gps_vis [m] host arrays."""
+        if ini is None:
+            raise ValueError('InsLoose on supplied measurements needs ini_pos_vel_att')
+        R = gyro.shape[0]
+        return engine.ins_loose_fed(fs, gyro, accel, gps, torch.from_numpy(np.asarray(gps_idx, dtype=np.int64)).cuda(),
+                                    engine.to_device(gps_vis), imu.gyro_err, imu.accel_err, imu.gps_err, ini,
+                                    seed=seed, ini_draw=ini_draw, run_offset=run_offset,
+                                    ini_att_std=self.ini_att_std, earth_rot=self.earth_rot, ref_nav=ref_nav,
+                                    dump_runs=R, vel_rw=self.vel_model_std, att_rw=self.att_model_std)

@@ -37,7 +37,7 @@ from . import engine, dist, logged
 from .free_integration import FreeIntegration
 from .free_integration_odo import FreeIntegration as FreeIntegrationOdo
 from .allan_analysis import Allan
-from .ins_loose import InsLoose
+from .ins_loose import InsLoose, gps_sample_index
 
 D2R = math.pi / 180
 R2D = 180 / math.pi
@@ -119,6 +119,16 @@ def lla_error_metres(x, r, frame):
                       -so * d[:, 0] + co * d[:, 1],
                       -cl * co * d[:, 0] - cl * so * d[:, 1] - sl * d[:, 2]], axis=1)
     return d
+
+
+def euler2dcm_zyx(att):
+    """(3,) yaw, pitch, roll -> the n -> b DCM (attitude.euler2dcm 'zyx' layout)."""
+    sy, cy = math.sin(att[0]), math.cos(att[0])
+    sp, cp = math.sin(att[1]), math.cos(att[1])
+    sr, cr = math.sin(att[2]), math.cos(att[2])
+    return np.array([[cp * cy, cp * sy, -sp],
+                     [sr * sp * cy - cr * sy, sr * sp * sy + cr * cy, sr * cp],
+                     [cr * sp * cy + sr * sy, cr * sp * sy - sr * cy, cr * cp]])
 
 
 def euler2quat_zyx(att):
@@ -545,9 +555,61 @@ class Sim(object):
             elif isinstance(a, Allan):
                 self._publish_allan(name, *a.run_batch(self.fs[0], self._logged_sets('accel'),
                                                        self._logged_sets('gyro')))
+            elif isinstance(a, InsLoose):
+                self._run_logged_ins_loose(i, a)
             else:
                 self._run_plugin(i, a, self._logged_inputs)
         self.sim_complete = True
+
+    def _run_logged_ins_loose(self, i, algo):
+        """The filter on the logged sets gyro-k, accel-k, gps-k (k < sim_count) with gps_time and, if present,
+        gps_visibility.  Model: algo.imu, else the Sim's imu.  Initial state: algo.ini, else the first reference
+        row (velocity rotated to the body frame), plus the initial-covariance draw of run run_base + k under the
+        Sim's seed, as the generated experiment draws it: a directory save_data wrote from a generated filter
+        experiment filters back to that experiment.  Run blocks are sized to the free device memory (inputs and
+        histories: 168 B per run-sample).  End-point errors and their statistics if the reference files exist."""
+        d, name, R = self._logged, self.algo_name(i), self.sim_count
+        if self.ref_frame != 0:
+            raise ValueError('ins_loose works in ref_frame 0 (LLA positions, NED velocities)')
+        imu = algo.model(self.imu)
+        has_ref = all(k in d for k in ('ref_att_euler', 'ref_pos', 'ref_vel'))
+        ini = algo.ini
+        if ini is None:
+            if not has_ref:
+                raise ValueError('InsLoose on a data directory needs ini_pos_vel_att or the ref_pos, ref_vel and '
+                                 'ref_att_euler files')
+            att = d['ref_att_euler'][0]
+            ini = np.concatenate([d['ref_pos'][0], euler2dcm_zyx(att).dot(d['ref_vel'][0]), att])
+        if 'gps_time' not in d:
+            raise ValueError('the data directory holds no gps_time.csv')
+        gyro, accel, gps = (self._logged_sets(k) for k in ('gyro', 'accel', 'gps'))
+        vis = d.get('gps_visibility')
+        vis = np.ones(len(d['gps_time'])) if vis is None else vis
+        gps_idx = gps_sample_index(self.fs[0], d['time'], d['gps_time'])
+        ref_nav = engine.to_device(np.concatenate([d['ref_att_euler'], d['ref_pos'], d['ref_vel']], axis=1)) \
+            if has_ref else None
+        outs = {o: [] for o in ('pos', 'vel', 'att_euler', 'wb', 'ab')}
+        errs, bias = [], []
+        block = self._allan_block(168, 3)
+        for r0 in range(0, R, block):
+            r1 = min(R, r0 + block)
+            res = algo.launch(self.fs[0], engine.to_device(gyro[r0:r1]), engine.to_device(accel[r0:r1]),
+                              engine.to_device(gps[r0:r1]), gps_idx, vis, imu, ini, self.seed, True,
+                              self.run_base + r0, ref_nav)
+            for o, t in zip(outs, (res.pos, res.vel, res.att, res.wb, res.ab)):
+                outs[o].append(t.cpu().numpy())
+            bias.append(res.end_bias.cpu().numpy())
+            if has_ref:
+                errs.append(res.end_err.cpu().numpy())
+            del res
+        algo.run_times += R
+        for o, parts in outs.items():
+            self.data[o] = dict(self.data[o]) if isinstance(self.data.get(o), dict) else {}
+            self.data[o].update(_keyed(name, np.concatenate(parts)))
+        self._mc[i] = {'base': 0, 'end_err': np.concatenate(errs) if has_ref else None,
+                       'end_bias': np.concatenate(bias)}
+        if has_ref:
+            self.err_stats[name] = engine.error_stats(engine.to_device(self._mc[i]['end_err'])).cpu().numpy()
 
     def _logged_inputs(self, algo, r):
         """Inputs of run r of a foreign plugin on logged data: set r of per-run data, everything else as is."""
@@ -715,7 +777,7 @@ class Sim(object):
         at most 1/share of the free device memory (free on the device + cached by torch's allocator but
         unused)."""
         lo, hi = self._shard
-        n = self._traj['ref_gyro'].shape[0]
+        n = len(self.data['time'])
         if torch.cuda.is_available():
             free_b = (torch.cuda.mem_get_info()[0] + torch.cuda.memory_reserved()
                       - torch.cuda.memory_allocated())
@@ -793,6 +855,9 @@ class Sim(object):
         device memory with PSD vibration, whose series K5 materialises, as for K9): end-point errors and their
         ensemble statistics (as for free integration), bias estimates, the consistency record."""
         name = self.algo_name(i)
+        if algo.imu is not None and algo.imu is not self.imu:
+            raise ValueError('a generating Sim filters with the IMU that makes its data: InsLoose(imu=...) must be '
+                             "the Sim's imu or None")
         lo, hi = self._shard
         self._mc[i] = {'base': 0, 'end_err': None}
         err, stats, con, bias = np.zeros((0, 9)), np.zeros((3, 9)), np.zeros((0, 19)), np.zeros((0, 6))

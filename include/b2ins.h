@@ -187,6 +187,22 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
                            double* end_bias, double* consist, double* dump_att, double* dump_pos,
                            double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
 
+/* K7 on SUPPLIED measurements (a drive log, another simulator, a saved experiment): the same filter,
+ * reading every run's IMU and GPS samples instead of generating them.
+ *   gyro, accel [runs][n][3] run-major (rad/s, m/s^2); gps [runs][m][6] LLA (rad, rad, m) and NED
+ *   velocity (m/s), applied at IMU sample gps_idx[j] (int64, strictly ascending, in [0, n); shared by all
+ *   runs) when gps_vis[j] > 0.
+ * cfg: gyro_err, accel_err, gps_stdp / gps_stdv are the filter's model only (Q, R, P0); ini is the initial
+ * state, plus the P0 draw of global run run_offset + r under seed when ini_draw is 1 (the draw of
+ * b2ins_ins_loose_f64, so the generated experiment's measurements filter to its results); stats_start is
+ * ignored: there is no consistency record (it needs the true biases).
+ * ref_nav [n][9] and end_err [runs][9]: both or neither; end_bias, dump_*: as in b2ins_ins_loose_f64.
+ * DEVICE pointers. */
+int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const double* gyro, const double* accel,
+                            const double* gps, const int64_t* gps_idx, const double* gps_vis,
+                            const double* ref_nav, double* end_err, double* end_bias, double* dump_att,
+                            double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
+
 /* ---- housekeeping ------------------------------------------------------ */
 int b2ins_version(void);
 const char* b2ins_last_error(void);

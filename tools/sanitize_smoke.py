@@ -86,6 +86,16 @@ def main():
                                torch.ones(len(idx), dtype=torch.float64, device='cuda'), dump_runs=2, dump_stride=10,
                                vib_gyro=vg, vib_accel=va)
         assert torch.isfinite(res.end_err).all() and torch.isfinite(res.consist).all()
+    # K7 on supplied measurements (K1 / K6 output of 13 runs), with and without end_err / the initial draw
+    gps_err = {'stdp': np.array([5.0, 5.0, 7.0]), 'stdv': np.full(3, 0.05)}
+    fg, fa = engine.imu_noise(100.0, 13, engine.to_device(g0['ref_gyro']), engine.to_device(g0['ref_accel']),
+                              MID_G, MID_A, 1)
+    fgps = engine.gps_noise(13, engine.to_device(gp['ref_gps']), gps_err, 0, 1)
+    vis = torch.ones(len(idx), dtype=torch.float64, device='cuda')
+    for draw, nav in ((1, engine.to_device(nav0)), (0, None)):
+        res = engine.ins_loose_fed(100.0, fg, fa, fgps, idx, vis, MID_G, MID_A, gps_err, g0['ini'], seed=1,
+                                   ini_draw=draw, ref_nav=nav, dump_runs=2, dump_stride=10)
+        assert torch.isfinite(res.end_bias).all() and torch.isfinite(res.pos).all()
     ref_gps =engine.to_device(np.tile(np.array([0.5, 2.0, 10.0, 1.0, 0.0, 0.0]), (50, 1)))
     engine.gps_noise(7, ref_gps, {'stdp': np.ones(3), 'stdv': np.ones(3)}, 0, 3)
     ref_mag = engine.to_device(np.tile(np.array([20.0, -3.0, 40.0]), (51, 1)))
