@@ -102,6 +102,7 @@ SIGNATURES = {
     'b2ins_ins_loose_f64': (_I, [ctypes.POINTER(EkfConfig)] + [_P] * 15),
     'b2ins_ins_loose_ex_f64': (_I, [ctypes.POINTER(EkfConfig), _VB, _VB] + [_P] * 15),
     'b2ins_ins_loose_fed_f64': (_I, [ctypes.POINTER(EkfConfig), _I] + [_P] * 14),
+    'b2ins_ins_loose_proc_f64': (_I, [ctypes.POINTER(EkfConfig), _VB, _VB, _L, _I] + [_P] * 16),
     'b2ins_diag_dfma_rate': (_I, [c_double_p]),
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),

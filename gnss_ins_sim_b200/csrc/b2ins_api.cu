@@ -897,6 +897,11 @@ void* b2ins_mc_plan_stream(b2ins_mc_plan* plan) { return plan ? plan->stream : n
 // ---------------------------------------------------------------- K7 --------
 static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
                       int ndump, EkfParams* out);
+static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                         int64_t proc_start, int proc_pos_frame, const double* ref_gyro, const double* ref_accel,
+                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx, const double* gps_vis,
+                         double* end_err, double* end_bias, double* consist, double* proc_stats, double* dump_att,
+                         double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
 
 int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, const double* ref_accel,
                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx,
@@ -912,6 +917,33 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
                            const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
                            double* end_bias, double* consist, double* dump_att, double* dump_pos,
                            double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+  return ins_loose_gen(cfg, vib_gyro, vib_accel, -1, B2INS_POS_FRAME_LLA, ref_gyro, ref_accel, ref_nav, ref_gps,
+                       gps_idx, gps_vis, end_err, end_bias, consist, nullptr, dump_att, dump_pos, dump_vel, dump_wb,
+                       dump_ab, stream);
+}
+
+int b2ins_ins_loose_proc_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                             int64_t proc_start, int proc_pos_frame, const double* ref_gyro, const double* ref_accel,
+                             const double* ref_nav, const double* ref_gps, const int64_t* gps_idx,
+                             const double* gps_vis, double* end_err, double* end_bias, double* consist,
+                             double* proc_stats, double* dump_att, double* dump_pos, double* dump_vel,
+                             double* dump_wb, double* dump_ab, void* stream) {
+  ARG_CHECK(cfg, "cfg is null");
+  ARG_CHECK(proc_pos_frame >= B2INS_POS_FRAME_LLA && proc_pos_frame <= B2INS_POS_FRAME_ECEF,
+            "proc_pos_frame must be B2INS_POS_FRAME_*");
+  ARG_CHECK(proc_stats, "null buffer: proc_stats is required");
+  ARG_CHECK(proc_start >= 0 && proc_start < cfg->n, "proc_start must be in [0, n)");
+  return ins_loose_gen(cfg, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel, ref_nav, ref_gps,
+                       gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att, dump_pos, dump_vel,
+                       dump_wb, dump_ab, stream);
+}
+
+// K7 on generated measurements; proc_stats NULL: no process statistics (ekf_kernel<VIB, false, false>)
+static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                         int64_t proc_start, int proc_pos_frame, const double* ref_gyro, const double* ref_accel,
+                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx, const double* gps_vis,
+                         double* end_err, double* end_bias, double* consist, double* proc_stats, double* dump_att,
+                         double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
   ARG_CHECK(cfg, "cfg is null");
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
@@ -942,11 +974,23 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
   p.out_vel = dump_vel;
   p.out_wb = dump_wb;
   p.out_ab = dump_ab;
+  p.proc_stats = proc_stats;
+  p.proc_start = proc_start;
+  p.proc_pos_frame = proc_pos_frame;
   const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
-  if (p.gyro.vib_type == B2INS_VIB_NONE && p.accel.vib_type == B2INS_VIB_NONE)
-    ekf_kernel<false, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
-  else
-    ekf_kernel<true, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bool vib = !(p.gyro.vib_type == B2INS_VIB_NONE && p.accel.vib_type == B2INS_VIB_NONE);
+  if (proc_stats) {
+    if (vib)
+      ekf_kernel<true, false, true><<<grid, kEkfThreads, 0, s>>>(p);
+    else
+      ekf_kernel<false, false, true><<<grid, kEkfThreads, 0, s>>>(p);
+  } else {
+    if (vib)
+      ekf_kernel<true, false, false><<<grid, kEkfThreads, 0, s>>>(p);
+    else
+      ekf_kernel<false, false, false><<<grid, kEkfThreads, 0, s>>>(p);
+  }
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
@@ -987,7 +1031,7 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
   p.out_wb = dump_wb;
   p.out_ab = dump_ab;
   const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
-  ekf_kernel<false, true><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  ekf_kernel<false, true, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }

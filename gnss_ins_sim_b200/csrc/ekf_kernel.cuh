@@ -60,6 +60,11 @@ struct EkfParams {
   const double* fed_accel;
   const double* fed_gps;
   int ini_draw;                    // 1: the initial state is ini + the P0 draw of the run; 0: ini itself
+  // process-error statistics (ekf_kernel<VIB, false, true>): samples >= proc_start, position columns as
+  // B2INS_POS_FRAME_* proc_pos_frame
+  double* proc_stats;              // [runs][3][9] max|e|, mean, std of att, pos, vel
+  int64_t proc_start;
+  int proc_pos_frame;
 };
 
 // 3 x 3 symmetric-positive NEES  e^T A^-1 e  via the adjugate
@@ -131,10 +136,16 @@ __device__ __forceinline__ int ekf_own(int q, int m) {
 // in the data).  Lane q reads the channels it would generate, so the quad shuffles that build f and w are
 // the same; sample i + 1 and the next GPS row are loaded a step / an epoch before they are used.  The
 // consistency record needs the true biases and is compiled out; end_err is written when ref_nav is given.
-template <bool VIB, bool FED>
+// PROC: per-run process-error statistics (proc_stats), taken where history row i is written -- after the GPS
+// update of sample i -- against ref_nav row i for i >= proc_start.  The nominal state is replicated, so lane
+// q < 3 of a run takes column group q (attitude, position, velocity) with no shuffle; its accumulators live
+// in shared memory behind P, as [12][32 lanes], and lane 0 writes the run's [3][9] at the end.
+template <bool VIB, bool FED, bool PROC>
 __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant__ EkfParams p) {
   static_assert(!(VIB && FED), "supplied measurements carry their vibration already");
-  __shared__ double Psm[kEkfN * kEkfN * kEkfRuns];      // 14.4 KB
+  static_assert(!(FED && PROC), "supplied-data histories are on the host: their statistics are taken there");
+  constexpr int kAcc = PROC ? 12 * kEkfThreads : 0;    // 3 KB: max, sum, sum of squares, shift, 3 columns each
+  __shared__ double Psm[kEkfN * kEkfN * kEkfRuns + kAcc];      // 14.4 KB (+ 3 KB)
   const int lane = threadIdx.x;
   // lane = q * 8 + rs: the eight runs of a quad index are neighbours, so a warp's 64-bit accesses to
   // P[element][run] fall on distinct banks whether the four q's differ in the column (sweep 1) or in
@@ -149,6 +160,13 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   const double dt = p.dt;
   auto P = [&](int i, int j) -> double& { return Psm[(i * kEkfN + j) * kEkfRuns + rs]; };
   auto quad = [&](double v, int owner) { return __shfl_sync(0xffffffffu, v, owner * kEkfRuns + rs); };
+  // PROC: this lane's accumulators, column c of max|e| / shifted sum / shifted sum of squares / shift at
+  // acc[(0 | 3 | 6 | 9 + c) * 32]
+  double* const acc = Psm + kEkfN * kEkfN * kEkfRuns + lane;
+  if constexpr (PROC) {
+#pragma unroll
+    for (int j = 0; j < 12; ++j) acc[j * kEkfThreads] = 0.0;
+  }
 
   // GPS noise of the generator: horizontal sigmas in radians with the radii at the FIRST reference
   // sample, as pathgen.gps_gen does (pathgen.py:617-620)
@@ -397,6 +415,21 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
         p.out_ab[o + c3] = ba[c3];
       }
     }
+    if constexpr (PROC) {
+      // the state of history row i against truth row i (shared by all runs: it stays in L2)
+      if (q < 3 && i >= p.proc_start) {
+        const double* rn9 = p.ref_nav + i * 9;
+        double e[3];
+        if (q == 0)
+          proc_err_att(st, rn9, e);
+        else if (q == 1)
+          proc_err_pos<0>(st, rn9, p.proc_pos_frame, e);
+        else
+          proc_err_vel(st, rn9, e);
+        proc_fold<3, kEkfThreads>(e, i == p.proc_start, acc, acc + 3 * kEkfThreads, acc + 6 * kEkfThreads,
+                                  acc + 9 * kEkfThreads);
+      }
+    }
     if (i == p.n - 1) break;
     // ================= the measurements of sample i (the K12 generator, shared out over the quad) ==
     double m0, m1 = 0.0;
@@ -542,7 +575,17 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
     }
   }
 
+  if constexpr (PROC) __syncwarp();       // lane 0 reads the accumulators of lanes 8 and 16 of its run
   if (active && q == 0) {
+    if constexpr (PROC) {
+      double* o = p.proc_stats + run * 27;
+      const double inv = 1.0 / static_cast<double>(p.n - p.proc_start);
+#pragma unroll
+      for (int g = 0; g < 3; ++g) {
+        const double* a = acc + g * kEkfRuns;          // lane g * 8 + rs
+        proc_put<3, kEkfThreads>(o + 3 * g, inv, a, a + 3 * kEkfThreads, a + 6 * kEkfThreads, a + 9 * kEkfThreads);
+      }
+    }
     if (!FED || p.end_err) {
       const double* r = p.ref_nav + (p.n - 1) * 9;
       double* e = p.end_err + run * 9;

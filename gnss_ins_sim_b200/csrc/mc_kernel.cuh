@@ -371,18 +371,20 @@ __device__ __forceinline__ void put_end(const McParams& p, int64_t run, double y
   }
 }
 
-// process-error accumulation of one sample (ins_data_manager.py:536-541, :761-808).  In ref_frame 0 a
-// non-zero pos_frame (uniform over the launch) takes the position error in metres, as array_error does
-// for extra_opt 'ned' / 'ecef' (:543-552): d = lla2ecef(x) - lla2ecef(r), and for NED c_ne(r) . d.  Both
-// points are converted from their LLA values, not from the step's carried latitude sin/cos.
-template <int RF>
-__device__ __forceinline__ void proc_accumulate(const NavState& st, const double* r, int pos_frame,
-                                                double* pe_max, double* pe_sum, double* pe_sq, double* pe_k,
-                                                int64_t& pe_cnt) {
-  double e[9];
+// Process errors of one sample against the truth row r [9] (ins_data_manager.py:536-541), one column group
+// at a time (K12 takes all three, K7 gives each to one lane of a run): the attitude through angle_range_pi,
+// the velocity as plain differences.
+__device__ __forceinline__ void proc_err_att(const NavState& st, const double* r, double* e) {
   e[0] = angle_range_pi(st.yaw - r[0]);
   e[1] = angle_range_pi(st.pitch - r[1]);
   e[2] = angle_range_pi(st.roll - r[2]);
+}
+// The position: LLA differences, or in ref_frame 0 with a non-zero pos_frame (uniform over the launch) in
+// metres, as array_error does for extra_opt 'ned' / 'ecef' (:543-552): d = lla2ecef(x) - lla2ecef(r), and for
+// NED c_ne(r) . d.  Both points are converted from their LLA values, not from the step's carried latitude
+// sin/cos.
+template <int RF>
+__device__ __forceinline__ void proc_err_pos(const NavState& st, const double* r, int pos_frame, double* e) {
   if (RF == 0 && pos_frame != 0) {
     const Vec3 x = lla2ecef(st.pos.x, st.pos.y, st.pos.z);
     const Vec3 xr = lla2ecef(r[3], r[4], r[5]);
@@ -391,33 +393,68 @@ __device__ __forceinline__ void proc_accumulate(const NavState& st, const double
       double sl, cl, so, co;
       sincos_angle(r[3], &sl, &cl);
       sincos_angle(r[4], &so, &co);
-      e[3] = -sl * co * d.x - sl * so * d.y + cl * d.z;
-      e[4] = -so * d.x + co * d.y;
-      e[5] = -cl * co * d.x - cl * so * d.y - sl * d.z;
+      e[0] = -sl * co * d.x - sl * so * d.y + cl * d.z;
+      e[1] = -so * d.x + co * d.y;
+      e[2] = -cl * co * d.x - cl * so * d.y - sl * d.z;
     } else {
-      e[3] = d.x;
-      e[4] = d.y;
-      e[5] = d.z;
+      e[0] = d.x;
+      e[1] = d.y;
+      e[2] = d.z;
     }
   } else {
-    e[3] = st.pos.x - r[3];
-    e[4] = st.pos.y - r[4];
-    e[5] = st.pos.z - r[5];
+    e[0] = st.pos.x - r[3];
+    e[1] = st.pos.y - r[4];
+    e[2] = st.pos.z - r[5];
   }
-  e[6] = st.vel.x - r[6];
-  e[7] = st.vel.y - r[7];
-  e[8] = st.vel.z - r[8];
-  if (pe_cnt == 0) {
+}
+__device__ __forceinline__ void proc_err_vel(const NavState& st, const double* r, double* e) {
+  e[0] = st.vel.x - r[6];
+  e[1] = st.vel.y - r[7];
+  e[2] = st.vel.z - r[8];
+}
+
+// Adds the NC errors e to the accumulators max|e|, shifted sum, shifted sum of squares and shift K (the first
+// error sample, taken when `first`); column c of each accumulator is at [c * S].
+template <int NC, int S>
+__device__ __forceinline__ void proc_fold(const double* e, bool first, double* mx, double* sum, double* sq,
+                                          double* k) {
+  if (first) {
 #pragma unroll
-    for (int c = 0; c < 9; ++c) pe_k[c] = e[c];
+    for (int c = 0; c < NC; ++c) k[c * S] = e[c];
   }
 #pragma unroll
-  for (int c = 0; c < 9; ++c) {
-    pe_max[c] = fmax(pe_max[c], fabs(e[c]));
-    const double d = e[c] - pe_k[c];
-    pe_sum[c] += d;
-    pe_sq[c] += d * d;
+  for (int c = 0; c < NC; ++c) {
+    mx[c * S] = fmax(mx[c * S], fabs(e[c]));
+    const double d = e[c] - k[c * S];
+    sum[c * S] += d;
+    sq[c * S] += d * d;
   }
+}
+
+// max|e|, mean and std (ddof 0) of NC accumulated columns into o[c], o[9 + c], o[18 + c] (the [3][9] rows of
+// proc_stats); inv = 1 / the sample count
+template <int NC, int S>
+__device__ __forceinline__ void proc_put(double* o, double inv, const double* mx, const double* sum,
+                                         const double* sq, const double* k) {
+#pragma unroll
+  for (int c = 0; c < NC; ++c) {
+    const double m = sum[c * S] * inv;  // mean of (e - K)
+    o[c] = mx[c * S];
+    o[9 + c] = k[c * S] + m;
+    o[18 + c] = sqrt(fmax(sq[c * S] * inv - m * m, 0.0));
+  }
+}
+
+// process-error accumulation of one sample (ins_data_manager.py:536-541, :761-808) over all nine columns
+template <int RF>
+__device__ __forceinline__ void proc_accumulate(const NavState& st, const double* r, int pos_frame,
+                                                double* pe_max, double* pe_sum, double* pe_sq, double* pe_k,
+                                                int64_t& pe_cnt) {
+  double e[9];
+  proc_err_att(st, r, e);
+  proc_err_pos<RF>(st, r, pos_frame, e + 3);
+  proc_err_vel(st, r, e + 6);
+  proc_fold<9, 1>(e, pe_cnt == 0, pe_max, pe_sum, pe_sq, pe_k);
   ++pe_cnt;
 }
 
@@ -653,13 +690,7 @@ mc_kernel(const __grid_constant__ McParams p) {
     if (PROC && p.proc_stats) {
       double* o = p.proc_stats + mr.run * 27;
       const double inv = pe_cnt > 0 ? 1.0 / static_cast<double>(pe_cnt) : 0.0;
-#pragma unroll
-      for (int c = 0; c < 9; ++c) {
-        const double m = pe_sum[c] * inv;  // mean of (e - K)
-        o[c] = pe_max[c];
-        o[9 + c] = pe_k[c] + m;
-        o[18 + c] = sqrt(fmax(pe_sq[c] * inv - m * m, 0.0));
-      }
+      proc_put<9, 1>(o, inv, pe_max, pe_sum, pe_sq, pe_k);
     }
   }
 }

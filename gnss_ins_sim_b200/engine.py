@@ -491,20 +491,23 @@ class EkfResult:
         self.end_err = None      # [R,9] att (wrapped), pos (LLA), vel error at the last sample
         self.end_bias = None     # [R,6] gyro, accel bias estimates at the last sample
         self.consist = None      # [R,19] NEES sums (pos, vel, att), inside-3-sigma counts [15], epochs
+        self.proc_stats = None   # [R,3,9] max|e|, mean, std of att, pos, vel per run (proc_start given)
         self.att = self.pos = self.vel = self.wb = self.ab = None   # [dump_runs,rows,3]
 
 
 def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_accel, ref_nav, ref_gps,
               gps_idx, gps_vis, run_offset=0, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True,
               stats_start=0, dump_runs=0, dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0,
-              vib_gyro=None, vib_accel=None):
+              vib_gyro=None, vib_accel=None, proc_start=None, proc_pos_frame=0):
     """K7: Monte-Carlo loosely-coupled GNSS/INS filter (the spec: DESIGN.md section 11; csrc/ekf_kernel.cuh).
     ref_gyro, ref_accel [n,3], ref_nav [n,9], ref_gps [m,6], gps_vis [m]: CUDA f64; gps_idx [m]: CUDA
     int64 (IMU sample index of every GPS row).  ini: the 9 true initial values (LLA, body velocity, Euler
     angles).  vib_gyro / vib_accel: the vibration of the measurements the filter sees, as imu_noise takes
     them (a parsed dict, or a Vib such as vib_series over K5 series of exactly these runs); the filter
-    model does not include it (vel_rw / att_rw, DESIGN.md section 11).  Asynchronous on the current
-    stream."""
+    model does not include it (vel_rw / att_rw, DESIGN.md section 11).  proc_start (sample index in [0, n)):
+    also res.proc_stats [R,3,9], the per-run process-error statistics of samples >= proc_start, positions as
+    POS_FRAME_* proc_pos_frame (b2ins_ins_loose_proc_f64); every other output is unchanged.  Asynchronous on
+    the current stream."""
     _require_cuda()
     lib = _lib.load()
     n, m = ref_gyro.shape[0], ref_gps.shape[0]
@@ -517,10 +520,17 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
     res = _ekf_result(out, runs, n, dump_runs, dump_stride, dev, end_err=True)
     res.consist = _reuse(res.consist, (runs, 19), dev)
-    _lib.check(lib.b2ins_ins_loose_ex_f64(
-        ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), _ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps),
-        ctypes.c_void_p(gps_idx.data_ptr()), _ptr(gps_vis), _ptr(res.end_err), _ptr(res.end_bias),
-        _ptr(res.consist), _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream()))
+    refs = (_ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps), ctypes.c_void_p(gps_idx.data_ptr()),
+            _ptr(gps_vis), _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.consist))
+    dumps = (_ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream())
+    if proc_start is None:
+        res.proc_stats = None
+        _lib.check(lib.b2ins_ins_loose_ex_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), *refs, *dumps))
+    else:
+        res.proc_stats = _reuse(res.proc_stats, (runs, 3, 9), dev)
+        _lib.check(lib.b2ins_ins_loose_proc_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va),
+                                                int(proc_start), int(proc_pos_frame), *refs,
+                                                _ptr(res.proc_stats), *dumps))
     return res
 
 

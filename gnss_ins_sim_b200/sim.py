@@ -835,7 +835,8 @@ class Sim(object):
         d = self._dev
         return d['ref_gps'], d['gps_idx'], d['gps_vis']
 
-    def _ekf_launch(self, algo, r0, runs, stats_start=0, dump_runs=0, dump_stride=1):
+    def _ekf_launch(self, algo, r0, runs, stats_start=0, dump_runs=0, dump_stride=1, proc_start=None,
+                    proc_pos_frame=0):
         gps = self._ekf_inputs()
         d = self._dev
         ini = algo.ini if algo.ini is not None else self._traj.get('ini')
@@ -848,7 +849,22 @@ class Sim(object):
                                 ini_att_std=algo.ini_att_std, earth_rot=algo.earth_rot,
                                 stats_start=stats_start, dump_runs=dump_runs, dump_stride=dump_stride,
                                 vel_rw=algo.vel_model_std, att_rw=algo.att_model_std,
-                                vib_gyro=vib_gyro, vib_accel=vib_acc)
+                                vib_gyro=vib_gyro, vib_accel=vib_acc, proc_start=proc_start,
+                                proc_pos_frame=proc_pos_frame)
+
+    def _ekf_blocks(self, algo, **kw):
+        """K7 over this rank's shard (kw: _ekf_launch's), in run blocks sized to the free device memory with PSD
+        vibration, whose series K5 materialises (as for K9): the EkfResult of every block."""
+        lo, hi = self._shard
+        block = self._allan_block(48, 3) if self._uses_psd() else hi - lo
+        parts = []
+        for r0 in range(lo, hi, block):
+            runs = min(hi, r0 + block) - r0
+            parts.append(self._ekf_launch(algo, r0, runs, **kw))
+            if block < hi - lo:     # the next block's series take the memory of this block's
+                for sensor in (0, 1):
+                    self._psd_cache.pop((sensor, runs, r0), None)
+        return parts
 
     def _run_ins_loose(self, i, algo):
         """demo_ins_loose.py semantics, all runs of this rank in one K7 launch (in run blocks sized to the free
@@ -863,14 +879,7 @@ class Sim(object):
         err, stats, con, bias = np.zeros((0, 9)), np.zeros((3, 9)), np.zeros((0, 19)), np.zeros((0, 6))
         if hi > lo:
             start = int(round(min(30.0, 0.1 * len(self.data['time']) / self.fs[0]) * self.fs[0]))
-            block = self._allan_block(48, 3) if self._uses_psd() else hi - lo
-            parts = []
-            for r0 in range(lo, hi, block):
-                runs = min(hi, r0 + block) - r0
-                parts.append(self._ekf_launch(algo, r0, runs, stats_start=start))
-                if block < hi - lo:     # the next block's series take the memory of this block's
-                    for sensor in (0, 1):
-                        self._psd_cache.pop((sensor, runs, r0), None)
+            parts = self._ekf_blocks(algo, stats_start=start)
             end_err = torch.cat([r.end_err for r in parts])
             stats = engine.error_stats(end_err).cpu().numpy()
             err = end_err.cpu().numpy()
@@ -1226,7 +1235,13 @@ class Sim(object):
             else:
                 lo, hi = self._shard
                 ps = None
-                if hi > lo:
+                algo = self.algo[algo_index]
+                if hi > lo and isinstance(algo, InsLoose):
+                    # reduced inside the filter kernel: the histories of all runs would not fit
+                    ps = torch.cat([r.proc_stats for r in self._ekf_blocks(algo, proc_start=start,
+                                                                           proc_pos_frame=frame)])
+                    ps = ps.reshape(hi - lo, 27)
+                elif hi > lo:
                     ps = self._mc_launch(algo_index, lo, hi - lo, stats_start=start,
                                          proc_pos_frame=frame).proc_stats.reshape(hi - lo, 27)
                 ps = dist.gather_rows(ps, self.sim_count).reshape(-1, 3, 9)

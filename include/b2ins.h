@@ -187,6 +187,20 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
                            double* end_bias, double* consist, double* dump_att, double* dump_pos,
                            double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
 
+/* b2ins_ins_loose_ex_f64 that also reduces every run's process errors over the series: proc_stats
+ * [runs][3][9] = max|e|, mean, std (ddof 0) of the attitude (wrapped to [-pi, pi]), position and velocity
+ * errors of samples proc_start .. n-1 (proc_start in [0, n)), the reference's get_error_stats(err_stats_start
+ * >= 0) (ins_data_manager.py:761-808).  Sample i's error is the state of history row i (after that sample's
+ * GPS update) against ref_nav row i.  proc_pos_frame: the position columns, as in
+ * b2ins_mc_free_integration_ex_f64 (B2INS_POS_FRAME_LLA differences, _NED or _ECEF metres).  Everything else,
+ * including every other output, is b2ins_ins_loose_ex_f64's, bit for bit.  DEVICE pointers. */
+int b2ins_ins_loose_proc_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                             int64_t proc_start, int proc_pos_frame, const double* ref_gyro, const double* ref_accel,
+                             const double* ref_nav, const double* ref_gps, const int64_t* gps_idx,
+                             const double* gps_vis, double* end_err, double* end_bias, double* consist,
+                             double* proc_stats, double* dump_att, double* dump_pos, double* dump_vel,
+                             double* dump_wb, double* dump_ab, void* stream);
+
 /* K7 on SUPPLIED measurements (a drive log, another simulator, a saved experiment): the same filter,
  * reading every run's IMU and GPS samples instead of generating them.
  *   gyro, accel [runs][n][3] run-major (rad/s, m/s^2); gps [runs][m][6] LLA (rad, rad, m) and NED

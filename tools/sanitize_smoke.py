@@ -86,6 +86,14 @@ def main():
                                torch.ones(len(idx), dtype=torch.float64, device='cuda'), dump_runs=2, dump_stride=10,
                                vib_gyro=vg, vib_accel=va)
         assert torch.isfinite(res.end_err).all() and torch.isfinite(res.consist).all()
+    # K7's process statistics in each position frame (41 runs: a ragged last CTA), from a mid-series start
+    for frame in (engine.POS_FRAME_LLA, engine.POS_FRAME_NED, engine.POS_FRAME_ECEF):
+        res = engine.ins_loose(100.0, 41, 1, MID_G, MID_A, {'stdp': np.array([5.0, 5.0, 7.0]), 'stdv': np.full(3, 0.05)},
+                               g0['ini'], engine.to_device(g0['ref_gyro']), engine.to_device(g0['ref_accel']),
+                               engine.to_device(nav0), engine.to_device(gp['ref_gps']), idx,
+                               torch.ones(len(idx), dtype=torch.float64, device='cuda'), proc_start=n0 // 3,
+                               proc_pos_frame=frame)
+        assert torch.isfinite(res.proc_stats).all()
     # K7 on supplied measurements (K1 / K6 output of 13 runs), with and without end_err / the initial draw
     gps_err = {'stdp': np.array([5.0, 5.0, 7.0]), 'stdv': np.full(3, 0.05)}
     fg, fa = engine.imu_noise(100.0, 13, engine.to_device(g0['ref_gyro']), engine.to_device(g0['ref_accel']),
