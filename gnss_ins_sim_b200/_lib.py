@@ -14,6 +14,7 @@ OK, ERR_ARG, ERR_CUDA, ERR_NODEV = 0, 1, 2, 3
 LAYOUT_RUN_MAJOR, LAYOUT_TIME_MAJOR, LAYOUT_CHANNEL_MAJOR = 0, 1, 2
 VIB_NONE, VIB_RANDOM, VIB_SINUSOIDAL, VIB_SERIES = 0, 1, 2, 3
 POS_FRAME_LLA, POS_FRAME_NED, POS_FRAME_ECEF = 0, 1, 2
+ALIGN_OFF, ALIGN_YAW, ALIGN_GPS = 0, 1, 2
 
 
 class SensorErr(ctypes.Structure):
@@ -52,6 +53,11 @@ class EkfConfig(ctypes.Structure):
                 ('stats_start', ctypes.c_int64), ('dump_runs', ctypes.c_int64),
                 ('dump_stride', ctypes.c_int32), ('earth_rot', ctypes.c_int32),
                 ('vel_rw', ctypes.c_double), ('att_rw', ctypes.c_double)]
+
+
+class EkfAlign(ctypes.Structure):
+    _fields_ = [('mode', ctypes.c_int32), ('reserved', ctypes.c_int32), ('yaw', ctypes.c_double),
+                ('yaw_var', ctypes.c_double)]
 
 
 class B2insError(RuntimeError):
@@ -103,6 +109,9 @@ SIGNATURES = {
     'b2ins_ins_loose_ex_f64': (_I, [ctypes.POINTER(EkfConfig), _VB, _VB] + [_P] * 15),
     'b2ins_ins_loose_fed_f64': (_I, [ctypes.POINTER(EkfConfig), _I] + [_P] * 14),
     'b2ins_ins_loose_proc_f64': (_I, [ctypes.POINTER(EkfConfig), _VB, _VB, _L, _I] + [_P] * 16),
+    'b2ins_ins_loose_align_f64': (_I, [ctypes.POINTER(EkfConfig), ctypes.POINTER(EkfAlign), _VB, _VB, _L, _I]
+                                  + [_P] * 16),
+    'b2ins_ins_loose_fed_align_f64': (_I, [ctypes.POINTER(EkfConfig), ctypes.POINTER(EkfAlign)] + [_P] * 14),
     'b2ins_diag_dfma_rate': (_I, [c_double_p]),
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),

@@ -897,11 +897,17 @@ void* b2ins_mc_plan_stream(b2ins_mc_plan* plan) { return plan ? plan->stream : n
 // ---------------------------------------------------------------- K7 --------
 static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
                       int ndump, EkfParams* out);
-static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
-                         int64_t proc_start, int proc_pos_frame, const double* ref_gyro, const double* ref_accel,
-                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx, const double* gps_vis,
-                         double* end_err, double* end_bias, double* consist, double* proc_stats, double* dump_att,
-                         double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
+static int ekf_align_params(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, EkfParams* p);
+static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
+                         const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame, const double* ref_gyro,
+                         const double* ref_accel, const double* ref_nav, const double* ref_gps,
+                         const int64_t* gps_idx, const double* gps_vis, double* end_err, double* end_bias,
+                         double* consist, double* proc_stats, double* dump_att, double* dump_pos, double* dump_vel,
+                         double* dump_wb, double* dump_ab, void* stream);
+static int ins_loose_fed(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, int ini_draw, const double* gyro,
+                         const double* accel, const double* gps, const int64_t* gps_idx, const double* gps_vis,
+                         const double* ref_nav, double* end_err, double* end_bias, double* dump_att, double* dump_pos,
+                         double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
 
 int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, const double* ref_accel,
                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx,
@@ -917,9 +923,9 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
                            const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
                            double* end_bias, double* consist, double* dump_att, double* dump_pos,
                            double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
-  return ins_loose_gen(cfg, vib_gyro, vib_accel, -1, B2INS_POS_FRAME_LLA, ref_gyro, ref_accel, ref_nav, ref_gps,
-                       gps_idx, gps_vis, end_err, end_bias, consist, nullptr, dump_att, dump_pos, dump_vel, dump_wb,
-                       dump_ab, stream);
+  return ins_loose_gen(cfg, nullptr, vib_gyro, vib_accel, -1, B2INS_POS_FRAME_LLA, ref_gyro, ref_accel, ref_nav,
+                       ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, nullptr, dump_att, dump_pos, dump_vel,
+                       dump_wb, dump_ab, stream);
 }
 
 int b2ins_ins_loose_proc_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
@@ -933,17 +939,36 @@ int b2ins_ins_loose_proc_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_g
             "proc_pos_frame must be B2INS_POS_FRAME_*");
   ARG_CHECK(proc_stats, "null buffer: proc_stats is required");
   ARG_CHECK(proc_start >= 0 && proc_start < cfg->n, "proc_start must be in [0, n)");
-  return ins_loose_gen(cfg, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel, ref_nav, ref_gps,
-                       gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att, dump_pos, dump_vel,
+  return ins_loose_gen(cfg, nullptr, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel, ref_nav,
+                       ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att, dump_pos, dump_vel,
+                       dump_wb, dump_ab, stream);
+}
+
+int b2ins_ins_loose_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
+                              const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame,
+                              const double* ref_gyro, const double* ref_accel, const double* ref_nav,
+                              const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
+                              double* end_bias, double* consist, double* proc_stats, double* dump_att,
+                              double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+  ARG_CHECK(cfg, "cfg is null");
+  ARG_CHECK((proc_stats == nullptr) == (proc_start == -1), "proc_stats and proc_start >= 0 must be given together");
+  if (proc_stats) {
+    ARG_CHECK(proc_pos_frame >= B2INS_POS_FRAME_LLA && proc_pos_frame <= B2INS_POS_FRAME_ECEF,
+              "proc_pos_frame must be B2INS_POS_FRAME_*");
+    ARG_CHECK(proc_start >= 0 && proc_start < cfg->n, "proc_start must be in [0, n)");
+  }
+  return ins_loose_gen(cfg, align, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel, ref_nav,
+                       ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att, dump_pos, dump_vel,
                        dump_wb, dump_ab, stream);
 }
 
 // K7 on generated measurements; proc_stats NULL: no process statistics (ekf_kernel<VIB, false, false>)
-static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
-                         int64_t proc_start, int proc_pos_frame, const double* ref_gyro, const double* ref_accel,
-                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx, const double* gps_vis,
-                         double* end_err, double* end_bias, double* consist, double* proc_stats, double* dump_att,
-                         double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
+                         const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame, const double* ref_gyro,
+                         const double* ref_accel, const double* ref_nav, const double* ref_gps,
+                         const int64_t* gps_idx, const double* gps_vis, double* end_err, double* end_bias,
+                         double* consist, double* proc_stats, double* dump_att, double* dump_pos, double* dump_vel,
+                         double* dump_wb, double* dump_ab, void* stream) {
   ARG_CHECK(cfg, "cfg is null");
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
@@ -958,6 +983,8 @@ static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro,
   ARG_CHECK(cfg->dump_stride >= 0, "dump_stride must be >= 0");
   EkfParams p;
   int rc = ekf_params(cfg, vib_gyro, vib_accel, ndump, &p);
+  if (rc != B2INS_OK) return rc;
+  rc = ekf_align_params(cfg, align, &p);
   if (rc != B2INS_OK) return rc;
   p.ref_gyro = ref_gyro;
   p.ref_accel = ref_accel;
@@ -999,6 +1026,24 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
                             const double* gps, const int64_t* gps_idx, const double* gps_vis,
                             const double* ref_nav, double* end_err, double* end_bias, double* dump_att,
                             double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+  return ins_loose_fed(cfg, nullptr, ini_draw, gyro, accel, gps, gps_idx, gps_vis, ref_nav, end_err, end_bias,
+                       dump_att, dump_pos, dump_vel, dump_wb, dump_ab, stream);
+}
+
+int b2ins_ins_loose_fed_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const double* gyro,
+                                  const double* accel, const double* gps, const int64_t* gps_idx,
+                                  const double* gps_vis, const double* ref_nav, double* end_err, double* end_bias,
+                                  double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb,
+                                  double* dump_ab, void* stream) {
+  return ins_loose_fed(cfg, align, 0, gyro, accel, gps, gps_idx, gps_vis, ref_nav, end_err, end_bias, dump_att,
+                       dump_pos, dump_vel, dump_wb, dump_ab, stream);
+}
+
+// K7 on supplied measurements (ekf_kernel<false, true, false, aligned>)
+static int ins_loose_fed(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, int ini_draw, const double* gyro,
+                         const double* accel, const double* gps, const int64_t* gps_idx, const double* gps_vis,
+                         const double* ref_nav, double* end_err, double* end_bias, double* dump_att, double* dump_pos,
+                         double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
   ARG_CHECK(cfg, "cfg is null");
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
@@ -1016,6 +1061,8 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
   EkfParams p;
   int rc = ekf_params(cfg, nullptr, nullptr, ndump, &p);
   if (rc != B2INS_OK) return rc;
+  rc = ekf_align_params(cfg, align, &p);
+  if (rc != B2INS_OK) return rc;
   p.ref_nav = ref_nav;
   p.gps_idx = gps_idx;
   p.gps_vis = gps_vis;
@@ -1031,7 +1078,10 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
   p.out_wb = dump_wb;
   p.out_ab = dump_ab;
   const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
-  ekf_kernel<false, true, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  if (p.align)
+    ekf_kernel<false, true, false, true><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  else
+    ekf_kernel<false, true, false, false><<<grid, kEkfThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
@@ -1078,6 +1128,29 @@ static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, co
   p.dump_runs = ndump ? cfg->dump_runs : 0;
   p.dump_stride = cfg->dump_stride > 1 ? cfg->dump_stride : 1;
   p.dump_rows = (cfg->n + p.dump_stride - 1) / p.dump_stride;
+  return B2INS_OK;
+}
+
+// The alignment of b2ins_ekf_align (NULL: off) into p: the mode, the given yaw and the P0 terms that are the
+// same for every run (include/b2ins.h).  Accelerometer y sets roll (the N misalignment), x sets pitch (E).
+static int ekf_align_params(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, EkfParams* p) {
+  p->align = align ? align->mode : B2INS_ALIGN_OFF;
+  if (p->align == B2INS_ALIGN_OFF) return B2INS_OK;
+  ARG_CHECK(p->align == B2INS_ALIGN_YAW || p->align == B2INS_ALIGN_GPS, "align->mode must be B2INS_ALIGN_*");
+  static_assert(kAlignGps == B2INS_ALIGN_GPS, "the kernel's GPS-heading mode");
+  ARG_CHECK(cfg->n == 0 || cfg->n >= kAlignN, "alignment needs n >= 10 IMU samples");
+  ARG_CHECK(std::isfinite(align->yaw) || p->align == B2INS_ALIGN_GPS, "align->yaw must be finite");
+  ARG_CHECK(align->yaw_var >= 0.0 || p->align == B2INS_ALIGN_GPS, "align->yaw_var must be >= 0");
+  constexpr double kG = 9.80665;
+  const b2ins_sensor_err& a = cfg->accel_err;
+  for (int c = 0; c < 2; ++c) {
+    const int ax = 1 - c;
+    p->align_p0[c] = (a.b[ax] * a.b[ax] + a.b_drift[ax] * a.b_drift[ax] + a.rw[ax] * a.rw[ax] * cfg->fs / kAlignN) /
+                     (kG * kG);
+  }
+  p->align_yaw = align->yaw;
+  p->align_p0[2] = align->yaw_var;
+  for (int c = 0; c < 3; ++c) p->arw2[c] = cfg->gyro_err.rw[c] * cfg->gyro_err.rw[c];
   return B2INS_OK;
 }
 

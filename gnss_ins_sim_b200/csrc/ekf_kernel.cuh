@@ -26,6 +26,8 @@ namespace b2ins {
 constexpr int kEkfThreads = 32;
 constexpr int kEkfN = 15;
 constexpr uint32_t kDrawIni = 27;   // + j, t = 0xFFFFFFFE: the initial-state errors (DESIGN.md section 11)
+constexpr int kAlignN = 10;         // alignment: accelerometer samples averaged for roll and pitch (ins_loose.py:72)
+constexpr int kAlignGps = 2;        // EkfParams::align of B2INS_ALIGN_GPS: yaw is the fix row's course over ground
 
 struct EkfParams {
   int64_t n, runs, run_offset, m;
@@ -65,7 +67,32 @@ struct EkfParams {
   double* proc_stats;              // [runs][3][9] max|e|, mean, std of att, pos, vel
   int64_t proc_start;
   int proc_pos_frame;
+  // alignment (DESIGN.md section 11): B2INS_ALIGN_* (0: off, the initial state is ini + the P0 draw); the given
+  // yaw; P0 of the level N / E misalignment and of the given yaw; the gyro's arw^2 per axis
+  int align;
+  double align_yaw, align_p0[3], arw2[3];
 };
+
+// The GPS row an aligned run starts at: the latest visible row at sample <= kAlignN - 1, else the first
+// visible row after it; -1 without a visible row in the series.  GPS rows and visibility are common to all runs.
+__device__ __forceinline__ int64_t ekf_fix_row(const EkfParams& p) {
+  int64_t f = -1;
+  for (int64_t j = 0; j < p.m; ++j) {
+    if (p.gps_idx[j] >= p.n) break;
+    const bool late = p.gps_idx[j] > kAlignN - 1;
+    if (late && f >= 0) break;
+    if (p.gps_vis[j] > 0.0) {
+      f = j;
+      if (late) break;
+    }
+  }
+  return f;
+}
+
+// First sample of an aligned run's filter: max(kAlignN - 1, the fix row's sample); n without a fix row
+__device__ __forceinline__ int64_t ekf_align_start(const EkfParams& p, int64_t fix) {
+  return fix < 0 ? p.n : max(static_cast<int64_t>(kAlignN - 1), p.gps_idx[fix]);
+}
 
 // 3 x 3 symmetric-positive NEES  e^T A^-1 e  via the adjugate
 __device__ __forceinline__ double nees3(const double* a /* row-major 3x3 */, const double* e) {
@@ -136,13 +163,25 @@ __device__ __forceinline__ int ekf_own(int q, int m) {
 // in the data).  Lane q reads the channels it would generate, so the quad shuffles that build f and w are
 // the same; sample i + 1 and the next GPS row are loaded a step / an epoch before they are used.  The
 // consistency record needs the true biases and is compiled out; end_err is written when ref_nav is given.
+// Alignment (p.align, a uniform run-time flag): the run initialises itself from its measurements instead of
+// ini + the P0 draw.  Lanes q < 3 sum their accelerometer channel over samples 0..kAlignN-1 (a separate pass
+// with its own Gauss-Markov carries; the quad shuffles replicate the mean) for roll and pitch at kAlignN - 1;
+// yaw is given or the course of the fix row's GPS velocity (the draws that row's update would use).  The
+// attitude alone then propagates (att_step: no Earth or transport rate) to the start sample s0, where
+// position and velocity are the fix row as measured and P is the per-run diagonal P0; the filter runs from
+// s0 with the first GPS row after it.  History rows before the state exists are NaN, the consistency record
+// takes epochs after s0 and the process statistics start at max(proc_start, s0).
 // PROC: per-run process-error statistics (proc_stats), taken where history row i is written -- after the GPS
 // update of sample i -- against ref_nav row i for i >= proc_start.  The nominal state is replicated, so lane
 // q < 3 of a run takes column group q (attitude, position, velocity) with no shuffle; its accumulators live
 // in shared memory behind P, as [12][32 lanes], and lane 0 writes the run's [3][9] at the end.
-template <bool VIB, bool FED, bool PROC>
+// FA (FED only): alignment is compiled in and on; on supplied data it is a compile-time choice, because the
+// run-time flag costs the fed form spills (ptxas -v).
+template <bool VIB, bool FED, bool PROC, bool FA = false>
 __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant__ EkfParams p) {
   static_assert(!(VIB && FED), "supplied measurements carry their vibration already");
+  static_assert(FED || !FA, "generated measurements select the alignment at run time (p.align)");
+  const bool aligned = FED ? FA : (p.align != 0);
   static_assert(!(FED && PROC), "supplied-data histories are on the host: their statistics are taken there");
   constexpr int kAcc = PROC ? 12 * kEkfThreads : 0;    // 3 KB: max, sum, sum of squares, shift, 3 columns each
   __shared__ double Psm[kEkfN * kEkfN * kEkfRuns + kAcc];      // 14.4 KB (+ 3 KB)
@@ -177,24 +216,24 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
     sdp1 = div_nr(div_nr(sdp1, gp.rn), gp.cl);
   }
 
-  // ---- initial covariance and nominal state: truth + a draw from P0 -----------------------------
-  for (int m = 0; m < 4; ++m) {
-    const int r = ekf_own(q, m);
-    if (q < 3 || m < 3)
-      for (int c = 0; c < kEkfN; ++c) P(r, c) = (r == c) ? p.p0[r] : 0.0;
-  }
-  double e0[10];
-#pragma unroll
-  for (int j = 0; j < 5; ++j) {
-    Normal2 z{0.0, 0.0};        // FED without ini_draw: a zero draw through the same code
-    if (!FED || p.ini_draw) z = normal_pair(0xFFFFFFFEu, kDrawIni + j, run_lo, run_hi, p.k0, p.k1);
-    e0[2 * j] = z.z0;
-    e0[2 * j + 1] = z.z1;
-  }
-#pragma unroll
-  for (int i = 0; i < 9; ++i) e0[i] *= sqrt(p.p0[i]);
+  // ---- initial covariance and nominal state: truth + a draw from P0 (aligned: at s0, below) -------
   NavState st;
-  {
+  if (!aligned) {
+    for (int m = 0; m < 4; ++m) {
+      const int r = ekf_own(q, m);
+      if (q < 3 || m < 3)
+        for (int c = 0; c < kEkfN; ++c) P(r, c) = (r == c) ? p.p0[r] : 0.0;
+    }
+    double e0[10];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      Normal2 z{0.0, 0.0};        // FED without ini_draw: a zero draw through the same code
+      if (!FED || p.ini_draw) z = normal_pair(0xFFFFFFFEu, kDrawIni + j, run_lo, run_hi, p.k0, p.k1);
+      e0[2 * j] = z.z0;
+      e0[2 * j + 1] = z.z1;
+    }
+#pragma unroll
+    for (int i = 0; i < 9; ++i) e0[i] *= sqrt(p.p0[i]);
     double ini[9];
 #pragma unroll
     for (int i = 0; i < 9; ++i) ini[i] = p.ini[i];
@@ -263,9 +302,172 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
 #pragma unroll
     for (int k = 0; k < 6; ++k) ng[k] = p.m > 0 ? fgps[k] : 0.0;
   }
+  // the measurements of sample i (the K12 generator, shared out over the quad): lane q's channels c0, c1 into
+  // m0, m1, whose Gauss-Markov drifts cr0, cr1 carry; FED: sample i, loaded a step before, and sample i + 1
+  auto measure = [&](int64_t i, double& cr0, double& cr1, double& m0, double& m1) {
+    if constexpr (FED) {
+      // sample i was loaded during step i - 1; sample i + 1 <= n - 1 is loaded now, a step before its use
+      m0 = nx0;
+      m1 = nx1;
+      nx0 = fch0[(i + 1) * 3];
+      nx1 = fch1[(i + 1) * 3];
+    } else {
+      const uint32_t t = static_cast<uint32_t>(i);
+      const double* ref0 = (c0 < 3) ? p.ref_accel + i * 3 + c0 : p.ref_gyro + i * 3 + (c0 - 3);
+      const Normal2 z0 = normal_pair(t, static_cast<uint32_t>(c0), run_lo, run_hi, p.k0, p.k1);
+      m0 = ((ref0[0] + b0) + w0 * z0.z1) + (cr0 + wd0 * z0.z0);
+      cr0 = fma(ga0, cr0, gb0 * z0.z0);
+      // every lane runs a second chain (lanes 2 and 3 repeat their first draw and drop the result): no
+      // divergent branch, and the two Box-Muller chains of a lane interleave
+      const int cc = two ? c1 : c0;
+      const double* ref1 = (cc < 3) ? p.ref_accel + i * 3 + cc : p.ref_gyro + i * 3 + (cc - 3);
+      const Normal2 z1 = normal_pair(t, static_cast<uint32_t>(cc), run_lo, run_hi, p.k0, p.k1);
+      m1 = ((ref1[0] + b1) + w1 * z1.z1) + (cr1 + wd1 * z1.z0);
+      cr1 = two ? fma(ga1, cr1, gb1 * z1.z0) : 0.0;
+      if constexpr (VIB) {
+        // vib_term's models (1 random, 2 sinusoidal, 3 series), added last as in oracle_np.sensor_gen.
+        // Random: lane q < 3 draws pair kDrawVib + q, whose z0 is its own accelerometer axis and whose z1
+        // (gyro axis q) belongs to lane (q + 3) & 3 -- one quad shuffle from lane (q + 1) & 3; lane 3's
+        // draw is dropped
+        const int ta = p.accel.vib_type, tg = p.gyro.vib_type;
+        double va = 0.0, vg = 0.0;
+        if ((ta == 1) | (tg == 1)) {
+          const Normal2 zv = normal_pair(t, kDrawVib + vax, run_lo, run_hi, p.k0, p.k1);
+          const double zvg = quad(zv.z1, (q + 1) & 3);
+          if (ta == 1) va = vamp_a * zv.z0;
+          if (tg == 1) vg = vamp_g * zvg;
+        }
+        if (ta == 2) va = vamp_a * sin(p.accel.vib_w * static_cast<double>(t) + 0.0);
+        if (tg == 2) vg = vamp_g * sin(p.gyro.vib_w * static_cast<double>(t) + vphase);
+        if (ta == 3) va = vser_a[t % static_cast<uint32_t>(p.accel.series_len)];
+        if (tg == 3) vg = vser_g[t % static_cast<uint32_t>(p.gyro.series_len)];
+        m0 += (q < 3) ? va : vg;
+        m1 += vg;
+      }
+    }
+  };
+  int64_t i0 = 0;                          // first sample of the filter
+  if (aligned) {
+    // ---- alignment: levelling at kAlignN - 1, the attitude alone to s0 = i0, the state and P0 at s0 ---
+    const int64_t jf = ekf_fix_row(p);
+    i0 = ekf_align_start(p, jf);
+    const double qnan = __longlong_as_double(0x7ff8000000000000LL);
+    // the fix row as measured (uniform branch): the GPS draws its update would use; FED: the supplied row
+    double fx[6];
+    if (jf < 0) {
+#pragma unroll
+      for (int k = 0; k < 6; ++k) fx[k] = qnan;
+    } else if constexpr (FED) {
+#pragma unroll
+      for (int k = 0; k < 6; ++k) fx[k] = fgps[jf * 6 + k];
+    } else {
+      Normal2 zz{0.0, 0.0};
+      if (q < 3) zz = normal_pair(static_cast<uint32_t>(jf), kPairGps + q, run_lo, run_hi, p.k0, p.k1);
+      double zn[6];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        zn[2 * j] = quad(zz.z0, j);
+        zn[2 * j + 1] = quad(zz.z1, j);
+      }
+      const double* rg = p.ref_gps + jf * 6;
+      fx[0] = rg[0] + sdp0 * zn[0];
+      fx[1] = rg[1] + sdp1 * zn[1];
+      fx[2] = rg[2] + p.stdp[2] * zn[2];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) fx[3 + k] = rg[3 + k] + p.stdv[k] * zn[3 + k];
+    }
+    // levelling: the mean of accelerometer samples 0..kAlignN-1 (ins_loose.py:76-91)
+    double asum = 0.0;
+    {
+      double l0 = 0.0, l1 = 0.0;
+      for (int64_t i = 0; i < kAlignN; ++i) {
+        double a0, a1;
+        if constexpr (FED)
+          a0 = fch0[i * 3];
+        else
+          measure(i, l0, l1, a0, a1);
+        asum += a0;
+      }
+    }
+    const double ax = quad(asum, 0) / kAlignN, ay = quad(asum, 1) / kAlignN, az = quad(asum, 2) / kAlignN;
+    const double nrm = sqrt(ax * ax + ay * ay + az * az);
+    AttState a;
+    a.yaw = (p.align == kAlignGps) ? atan2(fx[4], fx[3]) : p.align_yaw;
+    a.pitch = asin(ax / nrm);
+    a.roll = atan2(-(ay / nrm), -(az / nrm));
+    att_exact(a);
+    a.icp = rcp_nr(a.sc.cp) * dt;
+    for (int64_t i = 0; i < i0; ++i) {
+      int64_t row;
+      if (dump && dump_row_generic(p.dump_stride, i, &row)) {
+        const int64_t o = (run * p.dump_rows + row) * 3;
+        const bool up = i >= kAlignN - 1;
+        p.out_att[o] = up ? wrap_once(a.yaw) : qnan;
+        p.out_att[o + 1] = up ? a.pitch : qnan;
+        p.out_att[o + 2] = up ? wrap_once(a.roll) : qnan;
+#pragma unroll
+        for (int c3 = 0; c3 < 3; ++c3) {
+          p.out_pos[o + c3] = qnan;
+          p.out_vel[o + c3] = qnan;
+          p.out_wb[o + c3] = 0.0;
+          p.out_ab[o + c3] = 0.0;
+        }
+      }
+      if (i == p.n - 1) break;
+      double m0, m1;
+      measure(i, carry0, carry1, m0, m1);
+      const Vec3 w{quad(m0, 3), quad(m1, 0), quad(m1, 1)};
+      if (i >= kAlignN - 1) att_step(a, w, dt, ((i + 1) & (kResync - 1)) == 0);
+    }
+    // the state at s0: position and velocity as measured, the attitude with exact sin/cos (and the latitude's)
+    st.pos = Vec3{fx[0], fx[1], fx[2]};
+    st.vel = Vec3{fx[3], fx[4], fx[5]};
+    st.vel_b = Vec3{0.0, 0.0, 0.0};
+    st.g = 0.0;
+    st.fixed_g = false;
+    set_attitude(st, a.yaw, a.pitch, a.roll, dt);
+    // P0 at s0 (diagonal): the level / yaw variances plus the gyro's growth over the gap, the rest as p0
+    const double gap = static_cast<double>(i0 - (kAlignN - 1)) * dt;
+    double yv = p.align_p0[2];
+    if (p.align == kAlignGps) {
+      const double vn = fx[3], ve = fx[4], h2 = vn * vn + ve * ve;
+      yv = (p.stdv[0] * p.stdv[0] * (ve * ve) + p.stdv[1] * p.stdv[1] * (vn * vn)) / (h2 * h2);
+    }
+    for (int m = 0; m < 4; ++m) {
+      const int r = ekf_own(q, m);
+      double d = p.p0[r];
+      if (r >= 6 && r < 9) {
+        const int c = r - 6;
+        d = ((c == 2) ? yv : p.align_p0[c]) + (p.arw2[c] * gap + p.p0[9 + c] * (gap * gap));
+      }
+      if (q < 3 || m < 3)
+        for (int c = 0; c < kEkfN; ++c) P(r, c) = (r == c) ? d : 0.0;
+    }
+    if constexpr (PROC) {
+      // statistics from proc_start < s0 start at s0: its error is the shift of the accumulators
+      if (q < 3 && p.proc_start < i0 && i0 < p.n) {
+        const double* rn9 = p.ref_nav + i0 * 9;
+        double e[3];
+        if (q == 0)
+          proc_err_att(st, rn9, e);
+        else if (q == 1)
+          proc_err_pos<0>(st, rn9, p.proc_pos_frame, e);
+        else
+          proc_err_vel(st, rn9, e);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[(9 + c) * kEkfThreads] = e[c];
+      }
+    }
+    while (jg < p.m && p.gps_idx[jg] <= i0) ++jg;       // the fix row and those before it are used
+    next_gps = jg < p.m ? p.gps_idx[jg] : -1;
+    if constexpr (FED) {
+#pragma unroll
+      for (int k = 0; k < 6; ++k) ng[k] = jg < p.m ? fgps[jg * 6 + k] : 0.0;
+    }
+  }
   __syncwarp();
 
-  for (int64_t i = 0; i < p.n; ++i) {
+  for (int64_t i = i0; i < p.n; ++i) {
     // ================= GPS sample of IMU sample i: update, then the consistency record ==========
     if (i == next_gps) {
       if (p.gps_vis[jg] > 0.0) {
@@ -432,47 +634,8 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
     }
     if (i == p.n - 1) break;
     // ================= the measurements of sample i (the K12 generator, shared out over the quad) ==
-    double m0, m1 = 0.0;
-    if constexpr (FED) {
-      // sample i was loaded during step i - 1; sample i + 1 <= n - 1 is loaded now, a step before its use
-      m0 = nx0;
-      m1 = nx1;
-      nx0 = fch0[(i + 1) * 3];
-      nx1 = fch1[(i + 1) * 3];
-    } else {
-      const uint32_t t = static_cast<uint32_t>(i);
-      const double* ref0 = (c0 < 3) ? p.ref_accel + i * 3 + c0 : p.ref_gyro + i * 3 + (c0 - 3);
-      const Normal2 z0 = normal_pair(t, static_cast<uint32_t>(c0), run_lo, run_hi, p.k0, p.k1);
-      m0 = ((ref0[0] + b0) + w0 * z0.z1) + (carry0 + wd0 * z0.z0);
-      carry0 = fma(ga0, carry0, gb0 * z0.z0);
-      // every lane runs a second chain (lanes 2 and 3 repeat their first draw and drop the result): no
-      // divergent branch, and the two Box-Muller chains of a lane interleave
-      const int cc = two ? c1 : c0;
-      const double* ref1 = (cc < 3) ? p.ref_accel + i * 3 + cc : p.ref_gyro + i * 3 + (cc - 3);
-      const Normal2 z1 = normal_pair(t, static_cast<uint32_t>(cc), run_lo, run_hi, p.k0, p.k1);
-      m1 = ((ref1[0] + b1) + w1 * z1.z1) + (carry1 + wd1 * z1.z0);
-      carry1 = two ? fma(ga1, carry1, gb1 * z1.z0) : 0.0;
-      if constexpr (VIB) {
-        // vib_term's models (1 random, 2 sinusoidal, 3 series), added last as in oracle_np.sensor_gen.
-        // Random: lane q < 3 draws pair kDrawVib + q, whose z0 is its own accelerometer axis and whose z1
-        // (gyro axis q) belongs to lane (q + 3) & 3 -- one quad shuffle from lane (q + 1) & 3; lane 3's
-        // draw is dropped
-        const int ta = p.accel.vib_type, tg = p.gyro.vib_type;
-        double va = 0.0, vg = 0.0;
-        if ((ta == 1) | (tg == 1)) {
-          const Normal2 zv = normal_pair(t, kDrawVib + vax, run_lo, run_hi, p.k0, p.k1);
-          const double zvg = quad(zv.z1, (q + 1) & 3);
-          if (ta == 1) va = vamp_a * zv.z0;
-          if (tg == 1) vg = vamp_g * zvg;
-        }
-        if (ta == 2) va = vamp_a * sin(p.accel.vib_w * static_cast<double>(t) + 0.0);
-        if (tg == 2) vg = vamp_g * sin(p.gyro.vib_w * static_cast<double>(t) + vphase);
-        if (ta == 3) va = vser_a[t % static_cast<uint32_t>(p.accel.series_len)];
-        if (tg == 3) vg = vser_g[t % static_cast<uint32_t>(p.gyro.series_len)];
-        m0 += (q < 3) ? va : vg;
-        m1 += vg;
-      }
-    }
+    double m0, m1;
+    measure(i, carry0, carry1, m0, m1);
     const Vec3 f{quad(m0, 0) - ba[0], quad(m0, 1) - ba[1], quad(m0, 2) - ba[2]};
     const Vec3 w{quad(m0, 3) - bg[0], quad(m1, 0) - bg[1], quad(m1, 1) - bg[2]};
     // ================= covariance: P <- Phi P Phi^T + Q with the blocks of Phi ====================
@@ -579,7 +742,9 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   if (active && q == 0) {
     if constexpr (PROC) {
       double* o = p.proc_stats + run * 27;
-      const double inv = 1.0 / static_cast<double>(p.n - p.proc_start);
+      const int64_t ps = p.align ? max(p.proc_start, ekf_align_start(p, ekf_fix_row(p))) : p.proc_start;
+      // no fix in the series (ps = n): NaN statistics
+      const double inv = ps < p.n ? 1.0 / static_cast<double>(p.n - ps) : __longlong_as_double(0x7ff8000000000000LL);
 #pragma unroll
       for (int g = 0; g < 3; ++g) {
         const double* a = acc + g * kEkfRuns;          // lane g * 8 + rs

@@ -484,6 +484,44 @@ def _ekf_result(out, runs, n, dump_runs, dump_stride, dev, end_err):
     return res
 
 
+ALIGN_N = 10       # alignment: accelerometer samples averaged for roll and pitch (ins_loose.py:72)
+
+
+def align_fix(gps_idx, gps_vis):
+    """(fix row, start sample) of an aligned filter (b2ins_ekf_align): the latest visible GPS row at or before
+    sample ALIGN_N - 1, else the first visible row after it, and max(ALIGN_N - 1, its sample); (None, None)
+    without a visible row.  gps_idx, gps_vis: host arrays [m]."""
+    gps_idx = np.asarray(gps_idx, dtype=np.int64).reshape(-1)
+    vis = np.nonzero(np.asarray(gps_vis, dtype=np.float64).reshape(-1) > 0.0)[0]
+    if vis.size == 0:
+        return None, None
+    before = vis[gps_idx[vis] <= ALIGN_N - 1]
+    j = int(before[-1]) if before.size else int(vis[0])
+    return j, max(ALIGN_N - 1, int(gps_idx[j]))
+
+
+def _ekf_ini(ini, align):
+    """The initial state of a K7 launch: ini, which an aligned launch does not use (zeros if None)."""
+    if ini is None:
+        if align is None:
+            raise ValueError('the filter needs its initial state ini (or align)')
+        return np.zeros(9)
+    return ini
+
+
+def _ekf_align(align):
+    """b2ins_ekf_align of align = (yaw, yaw_var): yaw a heading [rad] or 'gps' (the fix row's course)."""
+    a = _lib.EkfAlign()
+    yaw, yaw_var = align
+    if isinstance(yaw, str):
+        if yaw != 'gps':
+            raise ValueError("align yaw must be a heading in rad or 'gps'")
+        a.mode = _lib.ALIGN_GPS
+    else:
+        a.mode, a.yaw, a.yaw_var = _lib.ALIGN_YAW, float(yaw), float(yaw_var)
+    return a
+
+
 class EkfResult:
     """Device-side results of one loosely-coupled-filter launch (K7)."""
 
@@ -493,12 +531,13 @@ class EkfResult:
         self.consist = None      # [R,19] NEES sums (pos, vel, att), inside-3-sigma counts [15], epochs
         self.proc_stats = None   # [R,3,9] max|e|, mean, std of att, pos, vel per run (proc_start given)
         self.att = self.pos = self.vel = self.wb = self.ab = None   # [dump_runs,rows,3]
+        self.start = 0           # first sample of the filter (aligned: the fix sample, align_fix)
 
 
 def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_accel, ref_nav, ref_gps,
               gps_idx, gps_vis, run_offset=0, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True,
               stats_start=0, dump_runs=0, dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0,
-              vib_gyro=None, vib_accel=None, proc_start=None, proc_pos_frame=0):
+              vib_gyro=None, vib_accel=None, proc_start=None, proc_pos_frame=0, align=None):
     """K7: Monte-Carlo loosely-coupled GNSS/INS filter (the spec: DESIGN.md section 11; csrc/ekf_kernel.cuh).
     ref_gyro, ref_accel [n,3], ref_nav [n,9], ref_gps [m,6], gps_vis [m]: CUDA f64; gps_idx [m]: CUDA
     int64 (IMU sample index of every GPS row).  ini: the 9 true initial values (LLA, body velocity, Euler
@@ -506,15 +545,18 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     them (a parsed dict, or a Vib such as vib_series over K5 series of exactly these runs); the filter
     model does not include it (vel_rw / att_rw, DESIGN.md section 11).  proc_start (sample index in [0, n)):
     also res.proc_stats [R,3,9], the per-run process-error statistics of samples >= proc_start, positions as
-    POS_FRAME_* proc_pos_frame (b2ins_ins_loose_proc_f64); every other output is unchanged.  Asynchronous on
-    the current stream."""
+    POS_FRAME_* proc_pos_frame (b2ins_ins_loose_proc_f64); every other output is unchanged.  align = (yaw, yaw_var):
+    every run initialises itself from its measurements (b2ins_ins_loose_align_f64; yaw a heading [rad] with
+    variance yaw_var, or 'gps'); ini is then unused, res.start is the fix sample (align_fix), the consistency
+    record takes the epochs after it and proc statistics start at max(proc_start, res.start).  Asynchronous on
+    the current stream (with align, after one host copy of gps_idx / gps_vis)."""
     _require_cuda()
     lib = _lib.load()
     n, m = ref_gyro.shape[0], ref_gps.shape[0]
     dev = ref_gyro.device
     assert gps_idx.dtype == torch.int64 and gps_idx.is_cuda and gps_idx.is_contiguous()
-    cfg = _ekf_config(fs, n, runs, m, seed, gyro_err, accel_err, gps_err, ini, run_offset, ini_att_std, earth_rot,
-                      stats_start, dump_runs, dump_stride, vel_rw, att_rw)
+    cfg = _ekf_config(fs, n, runs, m, seed, gyro_err, accel_err, gps_err, _ekf_ini(ini, align), run_offset,
+                      ini_att_std, earth_rot, stats_start, dump_runs, dump_stride, vel_rw, att_rw)
     # Vib structs are passed by pointer; a VIB_SERIES Vib keeps its series tensor alive through the call
     vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
@@ -523,7 +565,13 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     refs = (_ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps), ctypes.c_void_p(gps_idx.data_ptr()),
             _ptr(gps_vis), _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.consist))
     dumps = (_ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream())
-    if proc_start is None:
+    if align is not None:
+        res.start = align_fix(gps_idx.cpu().numpy(), gps_vis.cpu().numpy())[1]
+        res.proc_stats = None if proc_start is None else _reuse(res.proc_stats, (runs, 3, 9), dev)
+        _lib.check(lib.b2ins_ins_loose_align_f64(
+            ctypes.byref(cfg), ctypes.byref(_ekf_align(align)), ctypes.byref(vg), ctypes.byref(va),
+            -1 if proc_start is None else int(proc_start), int(proc_pos_frame), *refs, _ptr(res.proc_stats), *dumps))
+    elif proc_start is None:
         res.proc_stats = None
         _lib.check(lib.b2ins_ins_loose_ex_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), *refs, *dumps))
     else:
@@ -536,14 +584,15 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
 
 def ins_loose_fed(fs, gyro, accel, gps, gps_idx, gps_vis, gyro_err, accel_err, gps_err, ini, seed=0, ini_draw=False,
                   run_offset=0, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True, ref_nav=None, dump_runs=0,
-                  dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0):
+                  dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0, align=None):
     """K7 on supplied measurements (b2ins_ins_loose_fed_f64): gyro, accel [R,n,3] and gps [R,m,6] (LLA rad, m;
     NED m/s) CUDA f64, run-major; gps_idx [m] CUDA int64, strictly ascending IMU sample indices of the GPS rows;
     gps_vis [m] CUDA f64.  gyro_err / accel_err / gps_err are the filter's model (Q, R, P0) only.  Every run
     starts at ini, plus with ini_draw the P0 draw of global run run_offset + r under seed (the generated
     experiment's draw).  ref_nav [n,9] (optional): end_err as engine.ins_loose makes it.  Returns an
-    EkfResult without consist (and without end_err when ref_nav is None).  Asynchronous on the current
-    stream."""
+    EkfResult without consist (and without end_err when ref_nav is None).  align = (yaw, yaw_var): every run
+    initialises itself from its measurements instead (b2ins_ins_loose_fed_align_f64; ini, seed and ini_draw are
+    unused), res.start is the fix sample.  Asynchronous on the current stream."""
     _require_cuda()
     lib = _lib.load()
     R, n, three = gyro.shape
@@ -556,12 +605,16 @@ def ins_loose_fed(fs, gyro, accel, gps, gps_idx, gps_vis, gyro_err, accel_err, g
     if ref_nav is not None and tuple(ref_nav.shape) != (n, 9):
         raise ValueError('ref_nav must be [n, 9]')
     assert gps_idx.dtype == torch.int64 and gps_idx.is_cuda and gps_idx.is_contiguous()
-    cfg = _ekf_config(fs, n, R, m, seed, gyro_err, accel_err, gps_err, ini, run_offset, ini_att_std, earth_rot,
-                      -1, dump_runs, dump_stride, vel_rw, att_rw)
+    cfg = _ekf_config(fs, n, R, m, seed, gyro_err, accel_err, gps_err, _ekf_ini(ini, align), run_offset, ini_att_std,
+                      earth_rot, -1, dump_runs, dump_stride, vel_rw, att_rw)
     res = _ekf_result(out, R, n, dump_runs, dump_stride, gyro.device, end_err=ref_nav is not None)
     res.consist = None
-    _lib.check(lib.b2ins_ins_loose_fed_f64(
-        ctypes.byref(cfg), int(bool(ini_draw)), _ptr(gyro), _ptr(accel), _ptr(gps), ctypes.c_void_p(gps_idx.data_ptr()),
-        _ptr(gps_vis), _ptr(ref_nav), _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.att), _ptr(res.pos),
-        _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream()))
+    bufs = (_ptr(gyro), _ptr(accel), _ptr(gps), ctypes.c_void_p(gps_idx.data_ptr()), _ptr(gps_vis), _ptr(ref_nav),
+            _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb),
+            _ptr(res.ab), _stream())
+    if align is None:
+        _lib.check(lib.b2ins_ins_loose_fed_f64(ctypes.byref(cfg), int(bool(ini_draw)), *bufs))
+    else:
+        res.start = align_fix(gps_idx.cpu().numpy(), gps_vis.cpu().numpy())[1]
+        _lib.check(lib.b2ins_ins_loose_fed_align_f64(ctypes.byref(cfg), ctypes.byref(_ekf_align(align)), *bufs))
     return res

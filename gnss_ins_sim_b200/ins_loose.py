@@ -13,7 +13,8 @@ streams), filters them, and leaves end-point errors, bias estimates and a consis
 It is driven by gnss_ins_sim_b200.sim.Sim (ref_frame 0, IMU(gps=True), fs = [fs_imu, fs_gps, 0]).  The same
 filter also runs on SUPPLIED measurements (a drive log, another simulator, a saved experiment): run_batch() for
 R runs in one launch, the reference's per-run .run(set_of_input), and Sim on a logged-data directory.  There it
-needs its noise model, InsLoose(imu=IMU(..., gps=True)), and an initial state.
+needs its noise model, InsLoose(imu=IMU(..., gps=True)), and an initial state -- or InsLoose(align_yaw=...), with
+which it initialises itself from its measurements as the reference's InsLoose.ins_loose does (ins_loose.py:54-126).
 """
 import numpy as np
 import torch
@@ -56,7 +57,7 @@ class InsLoose(object):
     '''
 
     def __init__(self, ini_pos_vel_att=None, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True,
-                 vel_model_std=0.02, att_model_std=0.0, imu=None):
+                 vel_model_std=0.02, att_model_std=0.0, imu=None, align_yaw=None):
         '''
         Args:
             ini_pos_vel_att: (9,) true initial LLA [rad, rad, m], body velocity, ZYX Euler angles; None:
@@ -81,6 +82,21 @@ class InsLoose(object):
             vel_model_std = sqrt(0.02**2 + sa**2 * dt),   att_model_std = sg * sqrt(dt)
         (plus any att_model_std of its own, in quadrature).  With the default model the velocity and
         attitude blocks become overconfident (DESIGN.md section 11 has the figures).
+
+        align_yaw: None (default): every run starts at the initial state above plus a draw from the initial
+            covariance.  A heading [rad] or 'gps': every run initialises itself from its own measurements, with no
+            initial state (DESIGN.md section 11, "Alignment"):
+              - roll and pitch from the mean of the first 10 accelerometer samples, at sample 9
+                (ins_loose.py:76-91); yaw is align_yaw (1-sigma ini_att_std[2]) or, with 'gps', the course over
+                ground atan2(v_E, v_N) of the fix row's GPS velocity (a land vehicle moving forward);
+              - the fix row is the latest visible GPS row at or before sample 9, else the first visible one
+                after it: position and velocity as measured there, the attitude propagated alone until then;
+              - P0 from the sensor models (level: accelerometer bias and noise; yaw: ini_att_std[2] or the
+                course variance from the GPS velocity noise; the gyro's growth over the gap).
+            History rows before the state exists are NaN; the consistency record and the process statistics
+            start at the fix sample.  The error model is small-angle: the heading converges only from yaw errors
+            the yaw P0 covers, so use 'gps' for a start in motion (a 'gps' fix needs >= 1 m/s horizontal
+            speed).  Not together with ini_pos_vel_att.
         '''
         self.input = ['fs', 'gyro', 'accel', 'time', 'gps_time', 'gps']   # ins_loose.py:31
         self.output = ['pos', 'vel', 'att_euler', 'wb', 'ab']             # ins_loose.py:32
@@ -94,11 +110,39 @@ class InsLoose(object):
         if imu is not None and not getattr(imu, 'gps', False):
             raise ValueError('InsLoose(imu=...) needs an IMU with gps=True: its GPS errors are the filter\'s R')
         self.imu = imu
+        if align_yaw is not None:
+            if ini_pos_vel_att is not None:
+                raise ValueError('InsLoose: align_yaw and ini_pos_vel_att exclude each other')
+            if not (align_yaw == 'gps' or (not isinstance(align_yaw, str) and np.isfinite(float(align_yaw)))):
+                raise ValueError("align_yaw must be a heading in rad or 'gps'")
+        self.align_yaw = align_yaw if align_yaw is None or align_yaw == 'gps' else float(align_yaw)
+
+    def align(self):
+        """engine's align argument: None, or (align_yaw, its variance ini_att_std[2]^2)."""
+        return None if self.align_yaw is None else (self.align_yaw, self.ini_att_std[2] ** 2)
+
+    def check_alignment(self, n, gps_idx, gps_vis, gps_vel):
+        """The host checks of an aligned launch, ValueError before any launch: n >= 10 IMU samples, a visible GPS
+        row and, with 'gps', a horizontal speed >= 1 m/s at the fix row in every run.  gps_vel [..., m, 2]
+        (v_N, v_E; numpy or a CUDA tensor, of which only the fix row is copied).  Returns the fix sample."""
+        if n < engine.ALIGN_N:
+            raise ValueError('InsLoose(align_yaw=...) needs at least %d IMU samples (got %d)' % (engine.ALIGN_N, n))
+        j, start = engine.align_fix(gps_idx, gps_vis)
+        if j is None:
+            raise ValueError('InsLoose(align_yaw=...) needs a visible GPS row')
+        if self.align_yaw == 'gps':
+            v = gps_vel[..., j, :]
+            v = np.asarray(v.cpu().numpy() if torch.is_tensor(v) else v, dtype=np.float64)
+            if not np.all(np.hypot(v[..., 0], v[..., 1]) >= 1.0):
+                raise ValueError("InsLoose(align_yaw='gps') needs a horizontal speed of at least 1 m/s at the fix "
+                                 "row (GPS row %d)" % j)
+        return start
 
     def run(self, set_of_input):
         '''
         One run of the reference protocol: set_of_input = [fs, gyro (n,3) rad/s, accel (n,3) m/s^2, time (n,)
-        s, gps_time (m,) s, gps (m,6) LLA rad, m, NED m/s].  Every GPS row is used; the run starts at ini.
+        s, gps_time (m,) s, gps (m,6) LLA rad, m, NED m/s].  Every GPS row is used; the run starts at ini, or
+        aligns itself with align_yaw.
         '''
         fs, gyro, accel, time, gps_time, gps = set_of_input
         out = self.run_batch(fs, np.asarray(gyro, dtype=np.float64)[None], np.asarray(accel, dtype=np.float64)[None],
@@ -120,7 +164,7 @@ class InsLoose(object):
         gps_time [m] s; gps [R, m, 6] (LLA rad, m; NED m/s); gps_visibility [m] (None: every row is used).  GPS
         row j is applied at the IMU sample nearest to gps_time[j] (gps_sample_index).  seed None: every run
         starts at ini; an integer: ini plus the initial-covariance draw of run run_times + r under that seed,
-        as a generated experiment draws it.  Returns pos, vel, att_euler, wb, ab [R, n, 3] (numpy, or CUDA
+        as a generated experiment draws it.  With align_yaw every run aligns itself (seed is unused).  Returns pos, vel, att_euler, wb, ab [R, n, 3] (numpy, or CUDA
         tensors if not to_host).
         '''
         imu = self.model()
@@ -154,12 +198,16 @@ class InsLoose(object):
 
     def launch(self, fs, gyro, accel, gps, gps_idx, gps_vis, imu, ini, seed, ini_draw, run_offset, ref_nav=None):
         """engine.ins_loose_fed with this filter's options and histories of every run: gyro, accel [R,n,3], gps
-        [R,m,6], ref_nav [n,9] (optional) CUDA; gps_idx, gps_vis [m] host arrays."""
-        if ini is None:
-            raise ValueError('InsLoose on supplied measurements needs ini_pos_vel_att')
+        [R,m,6], ref_nav [n,9] (optional) CUDA; gps_idx, gps_vis [m] host arrays.  With align_yaw, ini is unused
+        and the alignment's host checks run first."""
+        if self.align_yaw is not None:
+            self.check_alignment(gyro.shape[1], gps_idx, gps_vis, gps[:, :, 3:5])
+        elif ini is None:
+            raise ValueError('InsLoose on supplied measurements needs ini_pos_vel_att (or align_yaw)')
         R = gyro.shape[0]
         return engine.ins_loose_fed(fs, gyro, accel, gps, torch.from_numpy(np.asarray(gps_idx, dtype=np.int64)).cuda(),
                                     engine.to_device(gps_vis), imu.gyro_err, imu.accel_err, imu.gps_err, ini,
                                     seed=seed, ini_draw=ini_draw, run_offset=run_offset,
                                     ini_att_std=self.ini_att_std, earth_rot=self.earth_rot, ref_nav=ref_nav,
-                                    dump_runs=R, vel_rw=self.vel_model_std, att_rw=self.att_model_std)
+                                    dump_runs=R, vel_rw=self.vel_model_std, att_rw=self.att_model_std,
+                                    align=self.align())

@@ -567,14 +567,16 @@ class Sim(object):
         row (velocity rotated to the body frame), plus the initial-covariance draw of run run_base + k under the
         Sim's seed, as the generated experiment draws it: a directory save_data wrote from a generated filter
         experiment filters back to that experiment.  Run blocks are sized to the free device memory (inputs and
-        histories: 168 B per run-sample).  End-point errors and their statistics if the reference files exist."""
+        histories: 168 B per run-sample).  End-point errors and their statistics if the reference files exist.
+        With InsLoose(align_yaw=...) every run initialises itself from its measurements: no initial state, no
+        draw, and no reference files needed."""
         d, name, R = self._logged, self.algo_name(i), self.sim_count
         if self.ref_frame != 0:
             raise ValueError('ins_loose works in ref_frame 0 (LLA positions, NED velocities)')
         imu = algo.model(self.imu)
         has_ref = all(k in d for k in ('ref_att_euler', 'ref_pos', 'ref_vel'))
         ini = algo.ini
-        if ini is None:
+        if ini is None and algo.align_yaw is None:
             if not has_ref:
                 raise ValueError('InsLoose on a data directory needs ini_pos_vel_att or the ref_pos, ref_vel and '
                                  'ref_att_euler files')
@@ -589,13 +591,14 @@ class Sim(object):
         ref_nav = engine.to_device(np.concatenate([d['ref_att_euler'], d['ref_pos'], d['ref_vel']], axis=1)) \
             if has_ref else None
         outs = {o: [] for o in ('pos', 'vel', 'att_euler', 'wb', 'ab')}
-        errs, bias = [], []
+        errs, bias, start = [], [], 0
         block = self._allan_block(168, 3)
         for r0 in range(0, R, block):
             r1 = min(R, r0 + block)
             res = algo.launch(self.fs[0], engine.to_device(gyro[r0:r1]), engine.to_device(accel[r0:r1]),
                               engine.to_device(gps[r0:r1]), gps_idx, vis, imu, ini, self.seed, True,
                               self.run_base + r0, ref_nav)
+            start = res.start
             for o, t in zip(outs, (res.pos, res.vel, res.att, res.wb, res.ab)):
                 outs[o].append(t.cpu().numpy())
             bias.append(res.end_bias.cpu().numpy())
@@ -607,7 +610,7 @@ class Sim(object):
             self.data[o] = dict(self.data[o]) if isinstance(self.data.get(o), dict) else {}
             self.data[o].update(_keyed(name, np.concatenate(parts)))
         self._mc[i] = {'base': 0, 'end_err': np.concatenate(errs) if has_ref else None,
-                       'end_bias': np.concatenate(bias)}
+                       'end_bias': np.concatenate(bias), 'start': start if R else 0}
         if has_ref:
             self.err_stats[name] = engine.error_stats(engine.to_device(self._mc[i]['end_err'])).cpu().numpy()
 
@@ -840,7 +843,11 @@ class Sim(object):
         gps = self._ekf_inputs()
         d = self._dev
         ini = algo.ini if algo.ini is not None else self._traj.get('ini')
-        if ini is None:
+        if algo.align_yaw is not None:
+            t = self._traj
+            algo.check_alignment(len(t['ref_gyro']), np.rint(np.asarray(t['gps_time']) * self.fs[0]),
+                                 t['gps_visibility'], t['ref_gps'][:, 3:5])
+        elif ini is None:
             raise ValueError('InsLoose needs ini_pos_vel_att (the trajectory carries no initial state)')
         vib_gyro, vib_acc = self._vib_pair(runs, r0)       # K5 (PSD) runs on the stream K7 runs on
         return engine.ins_loose(self.fs[0], runs, self.seed, self.imu.gyro_err, self.imu.accel_err,
@@ -850,7 +857,7 @@ class Sim(object):
                                 stats_start=stats_start, dump_runs=dump_runs, dump_stride=dump_stride,
                                 vel_rw=algo.vel_model_std, att_rw=algo.att_model_std,
                                 vib_gyro=vib_gyro, vib_accel=vib_acc, proc_start=proc_start,
-                                proc_pos_frame=proc_pos_frame)
+                                proc_pos_frame=proc_pos_frame, align=algo.align())
 
     def _ekf_blocks(self, algo, **kw):
         """K7 over this rank's shard (kw: _ekf_launch's), in run blocks sized to the free device memory with PSD
@@ -1038,7 +1045,8 @@ class Sim(object):
         err_stats_start == -1: end-point statistics over runs {'max','avg','std'} (3,) (sensor data: (3,) or
         (6,)).  Otherwise: per-run process statistics from that time [s]: dicts keyed by run key ('<algo>_<r>'
         for algorithm outputs, the run index for sensor data).  GPS process statistics start at the first
-        GPS sample at or after that time.
+        GPS sample at or after that time.  For InsLoose(align_yaw=...) the statistics start at the later of that
+        time and the fix sample (the first sample with a full state; earlier history rows are NaN).
         '''
         if data_name == 'odo':
             raise ValueError('odo has no error statistics: the odometer history is one column per run, and the '
@@ -1225,6 +1233,7 @@ class Sim(object):
         if key not in self._proc:
             start = _first_at(self.data['time'], start_s)
             if self._logged is not None:
+                start = max(start, self._mc.get(algo_index, {}).get('start', 0))     # aligned: from the fix
                 # the histories are on the host already (array_error + __array_stats,
                 # ins_data_manager.py:512-541, :797-808)
                 ps = np.zeros((self.sim_count, 3, 9))
@@ -1237,7 +1246,8 @@ class Sim(object):
                 ps = None
                 algo = self.algo[algo_index]
                 if hi > lo and isinstance(algo, InsLoose):
-                    # reduced inside the filter kernel: the histories of all runs would not fit
+                    # reduced inside the filter kernel (which starts aligned runs at the fix sample): the
+                    # histories of all runs would not fit
                     ps = torch.cat([r.proc_stats for r in self._ekf_blocks(algo, proc_start=start,
                                                                            proc_pos_frame=frame)])
                     ps = ps.reshape(hi - lo, 27)

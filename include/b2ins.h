@@ -217,6 +217,50 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
                             const double* ref_nav, double* end_err, double* end_bias, double* dump_att,
                             double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
 
+/* Alignment: the filter initialises itself from its measurements instead of starting at cfg->ini plus a P0
+ * draw (DESIGN.md section 11, "Alignment"; demo_algorithms/ins_loose.py:54-126).  Roll and pitch come from the
+ * mean of accelerometer samples 0..9 at sample 9; yaw is `yaw` (B2INS_ALIGN_YAW) or the course over ground
+ * atan2(v_E, v_N) of the fix row's GPS velocity (B2INS_ALIGN_GPS).  The fix row is the latest visible GPS row
+ * at or before sample 9, else the first visible row after it; the filter starts at s0 = max(9, its sample)
+ * with position and velocity as measured there, the attitude propagated alone (no Earth or transport rate)
+ * from sample 9, and a diagonal P0: stdp^2, stdv^2; level N / E (b^2 + b_drift^2 + vrw^2 fs / 10) / 9.80665^2
+ * of accelerometer y / x; yaw yaw_var, or with B2INS_ALIGN_GPS (stdv_N^2 v_E^2 + stdv_E^2 v_N^2) / |v_h|^4;
+ * plus arw^2 dt_gap + (b^2 + b_drift^2) dt_gap^2 of the gyro on the attitude; biases as without alignment.
+ * History rows before the state exists are NaN (attitude before sample 9, position and velocity before s0;
+ * wb, ab are 0), the consistency record takes the GPS epochs after s0, process statistics start at
+ * max(proc_start, s0).  Without a visible GPS row at a sample < n (the host does not check: gps_idx and
+ * gps_vis are device data) there is no fix: position and velocity stay NaN in every history row and in end_err,
+ * the consistency record has no epochs, and proc_stats mean and std are NaN.  cfg->ini and cfg->ini_att_std[2]
+ * are not used; no initial-state draw is made. */
+#define B2INS_ALIGN_OFF 0
+#define B2INS_ALIGN_YAW 1
+#define B2INS_ALIGN_GPS 2
+typedef struct {
+  int32_t mode;         /* B2INS_ALIGN_* */
+  int32_t reserved;
+  double yaw;           /* B2INS_ALIGN_YAW: the heading [rad] */
+  double yaw_var;       /* B2INS_ALIGN_YAW: its variance [rad^2], P0 of the yaw misalignment */
+} b2ins_ekf_align;
+
+/* b2ins_ins_loose_proc_f64 with alignment (align NULL or B2INS_ALIGN_OFF: b2ins_ins_loose_proc_f64 itself).
+ * vib_gyro / vib_accel nullable; proc_start -1 with proc_stats NULL: no process statistics.  n >= 10.
+ * DEVICE pointers. */
+int b2ins_ins_loose_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
+                              const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame,
+                              const double* ref_gyro, const double* ref_accel, const double* ref_nav,
+                              const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
+                              double* end_bias, double* consist, double* proc_stats, double* dump_att,
+                              double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
+
+/* b2ins_ins_loose_fed_f64 with alignment: the fix row's position and velocity are the supplied gps row; no
+ * initial-state draw (align NULL or B2INS_ALIGN_OFF: b2ins_ins_loose_fed_f64 with ini_draw 0).  n >= 10.
+ * DEVICE pointers. */
+int b2ins_ins_loose_fed_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const double* gyro,
+                                  const double* accel, const double* gps, const int64_t* gps_idx,
+                                  const double* gps_vis, const double* ref_nav, double* end_err, double* end_bias,
+                                  double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb,
+                                  double* dump_ab, void* stream);
+
 /* ---- housekeeping ------------------------------------------------------ */
 int b2ins_version(void);
 const char* b2ins_last_error(void);
