@@ -157,6 +157,16 @@ __device__ __forceinline__ void fence_async_smem() {
 
 __host__ __device__ __forceinline__ int64_t min64(int64_t a, int64_t b) { return a < b ? a : b; }
 
+// ---- statistics with NumPy's non-finite rules (np.max, np.mean, np.std) ----
+// max that keeps a NaN in either argument, as np.max does (fmax is IEEE maxNum: it drops the NaN)
+__device__ __forceinline__ double max_nan(double a, double b) { return (a > b || a != a) ? a : b; }
+// a running mean m moved toward the sample or partial mean x by the step d * f (d = x - m); when d is not
+// finite (x or m is +-inf or NaN) the mean is m + x instead: +-inf for infinities of one sign, NaN for a NaN
+// or for both signs, as np.mean of the samples (the finite step would make inf - inf = NaN of a lone inf)
+__device__ __forceinline__ double mean_step(double m, double x, double d, double f) {
+  return isfinite(d) ? fma(d, f, m) : m + x;
+}
+
 // 64-bit shuffle within a lane group of width W
 template <int W>
 __device__ __forceinline__ double shfl_grp(double v, int src) {

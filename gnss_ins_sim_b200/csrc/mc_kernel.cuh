@@ -415,6 +415,14 @@ __device__ __forceinline__ void proc_err_vel(const NavState& st, const double* r
 
 // Adds the NC errors e to the accumulators max|e|, shifted sum, shifted sum of squares and shift K (the first
 // error sample, taken when `first`); column c of each accumulator is at [c * S].
+//
+// The shift keeps the one-pass variance sq / n - (sum / n)^2 from cancelling when the errors sit far from 0:
+// its relative error grows with n and with the distance of the first sample from the others (with the first
+// sample 1e6 standard deviations away, ~5e-9 at n = 2e5; tests/test_gpu_stats_edges.py holds it to 1e-8).
+// The loop runs on every sample, so it is left as it is (fmax included): proc_put recovers NumPy's non-finite
+// results from the sums and the shift (see there).  `first` is not a branch taken once: the compiler turns it
+// into selects on every sample, and a finite-shift select there (K = isfinite(e) ? e : 0) made the K12 PROC
+// launch ~2% slower (1000 runs x 1000 samples, H100 80GB HBM3 at 700 W: 1.150 against 1.124 ms).
 template <int NC, int S>
 __device__ __forceinline__ void proc_fold(const double* e, bool first, double* mx, double* sum, double* sq,
                                           double* k) {
@@ -432,16 +440,25 @@ __device__ __forceinline__ void proc_fold(const double* e, bool first, double* m
 }
 
 // max|e|, mean and std (ddof 0) of NC accumulated columns into o[c], o[9 + c], o[18 + c] (the [3][9] rows of
-// proc_stats); inv = 1 / the sample count
+// proc_stats); inv = 1 / the sample count, NaN for no samples (all three statistics are then NaN).
+// NumPy's non-finite rules, from the sums: with a finite shift K, a NaN sample makes sq NaN, and then max,
+// mean and std are NaN; +-inf samples make sq = +inf, mean = +-inf (NaN for both signs), std =
+// sqrt(inf - inf) = NaN, and max = inf from the fmax of the loop.  A NaN K (a NaN first sample) makes
+// everything NaN.  A +-inf K (an infinite first sample) makes the sums NaN; max is then inf, mean K and std
+// NaN, NumPy's results unless the column also holds a NaN or the other infinity (which one pass cannot see).
 template <int NC, int S>
 __device__ __forceinline__ void proc_put(double* o, double inv, const double* mx, const double* sum,
                                          const double* sq, const double* k) {
 #pragma unroll
   for (int c = 0; c < NC; ++c) {
+    const double kc = k[c * S];
+    const bool kinf = isinf(kc);
     const double m = sum[c * S] * inv;  // mean of (e - K)
-    o[c] = mx[c * S];
-    o[9 + c] = k[c * S] + m;
-    o[18 + c] = sqrt(fmax(sq[c * S] * inv - m * m, 0.0));
+    const double q = sq[c * S] * inv;   // NaN iff a NaN sample, no samples or a +-inf K
+    o[c] = (q != q && !kinf) ? q : mx[c * S];
+    o[9 + c] = kinf ? kc : kc + m;
+    const double v = q - m * m;
+    o[18 + c] = sqrt(v < 0.0 ? 0.0 : v);
   }
 }
 
@@ -689,7 +706,7 @@ mc_kernel(const __grid_constant__ McParams p) {
     put_end<true, true>(p, mr.run, st.yaw, st.pitch, st.roll, st.pos, st.vel);
     if (PROC && p.proc_stats) {
       double* o = p.proc_stats + mr.run * 27;
-      const double inv = pe_cnt > 0 ? 1.0 / static_cast<double>(pe_cnt) : 0.0;
+      const double inv = pe_cnt > 0 ? 1.0 / static_cast<double>(pe_cnt) : __longlong_as_double(0x7ff8000000000000LL);
       proc_put<9, 1>(o, inv, pe_max, pe_sum, pe_sq, pe_k);
     }
   }

@@ -14,6 +14,9 @@
 // mean) and merges the result into its running (count, mean, M2, max) with Chan's update; the 128
 // thread partials are merged by a fixed shuffle tree and the four warp totals in warp order; time
 // segments are merged in segment order by err_stats_fold_kernel.
+//
+// Non-finite errors come out as NumPy's: max_nan keeps a NaN, mean_step carries a +-inf or NaN mean through
+// the merges, and the M2 of any stretch with a non-finite sample is NaN, so std is NaN there as np.std's is.
 #pragma once
 #include "noise_kernel.cuh"
 
@@ -42,16 +45,18 @@ __device__ __forceinline__ void chan_merge(double& na, double& ma, double& m2a, 
     return;
   }
   const double n = na + nb, d = mb - ma, f = nb / n;
-  ma = fma(d, f, ma);
+  ma = mean_step(ma, mb, d, f);
   m2a += m2b + d * d * (na * f);
-  xa = fmax(xa, xb);
+  xa = max_nan(xa, xb);
   na = n;
 }
 
+// the statistics of no samples (n = 0) are NaN
 __device__ __forceinline__ void write_stats(double* ps, int c, int nc, double n, double mean, double m2, double mx) {
-  ps[c] = mx;
-  ps[nc + c] = mean;
-  ps[2 * nc + c] = n > 0.0 ? sqrt(m2 / n) : 0.0;
+  const double none = __longlong_as_double(0x7ff8000000000000LL);
+  ps[c] = n > 0.0 ? mx : none;
+  ps[nc + c] = n > 0.0 ? mean : none;
+  ps[2 * nc + c] = n > 0.0 ? sqrt(m2 / n) : none;
 }
 
 __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const __grid_constant__ ErrStatsParams P) {
@@ -189,7 +194,7 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
 #pragma unroll
         for (int c = 0; c < 6; ++c) {
           bs[c] += e[c];
-          bx[c] = fmax(bx[c], fabs(e[c]));
+          bx[c] = max_nan(bx[c], fabs(e[c]));
         }
       }
     }
@@ -305,9 +310,9 @@ __global__ void __launch_bounds__(kProcThreads) proc_stats_kernel(int64_t m, int
       if (c < nc) {
         const double e = xr[i * nc + c] - ref[i * nc + c];
         const double d = e - am[c];
-        am[c] = fma(d, inv, am[c]);
+        am[c] = mean_step(am[c], e, d, inv);
         a2[c] = fma(d, e - am[c], a2[c]);
-        ax[c] = fmax(ax[c], fabs(e));
+        ax[c] = max_nan(ax[c], fabs(e));
       }
     }
   }

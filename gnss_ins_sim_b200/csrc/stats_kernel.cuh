@@ -2,6 +2,9 @@
 // (ins_data_manager.py:797-808): max|e|, mean, std (ddof 0, two-pass like np.std).
 // Deterministic two-stage reductions (no floating-point atomics): stage 1 writes one
 // partial per block, stage 2 (one block) folds them in a fixed order.
+// Non-finite errors come out as NumPy's: a NaN sample makes max NaN (max_or_nan,
+// max_nan), and the two passes make mean and std NaN or +-inf exactly where
+// np.average and np.std do.  No runs (K3x with every shard empty): NaN statistics.
 #pragma once
 #include "common.cuh"
 
@@ -11,6 +14,13 @@ constexpr int kStatBlocks = 128;   // stage-1 grid
 constexpr int kStatMaxComp = 32;
 
 __host__ __device__ inline int stat_threads(int ncomp) { return ncomp * (1024 / ncomp >= 32 ? 32 : 1024 / ncomp); }
+
+// The per-sample loops keep fmax (one instruction on the loop-carried max) and note a
+// NaN sample in a flag beside it; the thread's partial max is then NaN, and the folds
+// (max_nan) keep it.
+__device__ __forceinline__ double max_or_nan(double mx, bool nan) {
+  return nan ? __longlong_as_double(0x7ff8000000000000LL) : mx;
+}
 
 // MODE 0: sum e and max|e| ; MODE 1: sum (e - mean)^2
 template <int MODE>
@@ -22,25 +32,27 @@ __global__ void err_stage1_kernel(int64_t runs, int ncomp, const double* __restr
   const int64_t total = runs * ncomp;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * threads;
   double acc = 0.0, mx = 0.0;
+  bool nan = false;
   const double mu = (MODE == 1) ? mean[c] : 0.0;
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * threads + threadIdx.x; i < total; i += stride) {
     const double e = err[i];
     if (MODE == 0) {
       acc += e;
       mx = fmax(mx, fabs(e));
+      nan |= e != e;
     } else {
       const double d = e - mu;
       acc += d * d;
     }
   }
   sh[threadIdx.x] = acc;
-  sh[threads + threadIdx.x] = mx;
+  sh[threads + threadIdx.x] = max_or_nan(mx, nan);
   __syncthreads();
   if (threadIdx.x < ncomp) {
     double s = 0.0, m = 0.0;
     for (int k = threadIdx.x; k < threads; k += ncomp) {
       s += sh[k];
-      m = fmax(m, sh[threads + k]);
+      m = max_nan(m, sh[threads + k]);
     }
     ws[(static_cast<int64_t>(blockIdx.x) * 2) * ncomp + c] = s;
     ws[(static_cast<int64_t>(blockIdx.x) * 2 + 1) * ncomp + c] = m;
@@ -56,7 +68,7 @@ __global__ void err_stage2_kernel(int nblocks, int ncomp, const double* __restri
   double s = 0.0, m = 0.0;
   for (int b = 0; b < nblocks; ++b) {
     s += ws[(static_cast<int64_t>(b) * 2) * ncomp + c];
-    m = fmax(m, ws[(static_cast<int64_t>(b) * 2 + 1) * ncomp + c]);
+    m = max_nan(m, ws[(static_cast<int64_t>(b) * 2 + 1) * ncomp + c]);
   }
   out[c] = s;
   if (MODE == 0) out[ncomp + c] = m;
@@ -91,20 +103,22 @@ stats_small_kernel(int64_t runs, int ncomp, const double* __restrict__ err, doub
   const int64_t total = runs * ncomp;
   const bool on = threadIdx.x < threads;
   double acc = 0.0, mx = 0.0;
+  bool nan = false;
   if (on)
     for (int64_t i = threadIdx.x; i < total; i += threads) {
       const double e = err[i];
       acc += e;
       mx = fmax(mx, fabs(e));
+      nan |= e != e;
     }
   sh[threadIdx.x] = acc;
-  sh[kStatSmallThreads + threadIdx.x] = mx;
+  sh[kStatSmallThreads + threadIdx.x] = max_or_nan(mx, nan);
   __syncthreads();
   if (threadIdx.x < ncomp) {
     double s = 0.0, m = 0.0;
     for (int k = threadIdx.x; k < threads; k += ncomp) {
       s += sh[k];
-      m = fmax(m, sh[kStatSmallThreads + k]);
+      m = max_nan(m, sh[kStatSmallThreads + k]);
     }
     stats[c] = m;
     const double mean = s / static_cast<double>(runs);
@@ -159,20 +173,22 @@ stats_exchange_kernel(const __grid_constant__ XchgParams p) {
   const bool on = threadIdx.x < threads;
   // ---- local (max, mean, std): same two passes as stats_small_kernel -------------------------
   double acc = 0.0, mx = 0.0;
+  bool nan = false;
   if (on)
     for (int64_t i = threadIdx.x; i < total; i += threads) {
       const double e = p.err[i];
       acc += e;
       mx = fmax(mx, fabs(e));
+      nan |= e != e;
     }
   sh[threadIdx.x] = acc;
-  sh[kStatSmallThreads + threadIdx.x] = mx;
+  sh[kStatSmallThreads + threadIdx.x] = max_or_nan(mx, nan);
   __syncthreads();
   if (threadIdx.x < nc) {
     double s = 0.0, m = 0.0;
     for (int k = threadIdx.x; k < threads; k += nc) {
       s += sh[k];
-      m = fmax(m, sh[kStatSmallThreads + k]);
+      m = max_nan(m, sh[kStatSmallThreads + k]);
     }
     loc[c] = m;
     loc[nc + c] = p.runs > 0 ? s / static_cast<double>(p.runs) : 0.0;
@@ -235,15 +251,16 @@ stats_exchange_kernel(const __grid_constant__ XchgParams p) {
         n_a = n_b; mx_a = sl[c]; mean_a = mean_b; m2_a = m2_b;
       } else {
         const double n = n_a + n_b, delta = mean_b - mean_a;
-        mean_a += delta * (n_b / n);
+        mean_a = mean_step(mean_a, mean_b, delta, n_b / n);
         m2_a += m2_b + delta * delta * (n_a * n_b / n);
-        mx_a = fmax(mx_a, sl[c]);
+        mx_a = max_nan(mx_a, sl[c]);
         n_a = n;
       }
     }
-    p.out[c] = mx_a;
-    p.out[nc + c] = mean_a;
-    p.out[2 * nc + c] = n_a > 0.0 ? sqrt(m2_a / n_a) : 0.0;
+    const double none = __longlong_as_double(0x7ff8000000000000LL);   // no runs on any rank
+    p.out[c] = n_a > 0.0 ? mx_a : none;
+    p.out[nc + c] = n_a > 0.0 ? mean_a : none;
+    p.out[2 * nc + c] = n_a > 0.0 ? sqrt(m2_a / n_a) : none;
   }
 }
 

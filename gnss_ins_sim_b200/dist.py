@@ -58,7 +58,9 @@ def all_reduce(t, op):
 def merge_stats(blocks):
     """Chan et al. pairwise merge of per-rank (count, max|e|, mean, std) -> (max, mean, std) of
     the union, as robust as np.std's two passes.  blocks: iterable of (n, max[nc], mean[nc],
-    std[nc]) numpy; empty shards (n = 0) are skipped."""
+    std[nc]) numpy; empty shards (n = 0) are skipped.  Non-finite shard statistics merge as
+    NumPy's statistics of the union are: np.maximum keeps a NaN max, a NaN std stays NaN,
+    and a +-inf mean stays +-inf (NaN against the other sign or a NaN)."""
     n_a, mx_a, mean_a, m2_a = 0, None, None, None
     for n_b, mx_b, mean_b, std_b in blocks:
         n_b = int(n_b)
@@ -70,9 +72,13 @@ def merge_stats(blocks):
                 np.array(mean_b, dtype=np.float64), m2_b
             continue
         n = n_a + n_b
-        delta = mean_b - mean_a
-        mean_a = mean_a + delta * (n_b / n)
-        m2_a = m2_a + m2_b + delta * delta * (n_a * n_b / n)
+        with np.errstate(invalid='ignore'):
+            delta = mean_b - mean_a
+            # a +-inf or NaN mean on either side: the sum of the means, +-inf or NaN as
+            # np.mean of the union is
+            mean_a = np.where(np.isfinite(delta), mean_a + delta * (n_b / n),
+                              mean_a + mean_b)
+            m2_a = m2_a + m2_b + delta * delta * (n_a * n_b / n)
         mx_a = np.maximum(mx_a, mx_b)
         n_a = n
     return np.stack([mx_a, mean_a, np.sqrt(m2_a / n_a)]), n_a

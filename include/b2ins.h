@@ -230,7 +230,7 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
  * wb, ab are 0), the consistency record takes the GPS epochs after s0, process statistics start at
  * max(proc_start, s0).  Without a visible GPS row at a sample < n (the host does not check: gps_idx and
  * gps_vis are device data) there is no fix: position and velocity stay NaN in every history row and in end_err,
- * the consistency record has no epochs, and proc_stats mean and std are NaN.  cfg->ini and cfg->ini_att_std[2]
+ * the consistency record has no epochs, and proc_stats (max, mean and std) are NaN.  cfg->ini and cfg->ini_att_std[2]
  * are not used; no initial-state draw is made. */
 #define B2INS_ALIGN_OFF 0
 #define B2INS_ALIGN_YAW 1
@@ -388,7 +388,13 @@ void* b2ins_mc_plan_stream(b2ins_mc_plan* plan);
  * b2ins_error_stats_f64 does both phases for a single shard and writes
  * stats [3][ncomp] = max|e|, mean, std(ddof 0).  ncomp <= 32.  All reductions are
  * deterministic (fixed order, no floating-point atomics).  workspace: device scratch of
- * b2ins_error_stats_workspace_bytes(ncomp) bytes. */
+ * b2ins_error_stats_workspace_bytes(ncomp) bytes.
+ * Non-finite errors, here and in every max|e| / mean / std this library writes (K3x, K9, K3p,
+ * K12 and K7 proc_stats), follow NumPy's np.max(np.abs(e)), np.average and np.std: a NaN in a
+ * column makes its max, mean and std NaN; +-inf makes max inf, mean +-inf (NaN if both signs
+ * occur) and std NaN.  The statistics of no samples are NaN.  K12 and K7 reduce in one pass
+ * shifted by the first counted sample: if that sample is +-inf, its column reports max inf, mean
+ * that infinity and std NaN whatever the later samples hold. */
 int64_t b2ins_error_stats_workspace_bytes(int ncomp);
 int b2ins_error_partial_f64(int64_t runs, int ncomp, const double* err, double* partial,
                             void* workspace, void* stream);
