@@ -1,6 +1,7 @@
 """Allan plugin -- device-backed mirror of demo_algorithms/allan_analysis.py:15-61
 (input ['fs','accel','gyro'], output ['algo_time','ad_accel','ad_gyro']); the variance
-itself is csrc/allan_kernel.cuh (K4, allan.allan_var allan.py:18-59)."""
+itself is csrc/allan_kernel.cuh (K4, allan.allan_var allan.py:18-59) or, overlapping,
+csrc/oallan_kernel.cuh (K4o)."""
 import numpy as np
 import torch
 
@@ -10,9 +11,21 @@ from . import engine
 class Allan(object):
     '''
     Allan deviation of the three accelerometer and three gyroscope channels.
+
+    overlapping=False (the default) is the reference's estimator, allan.allan_var: clusters of m
+    samples start at multiples of m, so the longest cluster sizes average only a few differences.
+    overlapping=True is the overlapping Allan variance of NIST SP 1065 (eq. 10) and IEEE Std 952:
+    every start offset counts,
+        avar(m) = 1 / (2 m^2 M) * sum_{k<M} (S(k+m, m) - S(k, m))^2,  M = n - 2m + 1,
+    with S(k, m) the sum of the m samples from k.  It has many more degrees of freedom at long tau,
+    where bias instability and rate random walk are read.  Both use the same tau grid
+    (m = j*10^k <= n/9), so the two curves can be laid over each other.
     '''
 
-    def __init__(self):
+    def __init__(self, overlapping=False):
+        if not isinstance(overlapping, (bool, np.bool_)):
+            raise TypeError('overlapping must be True or False, got %r' % (overlapping,))
+        self.overlapping = bool(overlapping)
         self.input = ['fs', 'accel', 'gyro']
         self.output = ['algo_time', 'ad_accel', 'ad_gyro']
         self.batch = True
@@ -35,14 +48,15 @@ class Allan(object):
         '''
         a = engine.to_device(accel)
         g = engine.to_device(gyro)
+        var = engine.oallan if self.overlapping else engine.allan
         out = []
         for x in (a, g):
             if channel_major:     # 3R contiguous series: the bulk-copy front end of K4
                 R, _, n = x.shape
-                avar, tau = engine.allan(fs, x, n, R * 3)
+                avar, tau = var(fs, x, n, R * 3)
             else:                 # 3R interleaved series, read in place (no copy)
                 R, n, _ = x.shape
-                avar, tau = engine.allan(fs, x, n, R * 3, inner=3, outer_stride=3 * n, sample_stride=3)
+                avar, tau = var(fs, x, n, R * 3, inner=3, outer_stride=3 * n, sample_stride=3)
             out.append(torch.sqrt(avar).reshape(R, 3, -1).permute(0, 2, 1).contiguous())
         if to_host:
             return tau.cpu().numpy(), out[0].cpu().numpy(), out[1].cpu().numpy()

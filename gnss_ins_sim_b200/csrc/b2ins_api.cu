@@ -10,6 +10,7 @@
 
 #include "../../include/b2ins.h"
 #include "allan_kernel.cuh"
+#include "oallan_kernel.cuh"
 #include "internal.h"
 #include "noise_kernel.cuh"
 #include "pathgen_host.h"
@@ -1321,6 +1322,58 @@ int b2ins_allan_f64_host(double fs, int64_t n, int64_t nseries, const double* x,
                            cudaMemcpyHostToDevice, st.s));
   const int rc = b2ins_allan_f64(fs, n, nseries, dx.d(), inner, outer_stride, sample_stride,
                                  dav.d(), dtau.d(), ws.p, st.s);
+  if (rc != B2INS_OK) return rc;
+  CU_CHECK(cudaMemcpyAsync(avar, dav.p, static_cast<size_t>(nseries) * ntau * sizeof(double),
+                           cudaMemcpyDeviceToHost, st.s));
+  CU_CHECK(cudaMemcpyAsync(tau, dtau.p, static_cast<size_t>(ntau) * sizeof(double),
+                           cudaMemcpyDeviceToHost, st.s));
+  CU_CHECK(cudaStreamSynchronize(st.s));
+  return B2INS_OK;
+}
+
+// ---------------------------------------------------------------- K4o -------
+int64_t b2ins_oallan_workspace_bytes(int64_t n, int64_t nseries) {
+  return oallan_workspace_bytes(n, nseries);
+}
+
+int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                     int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
+                     void* workspace, void* stream) {
+  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
+  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
+  int64_t mult[128];
+  const int ntau = b2ins_allan_num_tau(n, fs, mult, 128);
+  if (ntau == 0 || nseries == 0) return B2INS_OK;
+  ARG_CHECK(ntau <= 128, "too many tau");
+  ARG_CHECK(x && avar && tau && workspace, "null buffer");
+  const int rc = oallan_launch(fs, n, nseries, x, inner, outer_stride, sample_stride, mult, ntau, avar, tau,
+                               workspace, static_cast<cudaStream_t>(stream));
+  if (rc == 4) return fail(B2INS_ERR_ARG, "overlapping Allan: too many series x samples for one call");
+  if (rc != 0) return fail(B2INS_ERR_CUDA, "oallan launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                          int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
+  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
+  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
+  const int ntau = b2ins_allan_num_tau(n, fs, nullptr, 0);
+  if (ntau == 0 || nseries == 0) return B2INS_OK;
+  ARG_CHECK(x && avar && tau, "null buffer");
+  const int64_t outer = (nseries + inner - 1) / inner;
+  const int64_t elems = (outer - 1) * outer_stride + (inner - 1) + (n - 1) * sample_stride + 1;
+  DevBuf dx, dav, dtau, ws;
+  Stream st;
+  CU_CHECK(st.create());
+  CU_CHECK(dx.alloc(static_cast<size_t>(elems) * sizeof(double)));
+  CU_CHECK(dav.alloc(static_cast<size_t>(nseries) * ntau * sizeof(double)));
+  CU_CHECK(dtau.alloc(static_cast<size_t>(ntau) * sizeof(double)));
+  CU_CHECK(ws.alloc(static_cast<size_t>(oallan_workspace_bytes(n, nseries))));
+  CU_CHECK(cudaMemcpyAsync(dx.p, x, static_cast<size_t>(elems) * sizeof(double),
+                           cudaMemcpyHostToDevice, st.s));
+  const int rc = b2ins_oallan_f64(fs, n, nseries, dx.d(), inner, outer_stride, sample_stride,
+                                  dav.d(), dtau.d(), ws.p, st.s);
   if (rc != B2INS_OK) return rc;
   CU_CHECK(cudaMemcpyAsync(avar, dav.p, static_cast<size_t>(nseries) * ntau * sizeof(double),
                            cudaMemcpyDeviceToHost, st.s));

@@ -427,6 +427,31 @@ def allan(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
     return avar, tau
 
 
+def oallan_workspace_bytes(n, nseries):
+    """Device scratch of engine.oallan for `nseries` series of n samples (about 16 B per series-sample)."""
+    return int(_lib.load().b2ins_oallan_workspace_bytes(int(n), int(nseries)))
+
+
+def oallan(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
+    """K4o: overlapping Allan variance on K4's tau grid, same addressing and outputs as allan():
+    avar_o(m) = 1/(2 m^2 M) sum_{k<M} (S(k+m, m) - S(k, m))^2, M = n - 2m + 1.
+    Returns avar [nseries, ntau], tau [ntau] (CUDA)."""
+    _require_cuda()
+    lib = _lib.load()
+    if outer_stride is None:
+        outer_stride = n * sample_stride if inner == 1 else n * inner
+    ntau = len(allan_num_tau(n, fs))
+    avar = torch.zeros((nseries, ntau), dtype=torch.float64, device=x.device)
+    tau = torch.zeros((ntau,), dtype=torch.float64, device=x.device)
+    if ntau == 0 or nseries == 0:
+        return avar, tau
+    ws = torch.empty(oallan_workspace_bytes(n, nseries) // 8 + 1, dtype=torch.float64, device=x.device)
+    _lib.check(lib.b2ins_oallan_f64(float(fs), int(n), int(nseries), _ptr(x), int(inner),
+                                    int(outer_stride), int(sample_stride), _ptr(avar), _ptr(tau),
+                                    _ptr(ws), _stream()))
+    return avar, tau
+
+
 def allan_mc(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0):
     """K1 fused into K4: Allan variance of `runs` Monte-Carlo runs x 6 channels whose series are
     generated inside the tau-binning kernel (never written).  ref_gyro, ref_accel: CUDA f64 [n,3].

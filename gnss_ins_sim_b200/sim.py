@@ -799,13 +799,21 @@ class Sim(object):
         memory; the [R, ntau, 6] deviations of all ranks are gathered (a few hundred KB).  Without a vibration
         model and with series longer than one chunk, K1 is fused into K4's first level (engine.allan_mc) and
         the only device memory is the decade-sum workspace (about 2 B per run-sample), so run blocks are
-        rarely needed; otherwise K1 materialises the series (48 B per run-sample) for K4 (~2 B of workspace)."""
+        rarely needed; otherwise K1 materialises the series (48 B per run-sample) for K4 (~2 B of workspace).
+        Allan(overlapping=True) always materialises: K4o needs its prefix workspace (about 48 B per run-sample
+        for the three series of one sensor) beside the series."""
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
-        fused = (self._vib_acc is None and self._vib_gyro is None and n > 5040
+        overlapping = getattr(algo, 'overlapping', False)
+        fused = (not overlapping and self._vib_acc is None and self._vib_gyro is None and n > 5040
                  and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
         tau = engine.allan_taus(n, self.fs[0])
-        block = self._allan_block(6 * 2, 2) if fused else self._allan_block(64, 3)
+        if fused:
+            block = self._allan_block(6 * 2, 2)
+        elif overlapping:   # K1's 48 B per run-sample, then K4o's workspace for one sensor's 3 series
+            block = self._allan_block(64 + engine.oallan_workspace_bytes(n, 3) / n, 3)
+        else:
+            block = self._allan_block(64, 3)
         parts = []      # [runs, ntau, 6]: accel, gyro
         for r0 in range(lo, hi, block):
             r1 = min(hi, r0 + block)

@@ -431,6 +431,22 @@ int b2ins_allan_f64_host(double fs, int64_t n, int64_t nseries, const double* x,
                          int64_t inner, int64_t outer_stride, int64_t sample_stride,
                          double* avar, double* tau);
 
+/* ---- K4o: overlapping Allan variance ---------------------------------------
+ * avar_o(m) = 1 / (2 m^2 M) sum_{k<M} (S(k+m, m) - S(k, m))^2, S(k, m) = x_k + ... + x_{k+m-1},
+ * M = n - 2m + 1 (NIST SP 1065 eq. 10): every start offset k, on the cluster sizes m of K4's grid
+ * (ntau = b2ins_allan_num_tau(n, fs), the same tau).  Series addressing as b2ins_allan_f64.
+ * A series with a NaN sample gives NaN at every tau; one with +-inf samples gives what the
+ * definitional sum gives in IEEE arithmetic (+inf, or NaN where a window holds inf - inf).
+ * avar [nseries][ntau], tau [ntau]; workspace: b2ins_oallan_workspace_bytes(n, nseries) bytes
+ * (about 16 B per series-sample).  Deterministic: bit-identical whatever the batch. */
+int64_t b2ins_oallan_workspace_bytes(int64_t n, int64_t nseries);
+int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x,
+                     int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                     double* avar, double* tau, void* workspace, void* stream);
+int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x,
+                          int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                          double* avar, double* tau);
+
 /* ---- K5: vibration series from a PSD -------------------------------------------
  * Replaces time_series_from_psd (gnss_ins_sim/psd/time_series_from_psd.py:17-65) as called
  * three times per sensor and run by acc_gen / gyro_gen (pathgen.py:478-485, :541-548).
