@@ -80,6 +80,9 @@ SIGNATURES = {
     'b2ins_imu_noise_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
     'b2ins_gps_noise_f64': (_I, [_L, _L, _P, _P, _P, _I, _U64, _L, _P, _P]),
     'b2ins_mag_noise_f64': (_I, [_L, _L, _P, _P, _P, _P, _U64, _L, _P, _P]),
+    'b2ins_magcal_f64': (_I, [_L, _L, c_int64_p, _P, _P, _P, _P, _U64, _L, _P, _P, _P, _P]),
+    'b2ins_magcal_fed_f64': (_I, [_L, _L, c_int64_p, _P, _L, _L, _P, _P, _P, _P]),
+    'b2ins_magcal_fed_f64_host': (_I, [_L, _L, c_int64_p, _P, _L, _L, _P, _P, _P]),
     'b2ins_imu_err_stats_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _L, _P, _P, _P]),
     'b2ins_proc_stats_f64': (_I, [_L, _L, _I, _P, _P, _L, _P, _P, _P]),
     'b2ins_mc_free_integration_f64': (_I, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

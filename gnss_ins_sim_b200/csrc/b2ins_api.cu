@@ -17,6 +17,7 @@
 #include "psd_kernel.cuh"
 #include "gps_kernel.cuh"
 #include "mag_kernel.cuh"
+#include "magcal_kernel.cuh"
 #include "ekf_kernel.cuh"
 #include "stats_kernel.cuh"
 #include "sensor_stats_kernel.cuh"
@@ -612,6 +613,103 @@ int b2ins_mag_noise_f64(int64_t runs, int64_t n, const double* ref_mag, const do
   if (blocks > cap) blocks = cap;
   mag_noise_kernel<<<static_cast<unsigned>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+// ---------------------------------------------------------------- K10 -------
+static int magcal_check(int64_t runs, int64_t n, const int64_t* seg, MagCalParams* p) {
+  ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
+  ARG_CHECK(seg, "null segments");
+  ARG_CHECK(runs < (int64_t(1) << 31), "runs must be < 2^31");
+  ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
+  for (int i = 0; i < 3; ++i)
+    ARG_CHECK(seg[2 * i] >= 0 && seg[2 * i + 1] <= n && seg[2 * i + 1] - seg[2 * i] >= 3,
+              "segment %d [%lld, %lld) must hold at least 3 rows inside [0, %lld)", i, (long long)seg[2 * i],
+              (long long)seg[2 * i + 1], (long long)n);
+  std::memset(p, 0, sizeof(*p));
+  p->runs = runs;
+  p->n = n;
+  for (int i = 0; i < 6; ++i) p->seg[i] = seg[i];
+  return B2INS_OK;
+}
+
+int b2ins_magcal_f64(int64_t runs, int64_t n, const int64_t* seg, const double* ref_mag, const double* si,
+                     const double* hi, const double* std, uint64_t seed, int64_t run_offset, double* soft_iron,
+                     double* hard_iron, double* err, void* stream) {
+  MagCalParams p;
+  const int rc = magcal_check(runs, n, seg, &p);
+  if (rc != B2INS_OK) return rc;
+  ARG_CHECK(si && hi && std, "null error model");
+  for (int i = 0; i < 3; ++i)
+    ARG_CHECK(std::isfinite(std[i]) && std[i] >= 0.0, "mag std must be finite and >= 0");
+  if (runs == 0) return B2INS_OK;
+  ARG_CHECK(ref_mag && soft_iron && hard_iron, "null buffer");
+  p.run_offset = run_offset;
+  p.ref = ref_mag;
+  for (int i = 0; i < 9; ++i) p.si[i] = si[i];
+  for (int i = 0; i < 3; ++i) {
+    p.hi[i] = hi[i];
+    p.std[i] = std[i];
+  }
+  p.k0 = static_cast<uint32_t>(seed);
+  p.k1 = static_cast<uint32_t>(seed >> 32);
+  p.soft_iron = soft_iron;
+  p.hard_iron = hard_iron;
+  p.err = err;
+  magcal_kernel<false><<<static_cast<unsigned>(runs), kMagCalThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+int b2ins_magcal_fed_f64(int64_t runs, int64_t n, const int64_t* seg, const double* mag, int64_t run_stride,
+                         int64_t sample_stride, double* soft_iron, double* hard_iron, double* mag_cal,
+                         void* stream) {
+  MagCalParams p;
+  const int rc = magcal_check(runs, n, seg, &p);
+  if (rc != B2INS_OK) return rc;
+  ARG_CHECK(run_stride >= 0 && sample_stride >= 3, "run_stride must be >= 0 and sample_stride >= 3");
+  if (runs == 0) return B2INS_OK;
+  ARG_CHECK(mag && soft_iron && hard_iron, "null buffer");
+  p.x = mag;
+  p.run_stride = run_stride;
+  p.sample_stride = sample_stride;
+  p.soft_iron = soft_iron;
+  p.hard_iron = hard_iron;
+  p.mag_cal = mag_cal;
+  magcal_kernel<true><<<static_cast<unsigned>(runs), kMagCalThreads, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+int b2ins_magcal_fed_f64_host(int64_t runs, int64_t n, const int64_t* seg, const double* mag, int64_t run_stride,
+                              int64_t sample_stride, double* soft_iron, double* hard_iron, double* mag_cal) {
+  MagCalParams chk;
+  const int rc = magcal_check(runs, n, seg, &chk);
+  if (rc != B2INS_OK) return rc;
+  ARG_CHECK(run_stride >= 0 && sample_stride >= 3, "run_stride must be >= 0 and sample_stride >= 3");
+  if (runs == 0) return B2INS_OK;
+  ARG_CHECK(mag && soft_iron && hard_iron, "null buffer");
+  const int64_t elems = (runs - 1) * run_stride + (n - 1) * sample_stride + 3;
+  const int64_t L = (seg[1] - seg[0]) + (seg[3] - seg[2]) + (seg[5] - seg[4]);
+  DevBuf dx, dsi, dhi, dcal;
+  Stream st;
+  CU_CHECK(st.create());
+  CU_CHECK(dx.alloc(static_cast<size_t>(elems) * sizeof(double)));
+  CU_CHECK(dsi.alloc(static_cast<size_t>(runs) * 9 * sizeof(double)));
+  CU_CHECK(dhi.alloc(static_cast<size_t>(runs) * 4 * sizeof(double)));
+  if (mag_cal) CU_CHECK(dcal.alloc(static_cast<size_t>(runs) * L * 3 * sizeof(double)));
+  CU_CHECK(cudaMemcpyAsync(dx.p, mag, static_cast<size_t>(elems) * sizeof(double), cudaMemcpyHostToDevice, st.s));
+  const int rc2 = b2ins_magcal_fed_f64(runs, n, seg, dx.d(), run_stride, sample_stride, dsi.d(), dhi.d(),
+                                       mag_cal ? dcal.d() : nullptr, st.s);
+  if (rc2 != B2INS_OK) return rc2;
+  CU_CHECK(cudaMemcpyAsync(soft_iron, dsi.p, static_cast<size_t>(runs) * 9 * sizeof(double), cudaMemcpyDeviceToHost,
+                           st.s));
+  CU_CHECK(cudaMemcpyAsync(hard_iron, dhi.p, static_cast<size_t>(runs) * 4 * sizeof(double), cudaMemcpyDeviceToHost,
+                           st.s));
+  if (mag_cal)
+    CU_CHECK(cudaMemcpyAsync(mag_cal, dcal.p, static_cast<size_t>(runs) * L * 3 * sizeof(double),
+                             cudaMemcpyDeviceToHost, st.s));
+  CU_CHECK(cudaStreamSynchronize(st.s));
   return B2INS_OK;
 }
 

@@ -153,6 +153,66 @@ def mag_noise(runs, ref_mag, mag_err, seed, run_offset=0):
     return out
 
 
+def _segments(segments):
+    """((x0, xf), (y0, yf), (z0, zf)) -> the int64[6] the C ABI takes (it checks the ranges)."""
+    seg = np.ascontiguousarray(np.asarray(segments, dtype=np.int64).reshape(6))
+    return seg, seg.ctypes.data_as(_lib.c_int64_p)
+
+
+class MagCalResult:
+    """Device-side results of one magnetometer-calibration launch (K10)."""
+
+    def __init__(self):
+        self.soft_iron = None    # [R,3,3] S: calibrated = S m - hard_iron[0:3]
+        self.hard_iron = None    # [R,4] hard iron [uT], field radius [uT]
+        self.err = None          # [R,13] calibration error against the generating model (mag_calibrate_mc)
+        self.mag_cal = None      # [R,L,3] the segments after the staged corrections (mag_calibrate, want_cal)
+
+
+def mag_calibrate(segments, mag, want_cal=False):
+    """K10 on supplied samples (b2ins_magcal_fed_f64): the soft- and hard-iron calibration of every run of mag
+    (CUDA f64 [R,n,3]) from its rotations about x, y and z, segments ((x0, xf), (y0, yf), (z0, zf)) (half-open
+    sample ranges, each >= 3 rows inside [0, n)).  want_cal: also mag_cal [R,L,3], the segments stacked after
+    the staged corrections.  Asynchronous on the current stream."""
+    _require_cuda()
+    lib = _lib.load()
+    R, n, three = mag.shape
+    if three != 3:
+        raise ValueError('mag must be [R, n, 3], got %s' % (tuple(mag.shape),))
+    seg, segp = _segments(segments)
+    res = MagCalResult()
+    res.soft_iron = torch.empty((R, 3, 3), dtype=torch.float64, device=mag.device)
+    res.hard_iron = torch.empty((R, 4), dtype=torch.float64, device=mag.device)
+    if want_cal:
+        L = max(0, int((seg[1] - seg[0]) + (seg[3] - seg[2]) + (seg[5] - seg[4])))
+        res.mag_cal = torch.empty((R, L, 3), dtype=torch.float64, device=mag.device)
+    _lib.check(lib.b2ins_magcal_fed_f64(R, n, segp, _ptr(mag), 3 * n, 3, _ptr(res.soft_iron), _ptr(res.hard_iron),
+                                        _ptr(res.mag_cal), _stream()))
+    return res
+
+
+def mag_calibrate_mc(runs, segments, ref_mag, mag_err, seed, run_offset=0, want_err=True):
+    """K8 fused into K10 (b2ins_magcal_f64): the calibration of `runs` runs of the magnetometer mag_noise makes
+    (same ref_mag [n,3] CUDA f64, mag_err, seed, run_offset), whose samples are regenerated inside the kernel
+    and never written.  want_err: res.err [R,13], the error against mag_err (include/b2ins.h)."""
+    _require_cuda()
+    lib = _lib.load()
+    n = ref_mag.shape[0]
+    seg, segp = _segments(segments)
+    dev = ref_mag.device
+    res = MagCalResult()
+    res.soft_iron = torch.empty((runs, 3, 3), dtype=torch.float64, device=dev)
+    res.hard_iron = torch.empty((runs, 4), dtype=torch.float64, device=dev)
+    res.err = torch.empty((runs, 13), dtype=torch.float64, device=dev) if want_err else None
+    si = np.ascontiguousarray(np.asarray(mag_err['si'], dtype=np.float64).reshape(3, 3))
+    hi = np.ascontiguousarray(np.broadcast_to(np.asarray(mag_err['hi'], dtype=np.float64).reshape(-1), (3,)))
+    std = np.ascontiguousarray(np.broadcast_to(np.asarray(mag_err['std'], dtype=np.float64).reshape(-1), (3,)))
+    _lib.check(lib.b2ins_magcal_f64(int(runs), n, segp, _ptr(ref_mag), _lib.host_ptr(si), _lib.host_ptr(hi),
+                                    _lib.host_ptr(std), int(seed) & 0xFFFFFFFFFFFFFFFF, int(run_offset),
+                                    _ptr(res.soft_iron), _ptr(res.hard_iron), _ptr(res.err), _stream()))
+    return res
+
+
 def imu_err_stats(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0,
                   vib_gyro=None, vib_accel=None, stats_start=-1):
     """K9: error statistics of the measurements imu_noise would make, reduced inside the generator.

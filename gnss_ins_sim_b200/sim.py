@@ -18,6 +18,7 @@ Dispatch on `algorithm`:
     lazily: counter-based Philox makes any run reproducible in isolation, so
     get_data(['pos'])[0]['algo0_7'] re-runs just run 7 with history output on.
   * gnss_ins_sim_b200 Allan            -> K1 (noise) + K4 (Allan variance) per run block.
+  * gnss_ins_sim_b200 MagCal           -> K8's samples regenerated inside K10 (magnetometer calibration).
   * any other reference-style plugin   -> K1 generates gyro/accel (K8 the magnetometer of a
     9-axis IMU) on the device, the plugin's own .run() is called per run on the host
     (compatibility path).
@@ -38,6 +39,7 @@ from .free_integration import FreeIntegration
 from .free_integration_odo import FreeIntegration as FreeIntegrationOdo
 from .allan_analysis import Allan
 from .ins_loose import InsLoose, gps_sample_index
+from .mag_calibrate import MagCal, check_segments
 
 D2R = math.pi / 180
 R2D = 180 / math.pi
@@ -338,6 +340,7 @@ _SENSOR_UNITS = {  # sensor data with a ref_ counterpart -> (units, output units
     'gps': (['rad', 'rad', 'm', 'm/s', 'm/s', 'm/s'], ['deg', 'deg', 'm', 'm/s', 'm/s', 'm/s']),
 }
 _REF_OF = {'att_euler': 'ref_att', 'pos': 'ref_pos', 'vel': 'ref_vel'}   # trajectory key of an output's truth
+_MAGCAL_UNITS = {'soft_iron': ['-'] * 9, 'hard_iron': ['uT'] * 4}   # MagCal calibration errors
 
 
 def _first_at(t, start_s):
@@ -465,6 +468,7 @@ class Sim(object):
         self._all_hist = None    # (algo index, first run, arrays) of the last histories() with stride 1
         self.err_stats = {}
         self._mc = {}
+        self._magcal = {}        # algo index -> [3, 13] statistics of the calibration errors (MagCal)
         self._vib_acc = parse_env(self.env['acc'], self.fs[0]) if self.env and 'acc' in self.env else None
         self._vib_gyro = parse_env(self.env['gyro'], self.fs[0]) if self.env and 'gyro' in self.env else None
         self._psd_cache = {}
@@ -493,6 +497,8 @@ class Sim(object):
                     self._run_allan(i, a)
                 elif isinstance(a, InsLoose):
                     self._run_ins_loose(i, a)
+                elif isinstance(a, MagCal):
+                    self._run_magcal(i, a)
                 else:
                     self._run_plugin(i, a, self._generated_inputs)
         self.sim_complete = True
@@ -529,7 +535,7 @@ class Sim(object):
         """Algorithms on the logged sets 0 .. sim_count-1 (InsAlgoMgr.run_algo over the keys,
         ins_algo_manager.py:73-95): one batched launch per algorithm, outputs keyed
         '<algo>_<key>'; end-point error statistics if the directory has the reference files."""
-        self._proc, self.err_stats, self._mc, self._sens = {}, {}, {}, {}
+        self._proc, self.err_stats, self._mc, self._sens, self._magcal = {}, {}, {}, {}, {}
         self._shard = (0, self.sim_count)
         d = self._logged
         for i, a in enumerate(self.algo or []):
@@ -557,6 +563,10 @@ class Sim(object):
                                                        self._logged_sets('gyro')))
             elif isinstance(a, InsLoose):
                 self._run_logged_ins_loose(i, a)
+            elif isinstance(a, MagCal):
+                si, hi, cal = a.run_batch(self._logged_sets('mag'))
+                self._publish_magcal(name, si, hi)
+                self.data['mag_cal'] = _keyed(name, cal)
             else:
                 self._run_plugin(i, a, self._logged_inputs)
         self.sim_complete = True
@@ -833,6 +843,35 @@ class Sim(object):
                                     self.sim_count).reshape(self.sim_count, len(tau), 6)
         self._publish_allan(self.algo_name(i), tau, both[:, :, 0:3], both[:, :, 3:6])
 
+    # ---- magnetometer calibration (K10) ---------------------------------------------------------
+    def _publish_magcal(self, name, soft_iron, hard_iron):
+        """soft_iron [R, 3, 3] and hard_iron [R, 4] under run keys, in the reference's shapes (3, 3) and (1, 4)."""
+        self.data['soft_iron'] = _keyed(name, np.asarray(soft_iron).reshape(-1, 3, 3))
+        self.data['hard_iron'] = _keyed(name, np.asarray(hard_iron).reshape(-1, 1, 4))
+
+    def _run_magcal(self, i, algo):
+        """All runs of this rank in one K10 launch that regenerates K8's samples (nothing is materialised):
+        soft_iron and hard_iron of every run (gathered over ranks) and the ensemble statistics of the calibration
+        errors; mag_cal is materialised per history block on request (K8, then the fed K10)."""
+        if not getattr(self.imu, 'magnetometer', False):
+            raise ValueError('MagCal calibrates the magnetometer: it needs IMU(axis=9)')
+        check_segments(algo.segments, self._traj['ref_gyro'].shape[0])
+        lo, hi = self._shard
+        si, hard, stats = np.zeros((0, 9)), np.zeros((0, 4)), np.zeros((3, 13))
+        if hi > lo:
+            res = engine.mag_calibrate_mc(hi - lo, algo.segments, self._dev['ref_mag'], self.imu.mag_err, self.seed,
+                                          run_offset=self.run_base + lo)
+            stats = engine.error_stats(res.err).cpu().numpy()
+            si, hard = res.soft_iron.reshape(-1, 9).cpu().numpy(), res.hard_iron.cpu().numpy()
+        self._magcal[i] = dist.combine_local_stats(stats, hi - lo)
+        if dist.world() > 1:
+            both = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(np.concatenate([si, hard], axis=1))),
+                                    self.sim_count)
+            si, hard = both[:, 0:9], both[:, 9:13]
+        name = self.algo_name(i)
+        self._publish_magcal(name, si, hard)
+        self.data['mag_cal'] = LazyRuns(self, (i, 'mag_cal'), self.sim_count, prefix=name)
+
     # ---- loosely-coupled GNSS/INS filter (K7) -------------------------------------------------
     def _ekf_inputs(self):
         """Device copies of what K7 reads beside the IMU truth: GPS truth rows, their IMU sample
@@ -944,6 +983,11 @@ class Sim(object):
             if not ai:
                 raise KeyError('odo histories are produced with the free_integration_odo plugin')
             name = (ai[0], 'pos')
+        if isinstance(name, tuple) and isinstance(self.algo[name[0]], MagCal):
+            mag = engine.mag_noise(runs, self._dev['ref_mag'], self.imu.mag_err, self.seed,
+                                   run_offset=self.run_base + r0)
+            res = engine.mag_calibrate(self.algo[name[0]].segments, mag, want_cal=True)
+            return {name: res.mag_cal.cpu().numpy()}
         if isinstance(name, tuple) and isinstance(self.algo[name[0]], InsLoose):
             res = self._ekf_launch(self.algo[name[0]], r0, runs, dump_runs=runs)
             return {(name[0], k): v.cpu().numpy() for k, v in (('att_euler', res.att), ('pos', res.pos),
@@ -1060,6 +1104,8 @@ class Sim(object):
             raise ValueError('odo has no error statistics: the odometer history is one column per run, and the '
                              "reference's own end-point statistics index it as a 2-D array "
                              '(ins_data_manager.py:737), so there is no defined result')
+        if data_name in _MAGCAL_UNITS:
+            return self._magcal_stats(data_name, err_stats_start, algo_index)
         if data_name in _SENSOR_UNITS:
             units, out_units = _SENSOR_UNITS[data_name]
             if data_name == 'gps' and self.ref_frame == 1:      # ins_data_manager.py:221-230
@@ -1098,6 +1144,20 @@ class Sim(object):
         else:
             st = self._process_stats(algo_index, err_stats_start, c0, frame)
         return self._with_units(st, units, out_units, use_output_units)
+
+    def _magcal_stats(self, data_name, start_s, algo_index):
+        """get_error_stats('soft_iron' | 'hard_iron', -1) of a MagCal on generated data: the statistics over runs
+        of E = S si / k - I (9 values, row-major) or of (hard_iron[0:3] / k - hi, hard_iron[3] / k - |b|) [uT],
+        with k = trace(S si) / 3 (b: the true field at the first sample)."""
+        if algo_index not in getattr(self, '_magcal', {}):
+            raise ValueError('%s error statistics need a MagCal run on generated data (algo_index %d is not one)'
+                             % (data_name, algo_index))
+        if start_s != -1:
+            raise ValueError('%s error statistics are over runs only (err_stats_start=-1)' % data_name)
+        st = self._magcal[algo_index]
+        cols = slice(0, 9) if data_name == 'soft_iron' else slice(9, 13)
+        return {'max': st[0, cols].copy(), 'avg': st[1, cols].copy(), 'std': st[2, cols].copy(),
+                'units': str(_MAGCAL_UNITS[data_name])}
 
     @staticmethod
     def _with_units(st, units, out_units, use_output_units):
@@ -1312,6 +1372,16 @@ class Sim(object):
                     s += '\t--Max error: %s\n' % str(st['max'])
                     s += '\t--Avg error: %s\n' % str(st['avg'])
                     s += '\t--Std of error: %s\n' % str(st['std'])
+        for i in sorted(getattr(self, '_magcal', {})):
+            s += '\n------------------------------------------------------------\n'
+            s += 'Calibration errors of %s over runs (S si / k - I; hard iron / k - hi, radius / k - |b|).' \
+                % self.algo_name(i)
+            for dn in ('soft_iron', 'hard_iron'):
+                st = self.get_error_stats(dn, algo_index=i)
+                s += '\n-----------statistics for %s (in units of %s)\n' % (dn, st['units'])
+                s += '\t--Max error: %s\n' % str(st['max'])
+                s += '\t--Avg error: %s\n' % str(st['avg'])
+                s += '\t--Std of error: %s\n' % str(st['std'])
         self.sum += s
         if dist.rank() == 0:
             print(self.sum)

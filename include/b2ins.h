@@ -485,6 +485,30 @@ int b2ins_mag_noise_f64(int64_t runs, int64_t n, const double* ref_mag, const do
                         const double* hi, const double* std, uint64_t seed, int64_t run_offset,
                         double* mag, void* stream);
 
+/* ---- K10: soft- and hard-iron magnetometer calibration -------------------------------
+ * MagCalibrate (demo_algorithms/mag_calibrate_src/src/MagCalibration.c:34-306) for `runs` runs at once,
+ * one CTA per run (DESIGN.md section 3.11).  seg: host [6] = (x0, xf, y0, yf, z0, zf), half-open sample
+ * ranges of the rotations about the sensor's x, y and z axes, each >= 3 rows inside [0, n).
+ * Outputs (device): soft_iron [runs][9] (row-major S) and hard_iron [runs][4] (hard iron, field radius);
+ * calibrated samples are S m - hard_iron[0:3].  A singular 3x3 or 4x4 system gives NaN in all 13 values of
+ * the run; a zero range gives what the division gives; a NaN sample gives NaN.  Deterministic: a run's
+ * result is bit-identical whatever runs, run_offset or the other runs.
+ * b2ins_magcal_f64: the samples of K8 (b2ins_mag_noise_f64 with the same ref_mag, si, hi, std, seed and
+ *   run_offset), regenerated, never stored.  err [runs][13] (nullable): the calibration error against that
+ *   model, with k = trace(S si) / 3: S si / k - I (9), hard_iron[0:3] / k - hi (3), hard_iron[3] / k - |ref_mag[0]|.
+ * b2ins_magcal_fed_f64: sample k of run r at mag[r * run_stride + k * sample_stride + c] (device;
+ *   sample_stride >= 3).  mag_cal [runs][L][3] (nullable), L = the three lengths summed: the segments stacked,
+ *   after the reference's staged corrections O m, diag(s) ., - hard_iron[0:3].
+ * b2ins_magcal_fed_f64_host: the fed form on host buffers (synchronous). */
+int b2ins_magcal_f64(int64_t runs, int64_t n, const int64_t* seg, const double* ref_mag, const double* si,
+                     const double* hi, const double* std, uint64_t seed, int64_t run_offset, double* soft_iron,
+                     double* hard_iron, double* err, void* stream);
+int b2ins_magcal_fed_f64(int64_t runs, int64_t n, const int64_t* seg, const double* mag, int64_t run_stride,
+                         int64_t sample_stride, double* soft_iron, double* hard_iron, double* mag_cal,
+                         void* stream);
+int b2ins_magcal_fed_f64_host(int64_t runs, int64_t n, const int64_t* seg, const double* mag, int64_t run_stride,
+                              int64_t sample_stride, double* soft_iron, double* hard_iron, double* mag_cal);
+
 /* ---- K9: IMU error statistics, reduced inside the noise generator ---------------------
  * InsDataMgr.get_error_stats('gyro' | 'accel') (ins_data_manager.py:385-452, :524-541, :717-808) for
  * `runs` runs without materialising them: the measurements of b2ins_imu_noise_f64 (same arguments, same
