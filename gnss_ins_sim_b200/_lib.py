@@ -121,6 +121,7 @@ SIGNATURES = {
     'b2ins_diag_dfma_rate': (_I, [c_double_p]),
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),
+    'b2ins_diag_psd_plan': (_I, [_L, ctypes.POINTER(ctypes.c_int)]),
 }
 
 _lib = None
@@ -165,6 +166,19 @@ def mc_shape(lanes, ref_frame=1):
     out = (ctypes.c_int * 3)()
     check(load().b2ins_diag_mc_shape(int(lanes), int(ref_frame), out))
     return '%d,%d,%d' % (out[0], out[1], out[2]) if out[0] else '0'
+
+
+PSD_PLANS = ('direct', 'radix2', 'bluestein')
+
+
+def psd_plan(n):
+    """(plan, P) of K5 for a series of n samples: 'direct' (P = 0), 'radix2' or 'bluestein' (P = the
+    transform length)."""
+    P = ctypes.c_int(0)
+    rc = load().b2ins_diag_psd_plan(int(n), ctypes.byref(P))
+    if rc < 0:
+        raise ValueError('b2ins: ' + load().b2ins_last_error().decode('utf-8', 'replace'))
+    return PSD_PLANS[rc], P.value
 
 
 def check(rc):

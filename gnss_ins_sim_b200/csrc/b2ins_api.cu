@@ -1482,7 +1482,25 @@ int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x
 }
 
 // ---------------------------------------------------------------- K5 --------
+// B2INS_PSD_DIRECT (tools: A/B the two paths) forces the direct synthesis; read once per process, so a
+// launch and b2ins_diag_psd_plan always agree
+static bool psd_direct_forced() {
+  static const bool forced = std::getenv("B2INS_PSD_DIRECT") != nullptr;
+  return forced;
+}
+
 int b2ins_psd_series_len(int64_t n) { return n > 0 ? psd_series_len(n) : 0; }
+
+int b2ins_diag_psd_plan(int64_t n, int* P) {
+  if (n <= 0 || !P) {
+    fail(B2INS_ERR_ARG, "bad n or null output");
+    return -1;
+  }
+  int bluestein = 0;
+  const int len = psd_direct_forced() ? 0 : psd_fft_plan(psd_series_len(n), &bluestein);
+  *P = len;
+  return len == 0 ? 0 : (bluestein ? 2 : 1);
+}
 
 int64_t b2ins_psd_workspace_bytes(int64_t n, int64_t runs) {
   if (n <= 0 || runs <= 0) return 16;
@@ -1519,8 +1537,7 @@ int b2ins_psd_series_f64(double fs, int64_t n, int64_t runs, int sensor, int tab
   dim3 g1((p.L + kPsdThreads - 1) / kPsdThreads, static_cast<unsigned>(runs * 3));
   psd_phase_kernel<<<g1, kPsdThreads, 0, s>>>(p);
   int bluestein = 0;
-  static const bool no_fft = std::getenv("B2INS_PSD_DIRECT") != nullptr;     // tools: A/B the two paths
-  const int P = no_fft ? 0 : psd_fft_plan(p.N, &bluestein);
+  const int P = psd_direct_forced() ? 0 : psd_fft_plan(p.N, &bluestein);
   if (P == 0) {      // lengths without an FFT path: the O(N L) cosine synthesis
     dim3 g2((p.N + kPsdThreads - 1) / kPsdThreads, static_cast<unsigned>(runs * 3));
     psd_synth_kernel<<<g2, kPsdThreads, 0, s>>>(p);

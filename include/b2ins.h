@@ -581,6 +581,13 @@ int b2ins_diag_auto_lanes(int64_t runs, int fused, int sm_count);
  * Honours the tools' B2INS_MC_SHAPE override, i.e. reports what a launch would use.  Pure host logic. */
 int b2ins_diag_mc_shape(int lanes_per_run, int ref_frame, int* shape3);
 
+/* The transform b2ins_psd_series_f64 uses for a series of n samples (N = b2ins_psd_series_len(n),
+ * M = N / 2): returns 0 for the direct cosine synthesis, 1 for the radix-2 transform of length M
+ * (M a power of two) and 2 for Bluestein, and writes the transform length to *P (M, the Bluestein
+ * length, or 0 for the direct synthesis).  Honours the tools' B2INS_PSD_DIRECT override (read once
+ * per process, as the launch reads it).  Returns -1 if n <= 0 or P is NULL.  Pure host logic. */
+int b2ins_diag_psd_plan(int64_t n, int* P);
+
 #ifdef __cplusplus
 }
 #endif

@@ -548,22 +548,18 @@ def allan_var(x, fs):
 # --------------------------------------------------------------------------
 # PSD vibration, psd/time_series_from_psd.py:17-65
 # --------------------------------------------------------------------------
-def time_series_from_psd(sxx, freq, fs, n, phase_normals):
-    """time_series_from_psd with the L random-phase normals supplied (first-call
-    behaviour: the caller's sxx is NOT halved in place, see SURVEY 7 'quirks')."""
+def psd_bins(sxx, freq, fs, n, phase_normals):
+    """The period N and the L = N/2 + 1 complex bins xk = A + jB that time_series_from_psd
+    transforms (time_series_from_psd.py:36-54); None if the table exceeds fs/2."""
     sxx = np.array(sxx, dtype=np.float64)
     freq = np.asarray(freq, dtype=np.float64)
-    x = np.zeros((n,))
     if fs < 2.0 * freq[-1] or fs < 0.0:
-        return False, x
-    repeat = False
+        return None
     N = n
     if n % 2 != 0:
         N = n + 1
-        repeat = True
     if N > 16384:
         N = 16384
-        repeat = True
     L = freq.shape[0]
     if L != N // 2 + 1:
         L = N // 2 + 1
@@ -571,11 +567,22 @@ def time_series_from_psd(sxx, freq, fs, n, phase_normals):
     sxx[1:L - 1] = 0.5 * sxx[1:L - 1]
     ax = np.sqrt(sxx * N * fs)
     phi = PI * np.asarray(phase_normals, dtype=np.float64)[:L]
-    xk = ax * np.exp(1j * phi)
+    return N, ax * np.exp(1j * phi)
+
+
+def tile_period(xt, n):
+    """A series of period N = len(xt) for n samples, as time_series_from_psd.py:58-63 repeats it."""
+    N = xt.shape[0]
+    return np.hstack([np.tile(xt, (n // N,)), xt[0:n % N]]) if n != N else xt
+
+
+def time_series_from_psd(sxx, freq, fs, n, phase_normals):
+    """time_series_from_psd with the L random-phase normals supplied (first-call
+    behaviour: the caller's sxx is NOT halved in place, see SURVEY 7 'quirks')."""
+    bins = psd_bins(sxx, freq, fs, n, phase_normals)
+    if bins is None:
+        return False, np.zeros((n,))
+    N, xk = bins
     xk = np.hstack([xk, xk[-2:0:-1].conj()])
     xt = np.fft.ifft(xk).real
-    if repeat:
-        x = np.hstack([np.tile(xt, (n // N,)), xt[0:n % N]])
-    else:
-        x = xt
-    return True, x
+    return True, tile_period(xt, n)
