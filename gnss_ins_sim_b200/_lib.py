@@ -122,7 +122,14 @@ SIGNATURES = {
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),
     'b2ins_diag_psd_plan': (_I, [_L, ctypes.POINTER(ctypes.c_int)]),
+    'b2ins_diag_fastmath_f64': (_I, [_I, _L, _P, _P, _P, _P]),
+    'b2ins_diag_philox': (_I, [_L, _P, _P]),
+    'b2ins_diag_normal_from_words': (_I, [_L, _P, _P]),
 }
+
+# function codes of b2ins_diag_fastmath_f64 (include/b2ins.h B2INS_FM_*)
+FASTMATH_FNS = ('rcp_nr', 'div_nr', 'sqrt_nr', 'rsqrt_nr', 'sincos_bounded', 'sincos_angle', 'sincospi_2u',
+                'log_unit')
 
 _lib = None
 _load_error = None       # a failed build is not retried in the same process (every caller gets the same error)

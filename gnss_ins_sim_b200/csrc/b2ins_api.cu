@@ -1654,6 +1654,105 @@ int b2ins_diag_dfma_rate(double* dfma_per_s) {
   return B2INS_OK;
 }
 
+}  // extern "C"
+
+// The production FP64 primitives and the noise generator, elementwise, so that the suite measures them
+// as the device runs them (tests/test_gpu_fastmath.py).  One instantiation per function: each body is
+// the inlined production function and nothing else.
+template <int FN>
+__global__ void fastmath_diag_kernel(int64_t n, const double* __restrict__ a, const double* __restrict__ b,
+                                     double* __restrict__ out0, double* __restrict__ out1) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const double x = a[i];
+    double s = 0.0, c = 0.0;
+    if (FN == B2INS_FM_RCP) s = rcp_nr(x);
+    if (FN == B2INS_FM_DIV) s = div_nr(x, b[i]);
+    if (FN == B2INS_FM_SQRT) s = sqrt_nr(x);
+    if (FN == B2INS_FM_RSQRT) s = rsqrt_nr(x);
+    if (FN == B2INS_FM_SINCOS) sincos_bounded(x, &s, &c);
+    if (FN == B2INS_FM_SINCOS_ANGLE) sincos_angle(x, &s, &c);
+    if (FN == B2INS_FM_SINCOSPI) sincospi_2u(x, &s, &c);
+    if (FN == B2INS_FM_LOG) s = log_unit(x);
+    out0[i] = s;
+    if (out1) out1[i] = c;
+  }
+}
+
+__global__ void philox_diag_kernel(int64_t n, const uint32_t* __restrict__ ck, uint32_t* __restrict__ words) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const uint32_t* c = ck + 6 * i;
+    const PhiloxOut x = philox4x32_10(c[0], c[1], c[2], c[3], c[4], c[5]);
+    words[4 * i] = x.x0;
+    words[4 * i + 1] = x.x1;
+    words[4 * i + 2] = x.x2;
+    words[4 * i + 3] = x.x3;
+  }
+}
+
+__global__ void normal_diag_kernel(int64_t n, const uint32_t* __restrict__ words, double* __restrict__ z) {
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const uint32_t* w = words + 4 * i;
+    const Normal2 p = normal_from_words(PhiloxOut{w[0], w[1], w[2], w[3]});
+    z[2 * i] = p.z0;
+    z[2 * i + 1] = p.z1;
+  }
+}
+
+static unsigned diag_grid(int64_t n) {
+  const int64_t cap = 32 * static_cast<int64_t>(sm_count());
+  const int64_t g = (n + 255) / 256;
+  return static_cast<unsigned>(g < cap ? g : cap);
+}
+
+extern "C" {
+
+int b2ins_diag_fastmath_f64(int fn, int64_t n, const double* a, const double* b, double* out0, double* out1) {
+  ARG_CHECK(fn >= B2INS_FM_RCP && fn <= B2INS_FM_LOG, "unknown function %d", fn);
+  ARG_CHECK(n >= 0, "bad n");
+  if (n == 0) return B2INS_OK;
+  const bool pair = fn == B2INS_FM_SINCOS || fn == B2INS_FM_SINCOS_ANGLE || fn == B2INS_FM_SINCOSPI;
+  ARG_CHECK(a && out0 && (fn != B2INS_FM_DIV || b) && (!pair || out1), "null buffer");
+  const unsigned g = diag_grid(n);
+  switch (fn) {
+    case B2INS_FM_RCP: fastmath_diag_kernel<B2INS_FM_RCP><<<g, 256>>>(n, a, b, out0, nullptr); break;
+    case B2INS_FM_DIV: fastmath_diag_kernel<B2INS_FM_DIV><<<g, 256>>>(n, a, b, out0, nullptr); break;
+    case B2INS_FM_SQRT: fastmath_diag_kernel<B2INS_FM_SQRT><<<g, 256>>>(n, a, b, out0, nullptr); break;
+    case B2INS_FM_RSQRT: fastmath_diag_kernel<B2INS_FM_RSQRT><<<g, 256>>>(n, a, b, out0, nullptr); break;
+    case B2INS_FM_SINCOS: fastmath_diag_kernel<B2INS_FM_SINCOS><<<g, 256>>>(n, a, b, out0, out1); break;
+    case B2INS_FM_SINCOS_ANGLE:
+      fastmath_diag_kernel<B2INS_FM_SINCOS_ANGLE><<<g, 256>>>(n, a, b, out0, out1);
+      break;
+    case B2INS_FM_SINCOSPI: fastmath_diag_kernel<B2INS_FM_SINCOSPI><<<g, 256>>>(n, a, b, out0, out1); break;
+    default: fastmath_diag_kernel<B2INS_FM_LOG><<<g, 256>>>(n, a, b, out0, nullptr); break;
+  }
+  CU_CHECK(cudaGetLastError());
+  CU_CHECK(cudaDeviceSynchronize());
+  return B2INS_OK;
+}
+
+int b2ins_diag_philox(int64_t n, const uint32_t* ctr_key, uint32_t* words) {
+  ARG_CHECK(n >= 0, "bad n");
+  if (n == 0) return B2INS_OK;
+  ARG_CHECK(ctr_key && words, "null buffer");
+  philox_diag_kernel<<<diag_grid(n), 256>>>(n, ctr_key, words);
+  CU_CHECK(cudaGetLastError());
+  CU_CHECK(cudaDeviceSynchronize());
+  return B2INS_OK;
+}
+
+int b2ins_diag_normal_from_words(int64_t n, const uint32_t* words, double* z) {
+  ARG_CHECK(n >= 0, "bad n");
+  if (n == 0) return B2INS_OK;
+  ARG_CHECK(words && z, "null buffer");
+  normal_diag_kernel<<<diag_grid(n), 256>>>(n, words, z);
+  CU_CHECK(cudaGetLastError());
+  CU_CHECK(cudaDeviceSynchronize());
+  return B2INS_OK;
+}
+
 #ifdef B2INS_PHASE_CLOCKS
 // tools only: the kPhaseClocks cumulative warp-cycle counters (slots: mc_kernel.cuh, mc_spec_kernel.cuh,
 // mc_av_kernel.cuh)

@@ -78,15 +78,19 @@ struct Normal2 {
   double z0, z1;
 };
 
-// Box-Muller in float64: r = sqrt(-2 ln u1), (z0, z1) = r (cos, sin)(2 pi u2).
-__device__ __forceinline__ Normal2 normal_pair(uint32_t t, uint32_t draw, uint32_t run_lo,
-                                               uint32_t run_hi, uint32_t k0, uint32_t k1) {
-  const PhiloxOut x = philox4x32_10(t, draw, run_lo, run_hi, k0, k1);
+// Box-Muller in float64 from one Philox output: r = sqrt(-2 ln u1), (z0, z1) = r (cos, sin)(2 pi u2),
+// u1 = 1 - m1 2^-52 with m1 = (x1:x0) >> 12 and u2 = m2 2^-52 with m2 = (x3:x2) >> 12.
+__device__ __forceinline__ Normal2 normal_from_words(const PhiloxOut& x) {
   const double u1 = 2.0 - one_plus_u01_from_bits(x.x0, x.x1);   // 1 - u in (0, 1], exact
   const double r = sqrt_nr(-2.0 * log_unit(u1));
   double s, c;
   sincospi_2u(fma(one_plus_u01_from_bits(x.x2, x.x3), 2.0, -2.0), &s, &c);    // 2 u2, u2 in [0, 1), exact
   return Normal2{r * c, r * s};
+}
+
+__device__ __forceinline__ Normal2 normal_pair(uint32_t t, uint32_t draw, uint32_t run_lo,
+                                               uint32_t run_hi, uint32_t k0, uint32_t k1) {
+  return normal_from_words(philox4x32_10(t, draw, run_lo, run_hi, k0, k1));
 }
 
 __device__ __forceinline__ double uniform01(uint32_t t, uint32_t draw, uint32_t run_lo,

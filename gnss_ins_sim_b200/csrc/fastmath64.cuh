@@ -4,13 +4,27 @@
 // instructions are inside sincos / log / sincospi.  The CUDA libm versions are written for
 // the whole double range (huge-argument Payne-Hanek path, denormals, NaN/Inf plumbing,
 // table lookups).  Here every call site has a small, known argument range:
-//   sincos_bounded   |x| <= 64            (Euler angles live in [-pi, pi]; lat/lon too)
+//   sincos_bounded   |x| <= 1e6           (Euler angles live in [-pi, pi]; lat/lon too; mech.cuh's
+//                                          sincos_angle maps larger angles to 0)
 //   sincospi_2u      x = 2u, u in [0, 1)  (Box-Muller angle)
 //   log_unit         x in [2^-52, 1]      (Box-Muller radius)
-// so a two/three-term Cody-Waite reduction and the classic minimax kernels (the public
+// so a three-term Cody-Waite reduction and the classic minimax kernels (the public
 // fdlibm / SunPro polynomial coefficients for sin, cos on [-pi/4, pi/4] and log on
-// [sqrt(1/2), sqrt(2)]) are enough.  Accuracy: <= 1.5 ulp (tools/check_fastmath.cu measures
-// it against long double libm); the parity tests see ~1e-12 end to end, as with CUDA libm.
+// [sqrt(1/2), sqrt(2)]) are enough; the parity tests see ~1e-12 end to end, as with CUDA libm.
+//
+// Accuracy, measured on the device (H100) against an exact reference at the hard cases and ~2^22 random
+// arguments per domain (tests/test_gpu_fastmath.py; the host forms in tests/test_cpu_fastmath.py):
+//   sincos_bounded   |x| <= 64: <= 1.6 ulp + |q| 8.5e-32 absolute (worst 1.554 ulp), q = rint(x 2/pi):
+//                    the split of pi/2 ends at PIO2_3, so results near the zeros of sin and cos, where
+//                    the reduced argument is tiny, carry up to 2.6e4 ulp (3e-30 absolute);
+//                    64 < |x| <= 1e6: <= 2.5 ulp + |q| 8.5e-32 (worst 2.39 ulp)
+//   sincospi_2u      <= 3e-16 absolute (worst 1.94e-16); exact at 0, 1/2, 1, 3/2
+//   log_unit         <= 2 ulp (worst 0.744 ulp; nvcc contracts five multiply/add pairs into DFMAs, so the
+//                    device's instruction sequence is not the host's)
+//   sqrt_nr          <= 0.5005 ulp on [0, 72.1] (worst 0.5: correctly rounded on every tested argument)
+//   rsqrt_nr         <= 1 ulp on [0.9933, 1] (worst 0.626)
+//   rcp_nr, div_nr   <= 1 ulp at their call sites (worst 0.5: correctly rounded on every tested argument)
+// sincos_bounded and sincospi_2u have no contractible pairs: device and host results are identical bits.
 //
 // All functions are __host__ __device__ so that the accuracy check runs on the CPU.
 #pragma once

@@ -31,8 +31,11 @@ struct SinCos3 {
 };
 
 // sin/cos of an angle that normally lives in [-pi, pi] (Euler angles after their wrap,
-// latitude, longitude).  sincos_bounded's three-term reduction stays accurate far beyond that
-// (|x| < 1e6: error < 1e-10); larger magnitudes are only reachable after the Euler-angle
+// latitude, longitude).  sincos_bounded's three-term reduction stays accurate far beyond that:
+// for 64 < |x| <= 1e6 the error is at most 2.5 ulp of the result + |q| 8.5e-32 absolute (q the
+// quadrant index, up to 636 620; the second term is the split of pi/2 ending at PIO2_3, 5.4e-26 at
+// 1e6), measured worst 2.39 ulp (tests/test_cpu_fastmath.py and, on the device, test_gpu_fastmath.py).
+// Larger magnitudes are only reachable after the Euler-angle
 // singularity at pitch = +-pi/2 has blown a rate up, where the recurrence is meaningless
 // anyway -- they are mapped to the angle 0 by a select (branch-free, off the critical path).
 // A NaN or an infinite angle maps to x - x = NaN, so its sin/cos are NaN as the reference's np.sin/np.cos

@@ -588,6 +588,30 @@ int b2ins_diag_mc_shape(int lanes_per_run, int ref_frame, int* shape3);
  * per process, as the launch reads it).  Returns -1 if n <= 0 or P is NULL.  Pure host logic. */
 int b2ins_diag_psd_plan(int64_t n, int* P);
 
+/* The device's own FP64 primitives (csrc/fastmath64.cuh, and mech.cuh's sincos_angle), applied
+ * elementwise to n arguments: out0[i] = f(a[i]) (div: a[i] / b[i]); the sin/cos functions write
+ * sin to out0 and cos to out1.  Each kernel inlines the production function itself.  Device
+ * pointers; synchronous.  An unknown fn is B2INS_ERR_ARG. */
+enum {
+  B2INS_FM_RCP = 0,          /* rcp_nr(a)           */
+  B2INS_FM_DIV = 1,          /* div_nr(a, b)        */
+  B2INS_FM_SQRT = 2,         /* sqrt_nr(a)          */
+  B2INS_FM_RSQRT = 3,        /* rsqrt_nr(a)         */
+  B2INS_FM_SINCOS = 4,       /* sincos_bounded(a)   */
+  B2INS_FM_SINCOS_ANGLE = 5, /* sincos_angle(a)     */
+  B2INS_FM_SINCOSPI = 6,     /* sincospi_2u(a)      */
+  B2INS_FM_LOG = 7           /* log_unit(a)         */
+};
+int b2ins_diag_fastmath_f64(int fn, int64_t n, const double* a, const double* b, double* out0, double* out1);
+
+/* The noise generator's Philox4x32-10 on n (counter[4], key[2]) rows of ctr_key [n][6]:
+ * words [n][4].  Device pointers; synchronous. */
+int b2ins_diag_philox(int64_t n, const uint32_t* ctr_key, uint32_t* words);
+
+/* The noise generator's Box-Muller pair from n Philox outputs words [n][4] (the normal_from_words
+ * that every noise draw goes through): z [n][2] = (z0, z1).  Device pointers; synchronous. */
+int b2ins_diag_normal_from_words(int64_t n, const uint32_t* words, double* z);
+
 #ifdef __cplusplus
 }
 #endif
