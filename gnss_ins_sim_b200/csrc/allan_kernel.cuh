@@ -6,12 +6,13 @@
 // S_k[10i..10i+9]) and yields the nine cluster sizes j*10^k plus S_{k+1}; the series is
 // read from HBM once (level 0) instead of once per tau as the reference does.
 //
-// One CTA owns one (series, chunk) pair; a chunk is kAllanChunk = 2*2520 level-k elements
+// A tile is one (series, chunk) pair; a chunk is kAllanChunk = 2*2520 level-k elements
 // (2520 = lcm(1..10): every cluster size starts a cluster at each chunk start) plus a
-// 9-element halo for the cluster that ends where the chunk starts.  The tile is prefix-
-// summed in shared memory (after subtracting its first element, which cancels exactly in
-// every difference and keeps the prefix small), so a successive-difference term is
-//   sum(bin b+1) - sum(bin b) = P[(b+2)j] - 2 P[(b+1)j] + P[bj].
+// 9-element halo for the cluster that ends where the chunk starts.  Every successive-difference
+// term is the difference of two cluster sums formed directly from the samples of its two bins, so
+// a non-finite sample reaches only the terms whose bins hold it, as in the reference.  Where a
+// tile subtracts an offset (its first element, which cancels in every difference), it uses it
+// only when it is finite: an infinite offset would turn every term of the tile into inf - inf.
 #pragma once
 #include <cstring>
 
@@ -22,7 +23,6 @@ namespace b2ins {
 
 constexpr int kAllanChunk = 5040;
 constexpr int kAllanHalo = 9;
-constexpr int kAllanThreads = 256;
 constexpr int kAllanMaxLevels = 10;
 
 struct AllanLevelParams {
@@ -41,121 +41,6 @@ struct AllanLevelParams {
   int64_t src_pitch;     // row pitch of S_k (levels >= 1) and of S_{k+1}: even, so that rows are
   int64_t next_pitch;    // 16-byte aligned for the bulk copies
 };
-
-__global__ void __launch_bounds__(kAllanThreads) allan_level_kernel(const __grid_constant__ AllanLevelParams p) {
-  extern __shared__ __align__(128) double tile[];  // [kAllanHalo + kAllanChunk + 1] prefix, tile[0] = 0
-  __shared__ double red[kAllanThreads / 32][9];
-  __shared__ double sh_scan[kAllanThreads];
-  const int64_t series = blockIdx.x / p.chunk_count;
-  const int64_t chunk = p.chunk_first + blockIdx.x % p.chunk_count;
-  const int64_t c0 = chunk * kAllanChunk;                 // first element of the chunk
-  const int halo = (chunk == 0) ? 0 : kAllanHalo;          // elements before c0 in the tile
-  const int64_t lo = c0 - halo;
-  const int cnt = static_cast<int>(min64(kAllanChunk, p.len - c0)) + halo;  // tile elems
-  const double* base;
-  int64_t stride;
-  if (p.level0) {
-    base = p.src + (series / p.inner) * p.outer_stride + (series % p.inner);
-    stride = p.sample_stride;
-  } else {
-    base = p.src + series * p.src_pitch;
-    stride = 1;
-  }
-  const double off = base[lo * stride];
-  // P[i] = sum_{q<i} (x[lo+q] - off), i = 0..cnt ; stored at tile[i]
-  // elements per thread in the serial part of the scan: odd, so that the threads of a warp walk
-  // shared memory with an odd stride (no bank conflicts)
-  constexpr int kPer = ((kAllanChunk + kAllanHalo + kAllanThreads - 1) / kAllanThreads) | 1;  // 21
-  // coalesced load into the tile (raw values), then a per-thread serial scan of kPer
-  // consecutive elements + block scan of the thread totals
-  {
-    // every load is issued before the first store (kPer independent requests in flight per thread)
-    double v[kPer];
-#pragma unroll
-    for (int q = 0; q < kPer; ++q) {
-      const int i = threadIdx.x + q * kAllanThreads;
-      v[q] = (i < cnt) ? base[(lo + i) * stride] : 0.0;
-    }
-#pragma unroll
-    for (int q = 0; q < kPer; ++q) {
-      const int i = threadIdx.x + q * kAllanThreads;
-      if (i < cnt) tile[1 + i] = v[q] - off;
-    }
-  }
-  if (threadIdx.x == 0) tile[0] = 0.0;
-  __syncthreads();
-  const int b0 = threadIdx.x * kPer;
-  double run = 0.0;
-  for (int q = 0; q < kPer; ++q) {
-    const int i = b0 + q;
-    if (i < cnt) {
-      run += tile[1 + i];
-      tile[1 + i] = run;
-    }
-  }
-  sh_scan[threadIdx.x] = run;
-  __syncthreads();
-  // exclusive scan of thread totals (Hillis-Steele in shared memory)
-  for (int o = 1; o < kAllanThreads; o <<= 1) {
-    const double v = (threadIdx.x >= o) ? sh_scan[threadIdx.x - o] : 0.0;
-    __syncthreads();
-    sh_scan[threadIdx.x] += v;
-    __syncthreads();
-  }
-  const double pre = (threadIdx.x == 0) ? 0.0 : sh_scan[threadIdx.x - 1];
-  for (int q = 0; q < kPer; ++q) {
-    const int i = b0 + q;
-    if (i < cnt) tile[1 + i] += pre;
-  }
-  __syncthreads();
-
-  // successive-difference terms whose SECOND bin starts inside this chunk
-  double acc[9];
-#pragma unroll
-  for (int j = 0; j < 9; ++j) acc[j] = 0.0;
-#pragma unroll
-  for (int j = 1; j <= 9; ++j) {
-    if (j <= p.jmax) {
-      const int64_t nb = p.len / j;  // bins of this cluster size in the whole series
-      // second bins b2 with c0 <= b2*j < c0 + kAllanChunk, 1 <= b2 <= nb-1
-      int64_t b2_lo = (c0 + j - 1) / j;
-      if (b2_lo < 1) b2_lo = 1;
-      int64_t b2_hi = (c0 + kAllanChunk + j - 1) / j;  // exclusive
-      if (b2_hi > nb) b2_hi = nb;
-      for (int64_t b2 = b2_lo + threadIdx.x; b2 < b2_hi; b2 += kAllanThreads) {
-        const int e1 = static_cast<int>(b2 * j - lo);  // tile index of the bin boundary
-        const double d = tile[e1 + j] - 2.0 * tile[e1] + tile[e1 - j];
-        acc[j - 1] += d * d;
-      }
-    }
-  }
-  // block reduction (warp shuffles, then one shared-memory hop), fixed order
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int j = 0; j < 9; ++j) {
-    double v = acc[j];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    if (lane == 0) red[warp][j] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    double v = 0.0;
-    for (int w = 0; w < kAllanThreads / 32; ++w) v += red[w][threadIdx.x];
-    p.partial[(series * p.chunks + chunk) * 9 + threadIdx.x] = v;
-  }
-  // decade sums for the next level
-  if (p.next_len > 0) {
-    const int64_t d_lo = c0 / 10;
-    for (int i = threadIdx.x; i < kAllanChunk / 10; i += kAllanThreads) {
-      const int64_t di = d_lo + i;
-      if (di < p.next_len) {
-        const int e = halo + i * 10;
-        p.next[series * p.next_pitch + di] = (tile[e + 10] - tile[e]) + 10.0 * off;
-      }
-    }
-  }
-}
 
 // ---- fast path: FULL chunks ---------------------------------------------------------------
 // A full chunk holds an integer number of clusters of every size (5040 = 2 lcm(1..10)), so the
@@ -176,7 +61,7 @@ __global__ void __launch_bounds__(kAllanThreads) allan_level_kernel(const __grid
 //                        flight behind the one being computed), the padded copy and the block
 //                        reduction are double-buffered: ONE __syncthreads per tile;
 //   allan_full_kernel    any stride / alignment: per-thread loads, one tile per CTA.
-// The prefix-sum kernel above remains the path for the ragged last chunk of a series.
+// Both take the ragged last chunk of a series with the masked form of the same work items.
 constexpr int kAllanItemsX = kAllanChunk / 48;    // 105
 constexpr int kAllanItemsY = kAllanChunk / 18;    // 280
 constexpr int kAllanItemsC = kAllanChunk / 70;    // 72
@@ -434,7 +319,10 @@ __global__ void __launch_bounds__(kAllanFastThreads, 2) allan_full_kernel(const 
     base = p.src + series * p.src_pitch;
     stride = 1;
   }
-  const double off = p.level0 ? 0.0 : base[(c0 - (has_prev ? kAllanHalo : 0)) * stride];
+  const double off0 = p.level0 ? 0.0 : base[(c0 - (has_prev ? kAllanHalo : 0)) * stride];
+  const double off = isfinite(off0) ? off0 : 0.0;
+  const bool ragged = c0 + kAllanChunk > p.len;
+  const int cnt = ragged ? static_cast<int>(p.len - c0) : kAllanChunk;   // elements of the chunk
   {
     // loaders: thread (g, pos) loads element 48 (7 q + g) + pos in pass q; every load is issued
     // before the first use (15 independent requests in flight per thread)
@@ -446,7 +334,8 @@ __global__ void __launch_bounds__(kAllanFastThreads, 2) allan_full_kernel(const 
     double hv = 0.0;
     if (tid < kLoaders) {
 #pragma unroll
-      for (int q = 0; q < kPasses; ++q) v[q] = src[static_cast<int64_t>(q) * kLoaders * stride];
+      for (int q = 0; q < kPasses; ++q)
+        v[q] = (48 * (7 * q + g) + pos < cnt) ? src[static_cast<int64_t>(q) * kLoaders * stride] : 0.0;
     } else if (has_prev && tid < kLoaders + kAllanHalo) {
       hv = base[(c0 - kAllanHalo + (tid - kLoaders)) * stride];
     }
@@ -466,10 +355,17 @@ __global__ void __launch_bounds__(kAllanFastThreads, 2) allan_full_kernel(const 
   }
   __syncthreads();
   double acc[4];
-  if (p.level0)
-    allan_tile_compute<false, false>(p, series, chunk, in, pad, 0.0, acc);
-  else
-    allan_tile_compute<true, false>(p, series, chunk, in, pad, off, acc);
+  if (p.level0) {
+    if (ragged)
+      allan_tile_compute<false, true>(p, series, chunk, in, pad, 0.0, acc);
+    else
+      allan_tile_compute<false, false>(p, series, chunk, in, pad, 0.0, acc);
+  } else {
+    if (ragged)
+      allan_tile_compute<true, true>(p, series, chunk, in, pad, off, acc);
+    else
+      allan_tile_compute<true, false>(p, series, chunk, in, pad, off, acc);
+  }
   allan_tile_reduce(acc, red);
   __syncthreads();
   if (tid < 9) allan_tile_fold(p, series, chunk, red);
@@ -530,7 +426,8 @@ __global__ void __launch_bounds__(kAllanFastThreads, 1) allan_stream_kernel(cons
     mbar_wait(&full[slot], (it / kAllanStages) & 1);
     const double* in = in_buf + slot * kAllanRawLen;
     double* pad = pad_buf + (it & 1) * kAllanPadLen + kAllanPadLead;
-    const double off = SUB ? in[chunk != 0 ? 1 : kAllanLead] : 0.0;
+    const double off0 = SUB ? in[chunk != 0 ? 1 : kAllanLead] : 0.0;
+    const double off = isfinite(off0) ? off0 : 0.0;
     {
       // X's copy: units of two samples; the five halo units land just below pad[0]
       const double2* in2 = reinterpret_cast<const double2*>(in);
@@ -813,7 +710,7 @@ __global__ void __launch_bounds__(kAllanRestThreads) allan_rest_kernel(const __g
     const double* x = (k & 1) ? buf_b : buf_a;
     double* nx = (k & 1) ? buf_a : buf_b;
     // the first element cancels in every difference: subtracting it keeps the cluster sums small
-    const double off = x[0];
+    const double off = isfinite(x[0]) ? x[0] : 0.0;
     double acc[9];
 #pragma unroll
     for (int j = 1; j <= 9; ++j) {
@@ -909,7 +806,6 @@ inline int allan_launch(double fs, int64_t n, int64_t nseries, const double* x, 
   double* buf[2] = {ws, ws + n1 * nseries};
   double* part = ws + 2 * n1 * nseries;
   int64_t len = n;
-  const size_t smem = (kAllanChunk + kAllanHalo + 1 + 16) * sizeof(double);
   const size_t smem_full = (kAllanRawLen + kAllanPadLen) * sizeof(double);
   const size_t smem_stream = (kAllanStages * kAllanRawLen + 2 * kAllanPadLen) * sizeof(double);
   const size_t smem_gen = (2 * kAllanRawLen + 2 * kAllanPadLen) * sizeof(double);
@@ -920,9 +816,6 @@ inline int allan_launch(double fs, int64_t n, int64_t nseries, const double* x, 
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
   bool& attr_set = attr_done[dev];
   if (!attr_set) {
-    if (cudaFuncSetAttribute(allan_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             static_cast<int>(smem)) != cudaSuccess)
-      return 2;
     if (cudaFuncSetAttribute(allan_full_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              static_cast<int>(smem_full)) != cudaSuccess ||
         cudaFuncSetAttribute(allan_full_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -934,13 +827,11 @@ inline int allan_launch(double fs, int64_t n, int64_t nseries, const double* x, 
         cudaFuncSetAttribute(allan_gen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              static_cast<int>(smem_gen)) != cudaSuccess)
       return 2;
-    // both kernels stage everything through shared memory: ask for the largest carve-out so that
-    // two (fast kernel) / five (tail kernel) CTAs are resident per SM
+    // the kernel stages everything through shared memory: ask for the largest carve-out so that
+    // two CTAs are resident per SM
     cudaFuncSetAttribute(allan_full_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout,
                          cudaSharedmemCarveoutMaxShared);
     cudaFuncSetAttribute(allan_full_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                         cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(allan_level_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                          cudaSharedmemCarveoutMaxShared);
     attr_set = true;
   }
@@ -985,8 +876,6 @@ inline int allan_launch(double fs, int64_t n, int64_t nseries, const double* x, 
       allan_rest_kernel<<<static_cast<unsigned>(nseries), kAllanRestThreads, 0, s>>>(rp);
       break;
     }
-    // full chunks (every cluster complete, next-level decades complete) take the fast kernels
-    const int64_t full = len / kAllanChunk;
     const bool contiguous = !lp.level0 || sample_stride == 1;
     // the bulk copies need 16-byte aligned rows: always true for the decade sums (even pitch),
     // for the caller's series if the base and the row stride allow it
@@ -1010,20 +899,14 @@ inline int allan_launch(double fs, int64_t n, int64_t nseries, const double* x, 
       else
         allan_stream_kernel<true><<<static_cast<unsigned>(grid), kAllanFastThreads, smem_stream, s>>>(lp);
     } else {
-      if (full > 0) {
-        lp.chunk_first = 0;
-        lp.chunk_count = full;
-        const int64_t tiles = full * nseries;
-        if (contiguous)
-          allan_full_kernel<true><<<static_cast<unsigned>(tiles), kAllanFastThreads, smem_full, s>>>(lp);
-        else
-          allan_full_kernel<false><<<static_cast<unsigned>(tiles), kAllanFastThreads, smem_full, s>>>(lp);
-      }
-      if (lp.chunks > full) {   // the ragged last chunk
-        lp.chunk_first = full;
-        lp.chunk_count = lp.chunks - full;
-        allan_level_kernel<<<static_cast<unsigned>(lp.chunk_count * nseries), kAllanThreads, smem, s>>>(lp);
-      }
+      // one tile per CTA, every chunk of every series (the ragged last one is masked)
+      lp.chunk_first = 0;
+      lp.chunk_count = lp.chunks;
+      const int64_t tiles = lp.chunks * nseries;
+      if (contiguous)
+        allan_full_kernel<true><<<static_cast<unsigned>(tiles), kAllanFastThreads, smem_full, s>>>(lp);
+      else
+        allan_full_kernel<false><<<static_cast<unsigned>(tiles), kAllanFastThreads, smem_full, s>>>(lp);
     }
     len /= 10;
   }

@@ -532,6 +532,7 @@ def allan_var(x, fs):
     mult = allan_multipliers(n, fs)
     if not mult:
         return np.array([]), np.array([])
+    ts = 1.0 / fs
     avar = np.zeros(len(mult))
     tau = np.zeros(len(mult))
     for i, m in enumerate(mult):
@@ -541,7 +542,7 @@ def allan_var(x, fs):
         means = np.mean(x[:nb * m].reshape(nb, m), 1)
         d = means[1:] - means[:-1]
         avar[i] = 0.5 / (nb - 1) * np.sum(d * d)
-        tau[i] = m / fs
+        tau[i] = m * ts          # allan.py:58 (not m / fs: the two differ in the last bit)
     return avar, tau
 
 
