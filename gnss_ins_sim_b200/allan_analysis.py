@@ -1,7 +1,8 @@
 """Allan plugin -- device-backed mirror of demo_algorithms/allan_analysis.py:15-61
 (input ['fs','accel','gyro'], output ['algo_time','ad_accel','ad_gyro']); the variance
 itself is csrc/allan_kernel.cuh (K4, allan.allan_var allan.py:18-59) or, overlapping,
-csrc/oallan_kernel.cuh (K4o)."""
+csrc/oallan_kernel.cuh (K4o).  Hadamard: the overlapping Hadamard deviation on the same
+tau grid (K4o's Hadamard form), output ['algo_time','hd_accel','hd_gyro']."""
 import numpy as np
 import torch
 
@@ -48,7 +49,7 @@ class Allan(object):
         '''
         a = engine.to_device(accel)
         g = engine.to_device(gyro)
-        var = engine.oallan if self.overlapping else engine.allan
+        var = self._variance()
         out = []
         for x in (a, g):
             if channel_major:     # 3R contiguous series: the bulk-copy front end of K4
@@ -62,8 +63,32 @@ class Allan(object):
             return tau.cpu().numpy(), out[0].cpu().numpy(), out[1].cpu().numpy()
         return tau, out[0], out[1]
 
+    def _variance(self):
+        return engine.oallan if self.overlapping else engine.allan
+
     def get_results(self):
         return self.results
 
     def reset(self):
         pass
+
+
+class Hadamard(Allan):
+    '''
+    Overlapping Hadamard deviation of the three accelerometer and three gyroscope channels
+    (NIST SP 1065), on Allan's tau grid (m = j*10^k <= n/9):
+        hvar(m) = 1 / (6 m^2 H) * sum_{k<H} (S(k+2m, m) - 2 S(k+m, m) + S(k, m))^2,  H = n - 3m + 1,
+    with S(k, m) the sum of the m samples from k.  A second difference of adjacent cluster sums: a linear
+    drift of the rate (thermal drift, the rate ramp R of IEEE Std 952), which adds b^2 tau^2 / 2 to the
+    Allan variance and hides bias instability and rate random walk at long tau, cancels exactly.  White
+    noise gives sigma^2 / m as the Allan variance does, so the two curves can be laid over each other.
+    run / run_batch / get_results / reset as Allan's; the deviations are published as hd_accel and
+    hd_gyro, never as ad_*.
+    '''
+
+    def __init__(self):
+        super().__init__(overlapping=True)
+        self.output = ['algo_time', 'hd_accel', 'hd_gyro']
+
+    def _variance(self):
+        return engine.ohadamard

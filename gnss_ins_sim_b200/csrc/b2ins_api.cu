@@ -1434,9 +1434,10 @@ int64_t b2ins_oallan_workspace_bytes(int64_t n, int64_t nseries) {
   return oallan_workspace_bytes(n, nseries);
 }
 
-int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
-                     int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
-                     void* workspace, void* stream) {
+// K4o and its Hadamard form: one argument check and one launch; the workspace serves both
+static int oallan_f64(bool hadamard, double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                      int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
+                      void* workspace, void* stream) {
   ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
   ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
   int64_t mult[128];
@@ -1445,15 +1446,19 @@ int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x, int
   ARG_CHECK(ntau <= 128, "too many tau");
   ARG_CHECK(x && avar && tau && workspace, "null buffer");
   const int rc = oallan_launch(fs, n, nseries, x, inner, outer_stride, sample_stride, mult, ntau, avar, tau,
-                               workspace, static_cast<cudaStream_t>(stream));
-  if (rc == 4) return fail(B2INS_ERR_ARG, "overlapping Allan: too many series x samples for one call");
-  if (rc != 0) return fail(B2INS_ERR_CUDA, "oallan launch failed (%d): %s", rc, cudaGetErrorString(cudaGetLastError()));
+                               workspace, static_cast<cudaStream_t>(stream), hadamard);
+  if (rc == 4)
+    return fail(B2INS_ERR_ARG, "overlapping %s: too many series x samples for one call",
+                hadamard ? "Hadamard" : "Allan");
+  if (rc != 0)
+    return fail(B2INS_ERR_CUDA, "%s launch failed (%d): %s", hadamard ? "ohadamard" : "oallan", rc,
+                cudaGetErrorString(cudaGetLastError()));
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
 
-int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
-                          int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
+static int oallan_f64_host(bool hadamard, double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                           int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
   ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
   ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
   const int ntau = b2ins_allan_num_tau(n, fs, nullptr, 0);
@@ -1470,8 +1475,8 @@ int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x
   CU_CHECK(ws.alloc(static_cast<size_t>(oallan_workspace_bytes(n, nseries))));
   CU_CHECK(cudaMemcpyAsync(dx.p, x, static_cast<size_t>(elems) * sizeof(double),
                            cudaMemcpyHostToDevice, st.s));
-  const int rc = b2ins_oallan_f64(fs, n, nseries, dx.d(), inner, outer_stride, sample_stride,
-                                  dav.d(), dtau.d(), ws.p, st.s);
+  const int rc = oallan_f64(hadamard, fs, n, nseries, dx.d(), inner, outer_stride, sample_stride,
+                            dav.d(), dtau.d(), ws.p, st.s);
   if (rc != B2INS_OK) return rc;
   CU_CHECK(cudaMemcpyAsync(avar, dav.p, static_cast<size_t>(nseries) * ntau * sizeof(double),
                            cudaMemcpyDeviceToHost, st.s));
@@ -1479,6 +1484,28 @@ int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x
                            cudaMemcpyDeviceToHost, st.s));
   CU_CHECK(cudaStreamSynchronize(st.s));
   return B2INS_OK;
+}
+
+int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                     int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
+                     void* workspace, void* stream) {
+  return oallan_f64(false, fs, n, nseries, x, inner, outer_stride, sample_stride, avar, tau, workspace, stream);
+}
+
+int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                          int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
+  return oallan_f64_host(false, fs, n, nseries, x, inner, outer_stride, sample_stride, avar, tau);
+}
+
+int b2ins_ohadamard_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                        int64_t outer_stride, int64_t sample_stride, double* hvar, double* tau,
+                        void* workspace, void* stream) {
+  return oallan_f64(true, fs, n, nseries, x, inner, outer_stride, sample_stride, hvar, tau, workspace, stream);
+}
+
+int b2ins_ohadamard_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                             int64_t outer_stride, int64_t sample_stride, double* hvar, double* tau) {
+  return oallan_f64_host(true, fs, n, nseries, x, inner, outer_stride, sample_stride, hvar, tau);
 }
 
 // ---------------------------------------------------------------- K5 --------

@@ -13,15 +13,31 @@
 // d = (D_2m.hi - 2 D_m.hi) + (D_2m.lo - 2 D_m.lo): both hi terms are ~2 S and the subtraction is
 // exact whenever they are within a factor of two.
 //
+// Hadamard form (HAD = true in passes 4 and 5): the overlapping Hadamard variance (NIST SP 1065) on the
+// same grid, a second difference of three adjacent window sums, so a linear drift cancels exactly:
+//   H = n - 3m + 1,
+//   hvar(m) = 1 / (6 m^2 H) * sum_{k=0}^{H-1} (S(k+2m, m) - 2 S(k+m, m) + S(k, m))^2
+//           = 1 / (6 m^2 H) * sum_{k=0}^{H-1} (C[k+3m] - 3 C[k+2m] + 3 C[k+m] - C[k])^2.
+// Precision of its term.  3 h is not exact as 2 h is, so the term is never formed from 3 C or 3 D.  The
+// window sums S_i = C[k+(i+1)m] - C[k+im] (i = 0, 1, 2) are taken straight from the prefix, each by an
+// exact TwoDiff of the hi parts (its error goes to lo) plus the lo difference; then
+//   t = ((S2.hi - S1.hi) - (S1.hi - S0.hi)) + ((S2.lo - S1.lo) - (S1.lo - S0.lo)).
+// A hi subtraction is exact (Sterbenz) when its operands are within a factor of two: adjacent window
+// sums are whenever a level or a drift dominates them, and the two first differences are whenever the
+// drift dominates the term, the cases in which the prefix is large beside the term.  An inexact one
+// rounds by at most half an ulp of a first difference of window sums, never of the prefix.  Only the
+// lo sums and the final add round otherwise; the lo parts are of the order of an ulp of C.
+//
 // Passes (one stream, five launches; tiles are fixed by n alone):
 //   1 oallan_tile_kernel<false>  per (series, scan tile): the tile's double-double total of x - x_0,
 //                                its +inf / -inf counts and NaN / inf flags
 //   2 oallan_carry_kernel        per series, sequential over its tiles: the series' class (finite,
 //                                inf without NaN, NaN) and the exclusive carry of every tile
 //   3 oallan_tile_kernel<true>   per (series, scan tile): C written to the workspace [nseries][n+1]
-//   4 oallan_sq_kernel           per (series, decade, output tile): the nine sizes j*10^d share the
-//                                14 lags {1..10, 12, 14, 16, 18}*10^d of C[k]; nine partial sums
-//   5 oallan_final_kernel        per (series, tau): the tiles' partials, folded in a fixed order
+//   4 oallan_sq_kernel<HAD>      per (series, decade, output tile): the nine sizes j*10^d share the
+//                                14 lags {1..10, 12, 14, 16, 18}*10^d of C[k] (Hadamard: 18 lags
+//                                {1..10, 12, 14, 15, 16, 18, 21, 24, 27}*10^d); nine partial sums
+//   5 oallan_final_kernel<HAD>   per (series, tau): the tiles' partials, folded in a fixed order
 //
 // Determinism: every sum runs in an order fixed by n (thread-serial runs, fixed butterflies, warps
 // and tiles in index order), never by the grid, the batch or the position of a series in it.
@@ -32,7 +48,10 @@
 // term is inf or NaN when its windows hold an inf, and it is NaN exactly when one window holds both
 // signs or both windows hold the same sign.  For these series pass 3 writes the prefix COUNTS of
 // +inf (hi) and -inf (lo) samples instead (exact small integers), pass 4 counts the NaN terms with
-// the same lags, and pass 5 gives NaN if there is one, else +inf.
+// the same lags, and pass 5 gives NaN if there is one, else +inf.  A Hadamard term is NaN exactly when
+// its signed contributions +S2, -2 S1, +S0 hold both infinities: a window holds both signs, or S2 and
+// S0 are infinite with opposite signs, or S1 is infinite with the sign of S2 or of S0.  That is what
+// the definitional sum gives in IEEE arithmetic, whatever the order of its additions.
 #pragma once
 #include <cmath>
 #include <cstring>
@@ -49,6 +68,7 @@ constexpr int kOallanSqPer = 8;                                             // o
 constexpr int kOallanSqTile = kOallanSqThreads * kOallanSqPer;              // 2048
 constexpr int kOallanMaxDec = 10;
 constexpr int kOallanLags = 14;
+constexpr int kOhadLags = 18;
 
 enum { kOallanFinite = 0, kOallanInf = 1, kOallanNan = 2 };
 
@@ -256,9 +276,13 @@ __global__ void __launch_bounds__(128) oallan_carry_kernel(const __grid_constant
   }
 }
 
-// Pass 4.  Thread tid takes offsets k = k0 + tid + 256 q; for each it forms the 14 lag differences
-// D_L = C[k + L 10^d] - C[k] once and the nine terms from them (size j: D_j and D_2j).
+// Pass 4.  Thread tid takes offsets k = k0 + tid + 256 q; for each it loads the prefix at the lags
+// once.  Allan: the 14 lag differences D_L = C[k + L 10^d] - C[k], and the nine terms from them (size
+// j: D_j and D_2j).  Hadamard: the 18 lags, and size j's window sums between lags 0, j, 2j and 3j.
+template <bool HAD>
 __global__ void __launch_bounds__(kOallanSqThreads) oallan_sq_kernel(const __grid_constant__ OallanParams p) {
+  constexpr int kSpan = HAD ? 3 : 2;          // windows per term
+  constexpr int kLags = HAD ? kOhadLags : kOallanLags;
   __shared__ double red[kOallanSqThreads / 32][9];
   const int64_t per_series = static_cast<int64_t>(p.ndec) * p.sq_tiles;
   const int64_t s = blockIdx.x / per_series;
@@ -275,19 +299,38 @@ __global__ void __launch_bounds__(kOallanSqThreads) oallan_sq_kernel(const __gri
 #pragma unroll
   for (int j = 0; j < 9; ++j) acc[j] = 0.0;
   constexpr int kLag[kOallanLags] = {1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 12, 14, 16, 18};
+  constexpr int kHadLag[kOhadLags] = {1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 12, 14, 15, 16, 18, 21, 24, 27};
+  constexpr int kHad2[9] = {1, 3, 5, 7, 9, 10, 11, 13, 14};       // slot of lag 2j in kHadLag
+  constexpr int kHad3[9] = {2, 5, 8, 10, 12, 14, 15, 16, 17};     // slot of lag 3j
   if (mode != kOallanNan) {
     for (int q = 0; q < kOallanSqPer; ++q) {
       const int64_t k = tile * kOallanSqTile + q * kOallanSqThreads + tid;
-      if (k + 2 * u > n) break;   // no term of any size of this decade starts here
+      if (k + kSpan * u > n) break;   // no term of any size of this decade starts here
       const double2 c0 = __ldg(c + k);
-      double2 cl[kOallanLags];
+      double2 cl[kLags];
 #pragma unroll
-      for (int l = 0; l < kOallanLags; ++l) {
-        const int64_t i = k + kLag[l] * u;
+      for (int l = 0; l < kLags; ++l) {
+        const int64_t i = k + (HAD ? kHadLag[l] : kLag[l]) * u;
         cl[l] = (i <= n) ? __ldg(c + i) : c0;
       }
 #pragma unroll
       for (int j = 1; j <= 9; ++j) {
+        if (HAD) {
+          if (j <= jmax && k + 3 * j * u <= n) {
+            const double2 c1 = cl[j - 1], c2 = cl[kHad2[j - 1]], c3 = cl[kHad3[j - 1]];
+            if (mode == kOallanFinite) {   // window sums S0, S1, S2 (see the file comment)
+              const DD s0 = dd_diff(c1, c0), s1 = dd_diff(c2, c1), s2 = dd_diff(c3, c2);
+              const double t = __dadd_rn(__dsub_rn(__dsub_rn(s2.hi, s1.hi), __dsub_rn(s1.hi, s0.hi)),
+                                         __dsub_rn(__dsub_rn(s2.lo, s1.lo), __dsub_rn(s1.lo, s0.lo)));
+              acc[j - 1] = fma(t, t, acc[j - 1]);
+            } else {   // +inf (x) / -inf (y) counts; an inf of S1 enters the term with its sign flipped
+              const bool pos = c1.x > c0.x || c2.y > c1.y || c3.x > c2.x;
+              const bool neg = c1.y > c0.y || c2.x > c1.x || c3.y > c2.y;
+              acc[j - 1] += (pos && neg) ? 1.0 : 0.0;
+            }
+          }
+          continue;
+        }
         if (j <= jmax && k + 2 * j * u <= n) {
           const int l1 = j - 1, l2 = (j <= 5) ? 2 * j - 1 : j + 4;   // lags j and 2j
           const DD a = dd_diff(cl[l1], c0), b = dd_diff(cl[l2], c0);
@@ -333,6 +376,7 @@ struct OallanFinalParams {
 };
 
 // Pass 5: one warp per (series, tau), lanes over the tiles in order, then a fixed butterfly.
+template <bool HAD>
 __global__ void __launch_bounds__(128) oallan_final_kernel(const __grid_constant__ OallanFinalParams p) {
   const int64_t idx = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (idx >= p.nseries * p.ntau) return;
@@ -352,6 +396,8 @@ __global__ void __launch_bounds__(128) oallan_final_kernel(const __grid_constant
       a = NAN;
     else if (mode == kOallanInf)
       a = v > 0.0 ? NAN : INFINITY;
+    else if (HAD)
+      a = v / (6.0 * m * m * static_cast<double>(p.n - 3 * p.m[i] + 1));
     else
       a = v / (2.0 * m * m * static_cast<double>(p.n - 2 * p.m[i] + 1));
     p.avar[s * p.ntau + i] = a;
@@ -392,10 +438,11 @@ inline int64_t oallan_workspace_bytes(int64_t n, int64_t nseries) {
   return oallan_layout(n, nseries).bytes + 256;   // + 256: the caller's base need not be aligned
 }
 
-// returns 0 on success; mult/ntau: the tau grid (b2ins_allan_num_tau)
+// returns 0 on success; mult/ntau: the tau grid (b2ins_allan_num_tau); hadamard: the Hadamard form of
+// passes 4 and 5 (avar is then hvar)
 inline int oallan_launch(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
                          int64_t outer_stride, int64_t sample_stride, const int64_t* mult, int ntau,
-                         double* avar, double* tau, void* workspace, cudaStream_t st) {
+                         double* avar, double* tau, void* workspace, cudaStream_t st, bool hadamard) {
   OallanParams p;
   std::memset(&p, 0, sizeof(p));
   OallanFinalParams fp;
@@ -437,7 +484,11 @@ inline int oallan_launch(double fs, int64_t n, int64_t nseries, const double* x,
   oallan_tile_kernel<false><<<scan_grid, kOallanScanThreads, 0, st>>>(p);
   oallan_carry_kernel<<<static_cast<unsigned>((nseries + 127) / 128), 128, 0, st>>>(p);
   oallan_tile_kernel<true><<<scan_grid, kOallanScanThreads, 0, st>>>(p);
-  oallan_sq_kernel<<<static_cast<unsigned>(nseries * p.ndec * p.sq_tiles), kOallanSqThreads, 0, st>>>(p);
+  const unsigned sq_grid = static_cast<unsigned>(nseries * p.ndec * p.sq_tiles);
+  if (hadamard)
+    oallan_sq_kernel<true><<<sq_grid, kOallanSqThreads, 0, st>>>(p);
+  else
+    oallan_sq_kernel<false><<<sq_grid, kOallanSqThreads, 0, st>>>(p);
   fp.n = n;
   fp.nseries = nseries;
   fp.sq_tiles = p.sq_tiles;
@@ -449,7 +500,11 @@ inline int oallan_launch(double fs, int64_t n, int64_t nseries, const double* x,
   fp.avar = avar;
   fp.tau = tau;
   const int64_t total = nseries * ntau;
-  oallan_final_kernel<<<static_cast<unsigned>((total + 3) / 4), 128, 0, st>>>(fp);
+  const unsigned final_grid = static_cast<unsigned>((total + 3) / 4);
+  if (hadamard)
+    oallan_final_kernel<true><<<final_grid, 128, 0, st>>>(fp);
+  else
+    oallan_final_kernel<false><<<final_grid, 128, 0, st>>>(fp);
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
 }
 

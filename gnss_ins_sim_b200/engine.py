@@ -496,20 +496,31 @@ def oallan(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
     """K4o: overlapping Allan variance on K4's tau grid, same addressing and outputs as allan():
     avar_o(m) = 1/(2 m^2 M) sum_{k<M} (S(k+m, m) - S(k, m))^2, M = n - 2m + 1.
     Returns avar [nseries, ntau], tau [ntau] (CUDA)."""
+    return _k4o('b2ins_oallan_f64', fs, x, n, nseries, inner, outer_stride, sample_stride)
+
+
+def ohadamard(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
+    """K4o's Hadamard form: overlapping Hadamard variance on K4's tau grid, same addressing and outputs
+    as allan(): hvar(m) = 1/(6 m^2 H) sum_{k<H} (S(k+2m, m) - 2 S(k+m, m) + S(k, m))^2, H = n - 3m + 1.
+    A linear drift of the samples cancels; white noise gives sigma^2 / m, as avar_o does.
+    Returns hvar [nseries, ntau], tau [ntau] (CUDA)."""
+    return _k4o('b2ins_ohadamard_f64', fs, x, n, nseries, inner, outer_stride, sample_stride)
+
+
+def _k4o(symbol, fs, x, n, nseries, inner, outer_stride, sample_stride):
     _require_cuda()
-    lib = _lib.load()
+    fn = getattr(_lib.load(), symbol)
     if outer_stride is None:
         outer_stride = n * sample_stride if inner == 1 else n * inner
     ntau = len(allan_num_tau(n, fs))
-    avar = torch.zeros((nseries, ntau), dtype=torch.float64, device=x.device)
+    var = torch.zeros((nseries, ntau), dtype=torch.float64, device=x.device)
     tau = torch.zeros((ntau,), dtype=torch.float64, device=x.device)
     if ntau == 0 or nseries == 0:
-        return avar, tau
+        return var, tau
     ws = torch.empty(oallan_workspace_bytes(n, nseries) // 8 + 1, dtype=torch.float64, device=x.device)
-    _lib.check(lib.b2ins_oallan_f64(float(fs), int(n), int(nseries), _ptr(x), int(inner),
-                                    int(outer_stride), int(sample_stride), _ptr(avar), _ptr(tau),
-                                    _ptr(ws), _stream()))
-    return avar, tau
+    _lib.check(fn(float(fs), int(n), int(nseries), _ptr(x), int(inner), int(outer_stride), int(sample_stride),
+                  _ptr(var), _ptr(tau), _ptr(ws), _stream()))
+    return var, tau
 
 
 def allan_mc(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0):

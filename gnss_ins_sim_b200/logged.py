@@ -167,6 +167,8 @@ OUTPUT_FORMAT = {
     'att_quat': (['q0', 'q1', 'q2', 'q3'], [''] * 4, [''] * 4),
     'ad_gyro': (['AD_gyro_x', 'AD_gyro_y', 'AD_gyro_z'], ['rad/s'] * 3, ['deg/s'] * 3),
     'ad_accel': (['AD_accel_x', 'AD_accel_y', 'AD_accel_z'], ['m/s^2'] * 3, ['m/s^2'] * 3),
+    'hd_gyro': (['HD_gyro_x', 'HD_gyro_y', 'HD_gyro_z'], ['rad/s'] * 3, ['deg/s'] * 3),
+    'hd_accel': (['HD_accel_x', 'HD_accel_y', 'HD_accel_z'], ['m/s^2'] * 3, ['m/s^2'] * 3),
 }
 
 

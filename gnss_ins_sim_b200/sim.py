@@ -559,8 +559,8 @@ class Sim(object):
                     self._mc[i]['end_err'] = err
                     self.err_stats[name] = engine.error_stats(engine.to_device(err)).cpu().numpy()
             elif isinstance(a, Allan):
-                self._publish_allan(name, *a.run_batch(self.fs[0], self._logged_sets('accel'),
-                                                       self._logged_sets('gyro')))
+                self._publish_allan(name, a, *a.run_batch(self.fs[0], self._logged_sets('accel'),
+                                                          self._logged_sets('gyro')))
             elif isinstance(a, InsLoose):
                 self._run_logged_ins_loose(i, a)
             elif isinstance(a, MagCal):
@@ -798,11 +798,16 @@ class Sim(object):
             free_b = 2 ** 31
         return max(1, min(max(hi - lo, 1), int(free_b / share // (n * bytes_per_sample)) or 1))
 
-    def _publish_allan(self, name, tau, ad_accel, ad_gyro):
-        """algo_time (the same tau for every run), ad_accel, ad_gyro [R, ntau, 3] under run keys."""
-        self.data['algo_time'] = _keyed(name, [tau] * len(ad_accel))
-        self.data['ad_accel'] = _keyed(name, ad_accel)
-        self.data['ad_gyro'] = _keyed(name, ad_gyro)
+    def _publish_allan(self, name, algo, tau, accel, gyro):
+        """algo_time (the same tau for every run) and the plugin's accel and gyro outputs [R, ntau, 3] (ad_* for
+        Allan, hd_* for Hadamard) under run keys.  Allan and Hadamard plugins of one Sim share algo_time: each
+        replaces its own run keys in it and keeps the others'."""
+        t, o_accel, o_gyro = algo.output
+        prev = self.data.get(t)
+        keep = {k: v for k, v in prev.items() if not k.startswith(name + '_')} if isinstance(prev, dict) else {}
+        self.data[t] = dict(keep, **_keyed(name, [tau] * len(accel)))
+        self.data[o_accel] = _keyed(name, accel)
+        self.data[o_gyro] = _keyed(name, gyro)
 
     def _run_allan(self, i, algo):
         """The Allan deviations of this rank's shard of the runs, in run blocks sized to the free device
@@ -810,8 +815,8 @@ class Sim(object):
         model and with series longer than one chunk, K1 is fused into K4's first level (engine.allan_mc) and
         the only device memory is the decade-sum workspace (about 2 B per run-sample), so run blocks are
         rarely needed; otherwise K1 materialises the series (48 B per run-sample) for K4 (~2 B of workspace).
-        Allan(overlapping=True) always materialises: K4o needs its prefix workspace (about 48 B per run-sample
-        for the three series of one sensor) beside the series."""
+        Allan(overlapping=True) and Hadamard() always materialise: K4o needs its prefix workspace (about 48 B per
+        run-sample for the three series of one sensor) beside the series."""
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
         overlapping = getattr(algo, 'overlapping', False)
@@ -841,7 +846,7 @@ class Sim(object):
         if dist.world() > 1:
             both = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(both.reshape(hi - lo, -1))),
                                     self.sim_count).reshape(self.sim_count, len(tau), 6)
-        self._publish_allan(self.algo_name(i), tau, both[:, :, 0:3], both[:, :, 3:6])
+        self._publish_allan(self.algo_name(i), algo, tau, both[:, :, 0:3], both[:, :, 3:6])
 
     # ---- magnetometer calibration (K10) ---------------------------------------------------------
     def _publish_magcal(self, name, soft_iron, hard_iron):

@@ -447,6 +447,21 @@ int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x
                           int64_t inner, int64_t outer_stride, int64_t sample_stride,
                           double* avar, double* tau);
 
+/* ---- K4o, Hadamard form: overlapping Hadamard variance -------------------------
+ * hvar(m) = 1 / (6 m^2 H) sum_{k<H} (S(k+2m, m) - 2 S(k+m, m) + S(k, m))^2, H = n - 3m + 1
+ * (NIST SP 1065), on the same cluster sizes and tau as b2ins_oallan_f64: a second difference of
+ * adjacent window sums, so a linear drift of the samples cancels, and white noise gives sigma^2 / m.
+ * Signature, series addressing, outputs and workspace (b2ins_oallan_workspace_bytes) as
+ * b2ins_oallan_f64.  A series with a NaN sample gives NaN at every tau; one with +-inf samples gives
+ * what the definitional sum gives in IEEE arithmetic: NaN where a term's contributions +S(k+2m),
+ * -2 S(k+m), +S(k) hold both infinities, else +inf.  Deterministic: bit-identical whatever the batch. */
+int b2ins_ohadamard_f64(double fs, int64_t n, int64_t nseries, const double* x,
+                        int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                        double* hvar, double* tau, void* workspace, void* stream);
+int b2ins_ohadamard_f64_host(double fs, int64_t n, int64_t nseries, const double* x,
+                             int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                             double* hvar, double* tau);
+
 /* ---- K5: vibration series from a PSD -------------------------------------------
  * Replaces time_series_from_psd (gnss_ins_sim/psd/time_series_from_psd.py:17-65) as called
  * three times per sensor and run by acc_gen / gyro_gen (pathgen.py:478-485, :541-548).
