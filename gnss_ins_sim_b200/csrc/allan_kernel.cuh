@@ -499,7 +499,7 @@ allan_gen_kernel(const __grid_constant__ AllanLevelParams p, const __grid_consta
   double* in_buf = smem;                                   // [2][kAllanRawLen]
   double* pad_buf = smem + 2 * kAllanRawLen;               // [2][kAllanPadLen]
   __shared__ double red[2][kAllanFastWarps][4];
-  __shared__ double wtot[kAllanFastWarps][2];              // (A, E) of every warp's stretch of the tile
+  __shared__ double wtot[1][kAllanFastWarps][2];           // (A, E) of every warp's stretch of the tile
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cc = static_cast<int>(p.chunk_count);
   int it = 0;
@@ -517,7 +517,7 @@ allan_gen_kernel(const __grid_constant__ AllanLevelParams p, const __grid_consta
     apow[0] = 1.0;
 #pragma unroll
     for (int q = 1; q <= kGenPer; ++q) apow[q] = apow[q - 1] * a;
-    double carry = 0.0;                                    // d at the first sample of the tile; d[0] = 0
+    double carry[1] = {0.0};                               // d at the first sample of the tile; d[0] = 0
     for (int chunk = 0; chunk < cc; ++chunk, ++it) {
       double* in = in_buf + (it & 1) * kAllanRawLen;
       const int64_t c0 = static_cast<int64_t>(chunk) * kAllanChunk;
@@ -544,51 +544,17 @@ allan_gen_kernel(const __grid_constant__ AllanLevelParams p, const __grid_consta
         }
         E = r;
       }
-      // ---- affine scan over the threads: (A, E) o (A', E') = (A A', A' E + E') -------------------
-      double sA = A, sE = E;                               // inclusive within the warp
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const double uA = __shfl_up_sync(0xffffffffu, sA, off);
-        const double uE = __shfl_up_sync(0xffffffffu, sE, off);
-        if (lane >= off) {
-          sE = fma(sA, uE, sE);
-          sA *= uA;
-        }
-      }
-      if (lane == 31) {
-        wtot[warp][0] = sA;
-        wtot[warp][1] = sE;
-      }
+      // ---- affine scan over the threads (K1's, common.cuh) --------------------------------------
+      double sA[1] = {A}, sE[1] = {E};
+      affine_scan_warp<1, kAllanFastWarps>(sA, sE, wtot, lane, warp);
       __syncthreads();                                     // (1) warp totals; everybody is done with tile it-1
       if (it > 0 && tid < 9) allan_tile_fold(p, prev_series, prev_chunk, red[(it - 1) & 1]);
-      // exclusive prefix of this thread: the warps before it, then the lanes before it
-      double pA = 1.0, pE = 0.0;
-      for (int w = 0; w < warp; ++w) {
-        pE = fma(wtot[w][0], pE, wtot[w][1]);
-        pA *= wtot[w][0];
-      }
-      {
-        const double lA = __shfl_up_sync(0xffffffffu, sA, 1), lE = __shfl_up_sync(0xffffffffu, sE, 1);
-        if (lane > 0) {
-          pE = fma(lA, pE, lE);
-          pA *= lA;
-        }
-      }
-      const double S = fma(pA, carry, pE);                 // drift at the first sample of the stretch
-      // the tile's total, by every thread alike (same operations, same result): the next carry
-      {
-        double tA = 1.0, tE = 0.0;
-#pragma unroll
-        for (int w = 0; w < kAllanFastWarps; ++w) {
-          tE = fma(wtot[w][0], tE, wtot[w][1]);
-          tA *= wtot[w][0];
-        }
-        carry = fma(tA, carry, tE);
-      }
+      double S[1];                                         // drift at the first sample of the stretch
+      affine_scan_block<1, kAllanFastWarps>(sA, sE, wtot, lane, warp, carry, S);
       if (tid < kGenThreads) {
 #pragma unroll
         for (int q = 0; q < kGenPer; ++q)
-          in[kAllanLead + tid * kGenPer + q] = mm[q] + fma(apow[q], S, rr[q]);
+          in[kAllanLead + tid * kGenPer + q] = mm[q] + fma(apow[q], S[0], rr[q]);
       }
       // halo: the nine samples before the chunk are the tail of the previous tile of this series
       if (chunk != 0 && tid >= kAllanFastThreads - 9) {

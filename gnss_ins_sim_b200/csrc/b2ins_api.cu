@@ -246,12 +246,29 @@ struct Stream {
   cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
 };
 
+// stream-ordered scratch: freed after the work queued on s before it, on every exit path; free() does it early
+// and returns the error
+struct AsyncBuf {
+  cudaStream_t s;
+  double* p = nullptr;
+  explicit AsyncBuf(cudaStream_t st) : s(st) {}
+  ~AsyncBuf() {
+    if (p) cudaFreeAsync(p, s);
+  }
+  cudaError_t alloc(size_t bytes) { return cudaMallocAsync(&p, bytes, s); }
+  cudaError_t free() {
+    double* q = p;
+    p = nullptr;
+    return q ? cudaFreeAsync(q, s) : cudaSuccess;
+  }
+};
+
 // K1's parameters and time segmentation, shared by K1 and K9; with segments, pass 1 and the carry chain are
-// launched here and *scratch holds their buffers (freed by the caller after its pass-0 launch).
+// launched here and *scratch holds their buffers until the caller has queued pass 0 on s.
 int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
                   const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
                   const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, cudaStream_t s, NoiseParams* out,
-                  double** out_scratch) {
+                  AsyncBuf* scratch) {
   NoiseParams& p = *out;
   std::memset(&p, 0, sizeof(p));
   p.n = n;
@@ -284,16 +301,14 @@ int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, co
   p.pass = 0;
   p.seg_carry = nullptr;
   p.seg_end = nullptr;
-  double* scratch = nullptr;
   if (nseg > 1) {
     int64_t len = (n + nseg - 1) / nseg;
     len = (len + kNoiseTile - 1) / kNoiseTile * kNoiseTile;   // whole tiles per segment
     p.seg_len = len;
     p.nseg = static_cast<int>((n + len - 1) / len);
-    CU_CHECK(cudaMallocAsync(&scratch, sizeof(double) * runs * p.nseg * 12, s));
-    *out_scratch = scratch;        // the caller frees it, also when a launch below fails
-    p.seg_end = scratch;
-    p.seg_carry = scratch + runs * p.nseg * 6;
+    CU_CHECK(scratch->alloc(sizeof(double) * runs * p.nseg * 12));
+    p.seg_end = scratch->p;
+    p.seg_carry = scratch->p + runs * p.nseg * 6;
     // pass 1 only needs the drives that still matter at the segment end: a^L < 1e-20
     int64_t keep = 1;
     for (int c = 0; c < 6; ++c) {
@@ -478,19 +493,16 @@ int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n, const double* ref_gy
   ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
   NoiseParams p;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  double* scratch = nullptr;
-  int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset,
-                         s, &p, &scratch);
-  if (rc != B2INS_OK) {
-    if (scratch) cudaFreeAsync(scratch, s);
-    return rc;
-  }
+  AsyncBuf scratch(s);
+  const int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed,
+                               run_offset, s, &p, &scratch);
+  if (rc != B2INS_OK) return rc;
   p.out_gyro = gyro;
   p.out_accel = accel;
   layout_strides(layout, runs, n, &p.osr, &p.ost, &p.osc);
   p.z_dump = z_dump;
   imu_noise_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p);
-  if (scratch) CU_CHECK(cudaFreeAsync(scratch, s));
+  CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
@@ -510,31 +522,25 @@ int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* re
   ErrStatsParams P;
   std::memset(&P, 0, sizeof(P));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  double* scratch = nullptr;
-  int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset,
-                         s, &P.np, &scratch);
-  if (rc != B2INS_OK) {
-    if (scratch) cudaFreeAsync(scratch, s);
-    return rc;
-  }
+  AsyncBuf scratch(s), partial(s);
+  const int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed,
+                               run_offset, s, &P.np, &scratch);
+  if (rc != B2INS_OK) return rc;
   P.stats_start = stats_start;
   P.end_err = end_err;
   P.proc_stats = proc_stats;
-  double* partial = nullptr;
   if (P.np.nseg > 1 && stats_start >= 0) {
-    const cudaError_t e = cudaMallocAsync(&partial, sizeof(double) * runs * P.np.nseg * kErrPartial, s);
-    if (e != cudaSuccess) {
-      if (scratch) cudaFreeAsync(scratch, s);
+    const cudaError_t e = partial.alloc(sizeof(double) * runs * P.np.nseg * kErrPartial);
+    if (e != cudaSuccess)
       return fail(B2INS_ERR_CUDA, "cudaMallocAsync of the segment partials: %s", cudaGetErrorString(e));
-    }
-    P.partial = partial;
+    P.partial = partial.p;
   }
   imu_err_stats_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P);
-  if (partial) {
+  if (partial.p) {
     err_stats_fold_kernel<<<static_cast<unsigned>((runs * kErrCh + 127) / 128), 128, 0, s>>>(P);
-    CU_CHECK(cudaFreeAsync(partial, s));
+    CU_CHECK(partial.free());
   }
-  if (scratch) CU_CHECK(cudaFreeAsync(scratch, s));
+  CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }

@@ -177,4 +177,62 @@ __device__ __forceinline__ double shfl_grp(double v, int src) {
   return __shfl_sync(0xffffffffu, v, src, W);
 }
 
+// ---- block-wide affine scan of a Gauss-Markov recurrence, C channels, W warps ----
+// Thread i holds the map x -> sA x + sE of its stretch of samples; the stretches compose in thread order
+// by (A, E) o (A', E') = (A A', A' E + E').  Two halves around the caller's __syncthreads:
+// warp half: the inclusive scan within the warp, and lane 31 leaves the warp's total in wtot[C][W][2].
+template <int C, int W>
+__device__ __forceinline__ void affine_scan_warp(double (&sA)[C], double (&sE)[C], double (*wtot)[W][2], int lane,
+                                                 int warp) {
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      const double uA = __shfl_up_sync(0xffffffffu, sA[c], off);
+      const double uE = __shfl_up_sync(0xffffffffu, sE[c], off);
+      if (lane >= off) {
+        sE[c] = fma(sA[c], uE, sE[c]);
+        sA[c] *= uA;
+      }
+    }
+  }
+  if (lane == 31) {
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      wtot[c][warp][0] = sA[c];
+      wtot[c][warp][1] = sE[c];
+    }
+  }
+}
+
+// block half, after the barrier: S = the state at this thread's first sample (the warps before it, then the
+// lanes before it, applied to carry, the state at the block's first sample), and carry advanced over the whole
+// block -- by every thread alike, so every thread holds the same next carry
+template <int C, int W>
+__device__ __forceinline__ void affine_scan_block(const double (&sA)[C], const double (&sE)[C],
+                                                  const double (*wtot)[W][2], int lane, int warp, double (&carry)[C],
+                                                  double (&S)[C]) {
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    double pA = 1.0, pE = 0.0;
+    for (int w = 0; w < warp; ++w) {
+      pE = fma(wtot[c][w][0], pE, wtot[c][w][1]);
+      pA *= wtot[c][w][0];
+    }
+    const double lA = __shfl_up_sync(0xffffffffu, sA[c], 1), lE = __shfl_up_sync(0xffffffffu, sE[c], 1);
+    if (lane > 0) {
+      pE = fma(lA, pE, lE);
+      pA *= lA;
+    }
+    S[c] = fma(pA, carry[c], pE);
+    double tA = 1.0, tE = 0.0;
+#pragma unroll
+    for (int w = 0; w < W; ++w) {
+      tE = fma(wtot[c][w][0], tE, wtot[c][w][1]);
+      tA *= wtot[c][w][0];
+    }
+    carry[c] = fma(tA, carry[c], tE);
+  }
+}
+
 }  // namespace b2ins

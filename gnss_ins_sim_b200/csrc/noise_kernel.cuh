@@ -7,8 +7,10 @@
 // an affine scan over the 128 threads of a tile -- shuffles within a warp, four warp totals through
 // shared memory: ONE exchange per kNoisePer samples instead of one per sample -- after which every
 // thread adds a^q S to its samples and the tile leaves shared memory in the caller's layout with
-// coalesced stores.  imu_err_stats_kernel (K9, sensor_stats_kernel.cuh) repeats this kernel's tile loop
-// (generation, affine scan, carry) with the store replaced by a reduction: a change here goes there too.
+// coalesced stores.  imu_err_stats_kernel (K9, sensor_stats_kernel.cuh) reduces the tile instead of
+// storing it; it calls noise_prologue and the scan of common.cuh, and repeats only the stretch loop
+// (triad_sample into the stage): with that loop in a shared function the compiler allocates K9's
+// registers differently, so a change to the loop here goes there too.
 #pragma once
 #include "mc_kernel.cuh"
 
@@ -67,6 +69,36 @@ __device__ __forceinline__ void triad_sample(const NoiseParams& p, const TriadNo
   }
 }
 
+// the prologue of a K1 or K9 CTA, before its first __syncthreads: a^q per channel into apow[kNoisePer + 1][6],
+// the run's sinusoidal gyro-vibration phase and, with carry_in, the Gauss-Markov state at the segment start
+// (zero without)
+__device__ __forceinline__ void noise_prologue(const NoiseParams& p, double (*apow)[6], int64_t run, int seg,
+                                               uint32_t run_lo, uint32_t run_hi, bool carry_in, double (&phase)[3],
+                                               double (&carry)[6]) {
+  const int tid = threadIdx.x;
+  if (tid < 6) {
+    const double a = (tid < 3) ? p.accel.gm_a[tid] : p.gyro.gm_a[tid - 3];
+    double v = 1.0;
+    for (int q = 0; q <= kNoisePer; ++q) {
+      apow[q][tid] = v;
+      v *= a;
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) phase[c] = 0.0;
+  if (p.gyro.vib_type == 2) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
+  }
+#pragma unroll
+  for (int c = 0; c < 6; ++c) carry[c] = 0.0;
+  if (carry_in && p.seg_carry) {
+#pragma unroll
+    for (int c = 0; c < 6; ++c) carry[c] = p.seg_carry[(run * p.nseg + seg) * 6 + c];
+  }
+}
+
 __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __grid_constant__ NoiseParams p) {
   __shared__ double stage[2][kNoiseTile * 3];     // accel, gyro of the tile, [sample][axis]
   __shared__ double wtot[6][kNoiseWarps][2];      // (A, E) of every warp's stretch, per channel
@@ -79,25 +111,8 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __gri
   const int64_t grun = p.run_offset + run;
   const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid < 6) {
-    const double a = (tid < 3) ? p.accel.gm_a[tid] : p.gyro.gm_a[tid - 3];
-    double v = 1.0;
-    for (int q = 0; q <= kNoisePer; ++q) {
-      apow[q][tid] = v;
-      v *= a;
-    }
-  }
-  double phase[3] = {0.0, 0.0, 0.0};
-  if (p.gyro.vib_type == 2) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
-  }
-  double carry[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // d at the first sample of the tile
-  if (p.pass == 0 && p.seg_carry) {
-#pragma unroll
-    for (int c = 0; c < 6; ++c) carry[c] = p.seg_carry[(run * p.nseg + seg) * 6 + c];
-  }
+  double phase[3], carry[6];                      // carry: d at the first sample of the tile
+  noise_prologue(p, apow, run, seg, run_lo, run_hi, p.pass == 0, phase, carry);
   __syncthreads();
 
   for (int64_t tile0 = seg_lo; tile0 < seg_hi; tile0 += kNoiseTile) {
@@ -127,48 +142,10 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __gri
       sA[c] = apow[mine][c];
       sE[c] = r[c];
     }
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        const double uA = __shfl_up_sync(0xffffffffu, sA[c], off);
-        const double uE = __shfl_up_sync(0xffffffffu, sE[c], off);
-        if (lane >= off) {
-          sE[c] = fma(sA[c], uE, sE[c]);
-          sA[c] *= uA;
-        }
-      }
-    }
-    if (lane == 31) {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        wtot[c][warp][0] = sA[c];
-        wtot[c][warp][1] = sE[c];
-      }
-    }
+    affine_scan_warp<6, kNoiseWarps>(sA, sE, wtot, lane, warp);
     __syncthreads();   // warp totals; the staged tile is complete
     double S[6];       // drift at the first sample of this thread's stretch
-#pragma unroll
-    for (int c = 0; c < 6; ++c) {
-      double pA = 1.0, pE = 0.0;
-      for (int w = 0; w < warp; ++w) {
-        pE = fma(wtot[c][w][0], pE, wtot[c][w][1]);
-        pA *= wtot[c][w][0];
-      }
-      const double lA = __shfl_up_sync(0xffffffffu, sA[c], 1), lE = __shfl_up_sync(0xffffffffu, sE[c], 1);
-      if (lane > 0) {
-        pE = fma(lA, pE, lE);
-        pA *= lA;
-      }
-      S[c] = fma(pA, carry[c], pE);
-      double tA = 1.0, tE = 0.0;       // the tile's total, by every thread alike: the next carry
-#pragma unroll
-      for (int w = 0; w < kNoiseWarps; ++w) {
-        tE = fma(wtot[c][w][0], tE, wtot[c][w][1]);
-        tA *= wtot[c][w][0];
-      }
-      carry[c] = fma(tA, carry[c], tE);
-    }
+    affine_scan_block<6, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
     if (p.pass == 0) {
       // ---- + a^q S on the thread's own samples, then the tile leaves in the caller's layout -------
 #pragma unroll 1

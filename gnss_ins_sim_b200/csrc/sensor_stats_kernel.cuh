@@ -4,9 +4,10 @@
 // e = meas - ref, its value at the last sample, and over the samples from a start index max|e|, mean
 // and std (ddof 0).
 //
-// K9 has K1's launch shape and generator (noise_kernel.cuh: one CTA per (run, time segment), 896-sample
-// tiles, triad_sample, the affine Gauss-Markov scan over the threads; the segmented form's pass 1 and
-// noise_carry_kernel are K1's own).  The finished tile is reduced instead of stored: nothing of the
+// K9 has K1's launch shape (one CTA per (run, time segment), 896-sample tiles; the segmented form's pass 1
+// and noise_carry_kernel are K1's own) and calls K1's generator: noise_prologue, triad_sample and the
+// affine Gauss-Markov scan over the threads (common.cuh).  The stretch loop around triad_sample is K1's,
+// repeated (noise_kernel.cuh says why).  The finished tile is reduced instead of stored: nothing of the
 // series leaves the SM.
 //
 // Determinism: every reduction runs in a fixed order, with no floating-point atomics.  A thread reduces
@@ -72,25 +73,8 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
   const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool want_stats = P.stats_start >= 0;
-  if (tid < 6) {
-    const double a = (tid < 3) ? p.accel.gm_a[tid] : p.gyro.gm_a[tid - 3];
-    double v = 1.0;
-    for (int q = 0; q <= kNoisePer; ++q) {
-      apow[q][tid] = v;
-      v *= a;
-    }
-  }
-  double phase[3] = {0.0, 0.0, 0.0};
-  if (p.gyro.vib_type == 2) {
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
-  }
-  double carry[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-  if (p.seg_carry) {
-#pragma unroll
-    for (int c = 0; c < 6; ++c) carry[c] = p.seg_carry[(run * p.nseg + seg) * 6 + c];
-  }
+  double phase[3], carry[6];
+  noise_prologue(p, apow, run, seg, run_lo, run_hi, true, phase, carry);
   double an = 0.0, am[6], a2[6], ax[6];           // the thread's running statistics
 #pragma unroll
   for (int c = 0; c < 6; ++c) am[c] = a2[c] = ax[c] = 0.0;
@@ -122,48 +106,10 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
       sA[c] = apow[mine][c];
       sE[c] = r[c];
     }
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        const double uA = __shfl_up_sync(0xffffffffu, sA[c], off);
-        const double uE = __shfl_up_sync(0xffffffffu, sE[c], off);
-        if (lane >= off) {
-          sE[c] = fma(sA[c], uE, sE[c]);
-          sA[c] *= uA;
-        }
-      }
-    }
-    if (lane == 31) {
-#pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        wtot[c][warp][0] = sA[c];
-        wtot[c][warp][1] = sE[c];
-      }
-    }
+    affine_scan_warp<6, kNoiseWarps>(sA, sE, wtot, lane, warp);
     __syncthreads();
     double S[6];
-#pragma unroll
-    for (int c = 0; c < 6; ++c) {
-      double pA = 1.0, pE = 0.0;
-      for (int w = 0; w < warp; ++w) {
-        pE = fma(wtot[c][w][0], pE, wtot[c][w][1]);
-        pA *= wtot[c][w][0];
-      }
-      const double lA = __shfl_up_sync(0xffffffffu, sA[c], 1), lE = __shfl_up_sync(0xffffffffu, sE[c], 1);
-      if (lane > 0) {
-        pE = fma(lA, pE, lE);
-        pA *= lA;
-      }
-      S[c] = fma(pA, carry[c], pE);
-      double tA = 1.0, tE = 0.0;
-#pragma unroll
-      for (int w = 0; w < kNoiseWarps; ++w) {
-        tE = fma(wtot[c][w][0], tE, wtot[c][w][1]);
-        tA *= wtot[c][w][0];
-      }
-      carry[c] = fma(tA, carry[c], tE);
-    }
+    affine_scan_block<6, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
     // ---- the thread's own samples: the measurement exactly as K1 stores it, minus the truth --------
     // pass A: e (kept in the stage), the end-point error, sum and max over the samples >= stats_start
     const int64_t t_lo = tile0 + tid * kNoisePer;

@@ -179,6 +179,34 @@ def test_k9_psd_vibration_equals_k1(eng):
         assert_close(proc[:, k], v, 1e-12, 1e-9, 'psd stat %d' % k)
 
 
+@pytest.mark.parametrize('vib', ['none', 'random', 'sinusoidal', 'psd'])
+def test_k9_end_err_is_k1_sample_bit_for_bit(eng, vib):
+    """Unsegmented path: K9's end points are K1's last stored samples minus the truth, bit for bit, with every
+    vibration type and a white-drift channel (b_corr = inf) next to Gauss-Markov ones."""
+    R_, n = 5, 2000
+    gerr = dict(MID_G, b_corr=np.array([100.0, np.inf, 50.0]))
+    aerr = dict(MID_A, b_corr=np.array([np.inf, 200.0, 100.0]))
+    vg = va = None
+    if vib == 'random':
+        va = {'type': 'random', 'x': 0.1, 'y': 0.2, 'z': 0.3}
+        vg = {'type': 'random', 'x': 0.01, 'y': 0.02, 'z': 0.03}
+    elif vib == 'sinusoidal':
+        va = {'type': 'sinusoidal', 'x': 0.1, 'y': 0.2, 'z': 0.3, 'freq': 3.0}
+        vg = {'type': 'sinusoidal', 'x': 0.01, 'y': 0.02, 'z': 0.03, 'freq': 2.0}
+    elif vib == 'psd':
+        tab = np.linspace(0.0, 50.0, 60)
+        v = {'type': 'psd', 'freq': tab, 'x': np.full(60, 1e-3), 'y': np.full(60, 2e-3), 'z': np.full(60, 5e-4)}
+        va = eng.vib_series(*eng.psd_series(100.0, n, R_, 0, v, 3, run_offset=2))
+        vg = eng.vib_series(*eng.psd_series(100.0, n, R_, 1, v, 3, run_offset=2))
+    rng = np.random.default_rng(11)
+    rg = eng.to_device(rng.standard_normal((n, 3)) * 0.3)
+    ra = eng.to_device(rng.standard_normal((n, 3)) * 3.0)
+    end, _ = eng.imu_err_stats(100.0, R_, rg, ra, gerr, aerr, 3, run_offset=2, vib_gyro=vg, vib_accel=va)
+    gyro, accel = eng.imu_noise(100.0, R_, rg, ra, gerr, aerr, 3, run_offset=2, vib_gyro=vg, vib_accel=va)
+    e = torch.cat([accel[:, -1] - ra[-1], gyro[:, -1] - rg[-1]], dim=1).cpu().numpy()
+    assert np.array_equal(end.cpu().numpy(), e)
+
+
 def test_k3p_matches_numpy(eng):
     rng = np.random.default_rng(4)
     for R_, m, C, start in ((1, 1, 1, 0), (7, 1000, 3, 0), (5, 777, 6, 300), (300, 101, 8, 100)):
