@@ -124,6 +124,7 @@ SIGNATURES = {
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),
     'b2ins_diag_psd_plan': (_I, [_L, ctypes.POINTER(ctypes.c_int)]),
+    'b2ins_diag_noise_plan': (_I, [_D, _L, _L, _SE, _SE, _I, c_double_p, c_int64_p]),
     'b2ins_diag_fastmath_f64': (_I, [_I, _L, _P, _P, _P, _P]),
     'b2ins_diag_philox': (_I, [_L, _P, _P]),
     'b2ins_diag_normal_from_words': (_I, [_L, _P, _P]),
@@ -188,6 +189,20 @@ def psd_plan(n):
     if rc < 0:
         raise ValueError('b2ins: ' + load().b2ins_last_error().decode('utf-8', 'replace'))
     return PSD_PLANS[rc], P.value
+
+
+def noise_plan(fs, runs, n, gyro_err, accel_err, sm_count=0):
+    """K1's (and K9's) digested Gauss-Markov coefficients and time segmentation for `runs` runs of n samples
+    on sm_count SMs (0: the current device): {'gm_a', 'gm_b', 'wd': [6] (accel xyz, gyro xyz), 'nseg',
+    'seg_len', 'pass1_len'}.  gyro_err / accel_err: imu_model dicts, as engine.imu_noise takes them."""
+    ge, ae = sensor_err(gyro_err, 'arw'), sensor_err(accel_err, 'vrw')
+    coef = np.zeros(18)
+    plan = np.zeros(3, dtype=np.int64)
+    check(load().b2ins_diag_noise_plan(float(fs), int(runs), int(n), ctypes.byref(ge), ctypes.byref(ae),
+                                        int(sm_count), coef.ctypes.data_as(c_double_p),
+                                        plan.ctypes.data_as(c_int64_p)))
+    return {'gm_a': coef[0:6], 'gm_b': coef[6:12], 'wd': coef[12:18], 'nseg': int(plan[0]),
+            'seg_len': int(plan[1]), 'pass1_len': int(plan[2])}
 
 
 def check(rc):

@@ -263,6 +263,47 @@ struct AsyncBuf {
   }
 };
 
+// K1's time segmentation on `sms` SMs: p.nseg, p.seg_len and p.pass1_len (0 without segments) from n, runs and
+// the digested decay factors.  Few runs and a long series (the Allan configuration): split the time axis into
+// segments so that every SM has work.  The Gauss-Markov state at a segment start needs the draws before it:
+// pass 1 reduces every segment to its zero-state end value, a tiny serial kernel chains them, pass 0
+// regenerates (counter-based Philox: nothing is stored) and writes.  Costs the noise twice, so it is only used
+// when one CTA per run would leave most of the GPU idle.
+void noise_plan(NoiseParams* out, int sms) {
+  NoiseParams& p = *out;
+  int nseg = 1;
+  const int64_t want_ctas = static_cast<int64_t>(sms) * 2;
+  if (p.runs < want_ctas && p.n >= (int64_t(1) << 18)) {
+    nseg = static_cast<int>((want_ctas + p.runs - 1) / p.runs);
+    const int64_t max_seg = p.n / (int64_t(1) << 16);
+    if (nseg > max_seg) nseg = static_cast<int>(max_seg);
+    if (nseg < 1) nseg = 1;
+  }
+  p.nseg = nseg;
+  p.seg_len = p.n;
+  p.pass1_len = 0;
+  if (nseg == 1) return;
+  int64_t len = (p.n + nseg - 1) / nseg;
+  len = (len + kNoiseTile - 1) / kNoiseTile * kNoiseTile;   // whole tiles per segment
+  p.seg_len = len;
+  p.nseg = static_cast<int>((p.n + len - 1) / len);
+  // pass 1 only needs the drives that still matter at the segment end: |a|^L < 1e-20.  The rule is on |a|:
+  // tau < dt gives a <= 0 (-1 at tau = dt / 2), whose drives decay as |a|^k; a = 0 keeps
+  // none; |a| >= 1 never decays and needs the whole segment.
+  int64_t keep = 1;
+  for (int c = 0; c < 6; ++c) {
+    const double a = std::fabs((c < 3) ? p.accel.gm_a[c] : p.gyro.gm_a[c - 3]);
+    if (a >= 1.0) {
+      keep = len;
+    } else if (a > 0.0) {
+      const double need = std::ceil(std::log(1e-20) / std::log(a));
+      if (need > static_cast<double>(keep)) keep = need >= static_cast<double>(len) ? len : static_cast<int64_t>(need);
+    }
+  }
+  keep = (keep + kNoiseTile - 1) / kNoiseTile * kNoiseTile;
+  p.pass1_len = keep < len ? keep : len;
+}
+
 // K1's parameters and time segmentation, shared by K1 and K9; with segments, pass 1 and the carry chain are
 // launched here and *scratch holds their buffers until the caller has queued pass 0 on s.
 int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
@@ -283,48 +324,16 @@ int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, co
   if (rc != B2INS_OK) return rc;
   p.ref_gyro = ref_gyro;
   p.ref_accel = ref_accel;
-  // Few runs and a long series (the Allan configuration): split the time axis into segments so
-  // that every SM has work.  The Gauss-Markov state at a segment start needs the draws before it:
-  // pass 1 reduces every segment to its zero-state end value, a tiny serial kernel chains them,
-  // pass 0 regenerates (counter-based Philox: nothing is stored) and writes.  Costs the noise
-  // twice, so it is only used when one CTA per run would leave most of the GPU idle.
-  int nseg = 1;
-  const int64_t want_ctas = static_cast<int64_t>(sm_count()) * 2;
-  if (runs < want_ctas && n >= (int64_t(1) << 18)) {
-    nseg = static_cast<int>((want_ctas + runs - 1) / runs);
-    const int64_t max_seg = n / (int64_t(1) << 16);
-    if (nseg > max_seg) nseg = static_cast<int>(max_seg);
-    if (nseg < 1) nseg = 1;
-  }
-  p.nseg = nseg;
-  p.seg_len = n;
+  noise_plan(&p, sm_count());
   p.pass = 0;
   p.seg_carry = nullptr;
   p.seg_end = nullptr;
-  if (nseg > 1) {
-    int64_t len = (n + nseg - 1) / nseg;
-    len = (len + kNoiseTile - 1) / kNoiseTile * kNoiseTile;   // whole tiles per segment
-    p.seg_len = len;
-    p.nseg = static_cast<int>((n + len - 1) / len);
+  if (p.nseg > 1) {
     CU_CHECK(scratch->alloc(sizeof(double) * runs * p.nseg * 12));
     p.seg_end = scratch->p;
     p.seg_carry = scratch->p + runs * p.nseg * 6;
-    // pass 1 only needs the drives that still matter at the segment end: a^L < 1e-20
-    int64_t keep = 1;
-    for (int c = 0; c < 6; ++c) {
-      const double a = (c < 3) ? p.accel.gm_a[c] : p.gyro.gm_a[c - 3];
-      if (a >= 1.0) {
-        keep = len;
-      } else if (a > 0.0) {
-        const double need = std::ceil(std::log(1e-20) / std::log(a));
-        if (need > static_cast<double>(keep)) keep = need >= static_cast<double>(len) ? len : static_cast<int64_t>(need);
-      }
-    }
-    keep = (keep + kNoiseTile - 1) / kNoiseTile * kNoiseTile;
-    p.pass1_len = keep < len ? keep : len;
     p.pass = 1;
-    if (p.nseg > 1)
-      imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
+    imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
     noise_carry_kernel<<<static_cast<unsigned>((runs * 6 + 127) / 128), 128, 0, s>>>(p);
     p.pass = 0;
   }
@@ -1533,6 +1542,33 @@ int b2ins_diag_psd_plan(int64_t n, int* P) {
   const int len = psd_direct_forced() ? 0 : psd_fft_plan(psd_series_len(n), &bluestein);
   *P = len;
   return len == 0 ? 0 : (bluestein ? 2 : 1);
+}
+
+// ---------------------------------------------------------------- K1 plan ---
+int b2ins_diag_noise_plan(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
+                          const b2ins_sensor_err* accel_err, int sm_count_arg, double* coef, int64_t* plan) {
+  ARG_CHECK(fs > 0.0, "fs must be positive");
+  ARG_CHECK(runs > 0 && n > 0, "runs and n must be positive");
+  ARG_CHECK(gyro_err && accel_err && coef && plan, "null buffer");
+  NoiseParams p;
+  std::memset(&p, 0, sizeof(p));
+  p.n = n;
+  p.runs = runs;
+  int rc = digest_triad(gyro_err, nullptr, fs, &p.gyro);
+  if (rc != B2INS_OK) return rc;
+  rc = digest_triad(accel_err, nullptr, fs, &p.accel);
+  if (rc != B2INS_OK) return rc;
+  noise_plan(&p, sm_count_arg > 0 ? sm_count_arg : sm_count());
+  for (int c = 0; c < 6; ++c) {
+    const TriadNoise& e = (c < 3) ? p.accel : p.gyro;
+    coef[c] = e.gm_a[c % 3];
+    coef[6 + c] = e.gm_b[c % 3];
+    coef[12 + c] = e.wd[c % 3];
+  }
+  plan[0] = p.nseg;
+  plan[1] = p.seg_len;
+  plan[2] = p.pass1_len;
+  return B2INS_OK;
 }
 
 int64_t b2ins_psd_workspace_bytes(int64_t n, int64_t runs) {

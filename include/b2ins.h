@@ -301,7 +301,13 @@ int b2ins_free_integration_odo_f64(int ref_frame, double fs, int64_t runs, int64
  * (seed, run_offset + r).  ref_gyro / ref_accel: [n][3] shared true IMU output.
  * gyro / accel: outputs in `layout`.  z_dump (nullable): the 12 normals per (run, t) as
  * [R][n][12] = (acc_gm[3], acc_w[3], gyr_gm[3], gyr_w[3]) for injection into the
- * reference's np.random.randn call sequence. */
+ * reference's np.random.randn call sequence.
+ * A correlation time below dt / 2 gives a decay factor |a| = |1 - dt / b_corr| > 1: the drift grows as |a|^t
+ * and, where the reference's serial recurrence overflows to alternating +-inf, the generators do not follow it
+ * (measured at a = -3 and a = -1.5): this generator (and b2ins_imu_err_stats_f64) gives NaN once an infinity
+ * enters a tile's scan, and for a = -1.5 +-inf; the fused Monte-Carlo kernels give alternating +-inf, a few
+ * samples from where the reference overflows; b2ins_allan_mc_f64 gives NaN at every tau.  Inside the float64 range
+ * all of them hold the drift to the same bound as for |a| <= 1. */
 int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n,
                         const double* ref_gyro, const double* ref_accel,
                         const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
@@ -602,6 +608,16 @@ int b2ins_diag_mc_shape(int lanes_per_run, int ref_frame, int* shape3);
  * length, or 0 for the direct synthesis).  Honours the tools' B2INS_PSD_DIRECT override (read once
  * per process, as the launch reads it).  Returns -1 if n <= 0 or P is NULL.  Pure host logic. */
 int b2ins_diag_psd_plan(int64_t n, int* P);
+
+/* The Gauss-Markov coefficients and the time segmentation b2ins_imu_noise_f64 and b2ins_imu_err_stats_f64
+ * use for `runs` runs of n samples on `sm_count` SMs (0: the current device, 132 if there is none):
+ * coef [3][6] = (gm_a, gm_b, wd) of the channels accel x y z, gyro x y z, as digested from the error models
+ * (d[t+1] = gm_a d[t] + gm_b z0[t], plus wd z0[t] for b_corr = +inf); plan [3] = (nseg, seg_len, pass1_len):
+ * nseg time segments of seg_len samples (the last one shorter), pass 1 reducing the last pass1_len samples
+ * of each (0 for nseg = 1).  Pass 1 is shortened only where every channel's |gm_a|^pass1_len < 1e-20.
+ * Pure host logic: the function the launch calls. */
+int b2ins_diag_noise_plan(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
+                          const b2ins_sensor_err* accel_err, int sm_count, double* coef, int64_t* plan);
 
 /* The device's own FP64 primitives (csrc/fastmath64.cuh, and mech.cuh's sincos_angle), applied
  * elementwise to n arguments: out0[i] = f(a[i]) (div: a[i] / b[i]); the sin/cos functions write
