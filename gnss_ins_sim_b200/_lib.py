@@ -110,6 +110,9 @@ SIGNATURES = {
     'b2ins_psd_series_len': (_I, [_L]),
     'b2ins_psd_workspace_bytes': (_L, [_L, _L]),
     'b2ins_psd_series_f64': (_I, [_D, _L, _L, _I, _I, _P, _P, _U64, _L, _P, _P, _P]),
+    'b2ins_welch_workspace_bytes': (_L, [_L, _L, _L, _L]),
+    'b2ins_welch_f64': (_I, [_D, _L, _L, _P, _L, _L, _L, _L, _L, _P, _P, _P, _P, _P]),
+    'b2ins_welch_f64_host': (_I, [_D, _L, _L, _P, _L, _L, _L, _L, _L, _P, _P, _P]),
     'b2ins_path_rows': (_L, [_P, _L, _D]),
     'b2ins_path_gen_host': (_L, [_P, _P, _L, _D, _D, _D, _D, _P, _I, _L, _P, _P, _P, c_int64_p, _P]),
     'b2ins_path_gen_ex_host': (_L, [_P, _P, _L, _D, _D, _D, _D, _P, _I, _L, _P, _P, _P, c_int64_p, _P, _P, _P]),

@@ -15,6 +15,7 @@
 #include "noise_kernel.cuh"
 #include "pathgen_host.h"
 #include "psd_kernel.cuh"
+#include "welch_kernel.cuh"
 #include "gps_kernel.cuh"
 #include "mag_kernel.cuh"
 #include "magcal_kernel.cuh"
@@ -1542,6 +1543,129 @@ int b2ins_diag_psd_plan(int64_t n, int* P) {
   const int len = psd_direct_forced() ? 0 : psd_fft_plan(psd_series_len(n), &bluestein);
   *P = len;
   return len == 0 ? 0 : (bluestein ? 2 : 1);
+}
+
+// ---------------------------------------------------------------- K11 -------
+// [0, 16): the bin scale; then K5's chirp transform (Bluestein, P <= 8192 complex); then the chunk sums
+static int64_t welch_partial_offset(const WelchPlan& w) { return 16 + (w.bluestein ? int64_t(w.P) * 16 : 0); }
+
+int64_t b2ins_welch_workspace_bytes(int64_t n, int64_t nseries, int64_t nperseg, int64_t noverlap) {
+  WelchPlan w;
+  if (nseries < 0 || !welch_plan(n, nperseg, noverlap, &w)) return -1;
+  const int64_t parts = w.nchunk > 1 ? nseries * w.nchunk * (w.M + 1) * 8 : 0;
+  return welch_partial_offset(w) + parts;
+}
+
+int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner, int64_t outer_stride,
+                    int64_t sample_stride, int64_t nperseg, int64_t noverlap, const double* window, double* psd,
+                    double* freq, void* workspace, void* stream) {
+  ARG_CHECK(fs > 0.0 && std::isfinite(fs) && nseries >= 0, "bad fs/nseries");
+  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
+  ARG_CHECK(noverlap >= 0 && noverlap < nperseg, "need 0 <= noverlap < nperseg, got noverlap=%lld, nperseg=%lld",
+            static_cast<long long>(noverlap), static_cast<long long>(nperseg));
+  ARG_CHECK(n >= nperseg, "a series of %lld samples is shorter than nperseg=%lld", static_cast<long long>(n),
+            static_cast<long long>(nperseg));
+  WelchPlan w;
+  ARG_CHECK(welch_plan(n, nperseg, noverlap, &w),
+            "nperseg=%lld: need an even length >= 16, a power of two up to 16384 or at most 8192",
+            static_cast<long long>(nperseg));
+  ARG_CHECK(window && freq && workspace && (nseries == 0 || (x && psd)), "null buffer");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  WelchParams p;
+  p.x = x;
+  p.inner = inner;
+  p.outer_stride = outer_stride;
+  p.sample_stride = sample_stride;
+  p.nseries = nseries;
+  p.S = w.S;
+  p.K = w.K;
+  p.Q = w.Q;
+  p.nchunk = w.nchunk;
+  p.N = w.N;
+  p.M = w.M;
+  p.P = w.P;
+  p.logP = w.logP;
+  p.G = w.G;
+  p.bluestein = w.bluestein;
+  p.fs = fs;
+  p.window = window;
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  p.wscale = reinterpret_cast<double*>(ws);
+  p.bhat = reinterpret_cast<const double2*>(ws + 16);
+  p.part = reinterpret_cast<double*>(ws + welch_partial_offset(w));
+  p.post = w.bluestein ? 0.25 / (static_cast<double>(w.P) * w.P) : 0.25;
+  p.psd = psd;
+  p.freq = freq;
+  welch_prep_kernel<<<1, kWelchThreads, 0, s>>>(p);
+  CU_CHECK(cudaGetLastError());
+  if (nseries == 0) return B2INS_OK;
+  const size_t fft_smem = static_cast<size_t>(w.P) * 24;
+  const size_t smem = (static_cast<size_t>(w.G) * w.P + w.P / 2) * 16;
+  if (w.bluestein) {   // K5's transform of the conjugate chirp: the forward transform runs K5's pipeline on conj z
+    PsdFftParams f;
+    std::memset(&f, 0, sizeof(f));
+    f.N = w.N;
+    f.M = w.M;
+    f.P = w.P;
+    f.logP = w.logP;
+    f.bluestein = 1;
+    f.bhat = reinterpret_cast<double2*>(ws + 16);
+    CU_CHECK(cudaFuncSetAttribute(psd_chirp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 24));
+    psd_chirp_kernel<<<1, kFftThreads, fft_smem, s>>>(f);
+    CU_CHECK(cudaGetLastError());
+  }
+  // the bins a thread accumulates: 3 for transforms of at most 1024 points (several segments per CTA), else 17
+  const bool small = w.P <= kWelchBatchPoints;
+  void (*const fn)(WelchParams) =
+      small ? (w.bluestein ? welch_kernel<kWelchAccSmall, true> : welch_kernel<kWelchAccSmall, false>)
+            : (w.bluestein ? welch_kernel<kWelchAccLarge, true> : welch_kernel<kWelchAccLarge, false>);
+  if (!small) CU_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 24));
+  int per_sm = 1;
+  CU_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kWelchThreads, smem));
+  const int64_t items = nseries * w.nchunk;
+  const int64_t cap = static_cast<int64_t>(sm_count()) * (per_sm > 0 ? per_sm : 1);
+  fn<<<static_cast<unsigned>(items < cap ? items : cap), kWelchThreads, smem, s>>>(p);
+  CU_CHECK(cudaGetLastError());
+  if (w.nchunk > 1) {
+    const int64_t total = nseries * (w.M + 1);
+    welch_finish_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(p);
+    CU_CHECK(cudaGetLastError());
+  }
+  return B2INS_OK;
+}
+
+int b2ins_welch_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner, int64_t outer_stride,
+                         int64_t sample_stride, int64_t nperseg, int64_t noverlap, const double* window, double* psd,
+                         double* freq) {
+  ARG_CHECK(nseries >= 0 && inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad nseries/strides");
+  const int64_t wsb = b2ins_welch_workspace_bytes(n, nseries, nperseg, noverlap);
+  ARG_CHECK(wsb >= 0, "bad n/nperseg/noverlap (n=%lld, nperseg=%lld, noverlap=%lld)", static_cast<long long>(n),
+            static_cast<long long>(nperseg), static_cast<long long>(noverlap));
+  ARG_CHECK(window && freq && (nseries == 0 || (x && psd)), "null buffer");
+  const int64_t L = nperseg / 2 + 1;
+  const int64_t outer = (nseries + inner - 1) / inner;
+  const int64_t elems = nseries == 0 ? 0 : (outer - 1) * outer_stride + (inner - 1) + (n - 1) * sample_stride + 1;
+  DevBuf dx, dw, dpsd, dfreq, ws;
+  Stream st;
+  CU_CHECK(st.create());
+  CU_CHECK(dx.alloc(static_cast<size_t>(elems > 0 ? elems : 1) * sizeof(double)));
+  CU_CHECK(dw.alloc(static_cast<size_t>(nperseg) * sizeof(double)));
+  CU_CHECK(dpsd.alloc(static_cast<size_t>(nseries > 0 ? nseries * L : 1) * sizeof(double)));
+  CU_CHECK(dfreq.alloc(static_cast<size_t>(L) * sizeof(double)));
+  CU_CHECK(ws.alloc(static_cast<size_t>(wsb)));
+  if (elems > 0)
+    CU_CHECK(cudaMemcpyAsync(dx.p, x, static_cast<size_t>(elems) * sizeof(double), cudaMemcpyHostToDevice, st.s));
+  CU_CHECK(cudaMemcpyAsync(dw.p, window, static_cast<size_t>(nperseg) * sizeof(double), cudaMemcpyHostToDevice,
+                           st.s));
+  const int rc = b2ins_welch_f64(fs, n, nseries, dx.d(), inner, outer_stride, sample_stride, nperseg, noverlap,
+                                 dw.d(), dpsd.d(), dfreq.d(), ws.p, st.s);
+  if (rc != B2INS_OK) return rc;
+  if (nseries > 0)
+    CU_CHECK(cudaMemcpyAsync(psd, dpsd.p, static_cast<size_t>(nseries * L) * sizeof(double), cudaMemcpyDeviceToHost,
+                             st.s));
+  CU_CHECK(cudaMemcpyAsync(freq, dfreq.p, static_cast<size_t>(L) * sizeof(double), cudaMemcpyDeviceToHost, st.s));
+  CU_CHECK(cudaStreamSynchronize(st.s));
+  return B2INS_OK;
 }
 
 // ---------------------------------------------------------------- K1 plan ---

@@ -151,13 +151,15 @@ __device__ __forceinline__ void fft_twiddles(double2* tw, int P) {
     tw[j] = make_double2(c, s);
   }
 }
-// in-place radix-2, decimation in time: bit-reversed input -> natural output; SIGN = +1: e^{+...}
+// in-place radix-2, decimation in time: bit-reversed input -> natural output; SIGN = +1: e^{+...}.
+// `batch` transforms of length P lie back to back in x: butterfly b of the batch indexes the same
+// pair and twiddle as in a single transform, because half divides P / 2.
 template <int SIGN>
-__device__ __forceinline__ void fft_dit(double2* x, const double2* tw, int P) {
+__device__ __forceinline__ void fft_dit(double2* x, const double2* tw, int P, int batch = 1) {
   for (int half = 1; half < P; half <<= 1) {
     const int tstep = P / (2 * half);
     __syncthreads();
-    for (int b = threadIdx.x; b < P / 2; b += blockDim.x) {
+    for (int b = threadIdx.x; b < (P / 2) * batch; b += blockDim.x) {
       const int j = b & (half - 1);
       const int i = ((b - j) << 1) + j;
       double2 w = tw[j * tstep];
@@ -171,11 +173,11 @@ __device__ __forceinline__ void fft_dit(double2* x, const double2* tw, int P) {
 }
 // decimation in frequency: natural input -> bit-reversed output
 template <int SIGN>
-__device__ __forceinline__ void fft_dif(double2* x, const double2* tw, int P) {
+__device__ __forceinline__ void fft_dif(double2* x, const double2* tw, int P, int batch = 1) {
   for (int half = P / 2; half >= 1; half >>= 1) {
     const int tstep = P / (2 * half);
     __syncthreads();
-    for (int b = threadIdx.x; b < P / 2; b += blockDim.x) {
+    for (int b = threadIdx.x; b < (P / 2) * batch; b += blockDim.x) {
       const int j = b & (half - 1);
       const int i = ((b - j) << 1) + j;
       double2 w = tw[j * tstep];

@@ -523,6 +523,33 @@ def _k4o(symbol, fs, x, n, nseries, inner, outer_stride, sample_stride):
     return var, tau
 
 
+def welch_workspace_bytes(n, nseries, nperseg, noverlap):
+    """Device scratch of engine.welch; negative if nperseg is not a length K11 transforms (or noverlap and n
+    give no segment)."""
+    return int(_lib.load().b2ins_welch_workspace_bytes(int(n), int(nseries), int(nperseg), int(noverlap)))
+
+
+def welch(fs, x, n, nseries, nperseg, noverlap, window, inner=1, outer_stride=None, sample_stride=1):
+    """K11: scipy.signal.welch(x, fs, window, nperseg, noverlap) (detrend='constant', scaling='density',
+    one-sided, nfft = nperseg) of `nseries` series of n samples, addressed as in allan().  window: [nperseg]
+    floats.  Returns psd [nseries, nperseg // 2 + 1], freq [nperseg // 2 + 1] (CUDA)."""
+    _require_cuda()
+    if outer_stride is None:
+        outer_stride = n * sample_stride if inner == 1 else n * inner
+    L = int(nperseg) // 2 + 1
+    w = to_device(window, x.device)
+    if w.shape != (int(nperseg),):
+        raise ValueError('window must have shape (%d,), got %s' % (int(nperseg), tuple(w.shape)))
+    psd = torch.empty((nseries, L), dtype=torch.float64, device=x.device)
+    freq = torch.empty((L,), dtype=torch.float64, device=x.device)
+    ws = torch.empty(max(welch_workspace_bytes(n, nseries, nperseg, noverlap), 8) // 8 + 1, dtype=torch.float64,
+                     device=x.device)
+    _lib.check(_lib.load().b2ins_welch_f64(float(fs), int(n), int(nseries), _ptr(x), int(inner), int(outer_stride),
+                                           int(sample_stride), int(nperseg), int(noverlap), _ptr(w), _ptr(psd),
+                                           _ptr(freq), _ptr(ws), _stream()))
+    return psd, freq
+
+
 def allan_mc(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0):
     """K1 fused into K4: Allan variance of `runs` Monte-Carlo runs x 6 channels whose series are
     generated inside the tau-binning kernel (never written).  ref_gyro, ref_accel: CUDA f64 [n,3].

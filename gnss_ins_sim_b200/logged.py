@@ -169,6 +169,9 @@ OUTPUT_FORMAT = {
     'ad_accel': (['AD_accel_x', 'AD_accel_y', 'AD_accel_z'], ['m/s^2'] * 3, ['m/s^2'] * 3),
     'hd_gyro': (['HD_gyro_x', 'HD_gyro_y', 'HD_gyro_z'], ['rad/s'] * 3, ['deg/s'] * 3),
     'hd_accel': (['HD_accel_x', 'HD_accel_y', 'HD_accel_z'], ['m/s^2'] * 3, ['m/s^2'] * 3),
+    'algo_freq': (['algo_freq'], ['Hz'], ['Hz']),
+    'psd_accel': (['PSD_accel_x', 'PSD_accel_y', 'PSD_accel_z'], ['m^2/s^4/Hz'] * 3, ['m^2/s^4/Hz'] * 3),
+    'psd_gyro': (['PSD_gyro_x', 'PSD_gyro_y', 'PSD_gyro_z'], ['rad^2/s^2/Hz'] * 3, ['rad^2/s^2/Hz'] * 3),
 }
 
 

@@ -18,6 +18,7 @@ Dispatch on `algorithm`:
     lazily: counter-based Philox makes any run reproducible in isolation, so
     get_data(['pos'])[0]['algo0_7'] re-runs just run 7 with history output on.
   * gnss_ins_sim_b200 Allan            -> K1 (noise) + K4 (Allan variance) per run block.
+  * gnss_ins_sim_b200 Psd              -> K1 (noise) + K11 (Welch power spectral density) per run block.
   * gnss_ins_sim_b200 MagCal           -> K8's samples regenerated inside K10 (magnetometer calibration).
   * any other reference-style plugin   -> K1 generates gyro/accel (K8 the magnetometer of a
     9-axis IMU) on the device, the plugin's own .run() is called per run on the host
@@ -38,6 +39,7 @@ from . import engine, dist, logged
 from .free_integration import FreeIntegration
 from .free_integration_odo import FreeIntegration as FreeIntegrationOdo
 from .allan_analysis import Allan
+from .psd_analysis import Psd
 from .ins_loose import InsLoose, gps_sample_index
 from .mag_calibrate import MagCal, check_segments
 
@@ -493,7 +495,7 @@ class Sim(object):
             for i, a in enumerate(self.algo):
                 if isinstance(a, FreeIntegration):     # incl. the odometer variant
                     self._run_free_integration(i, a)
-                elif isinstance(a, Allan):
+                elif isinstance(a, (Allan, Psd)):
                     self._run_allan(i, a)
                 elif isinstance(a, InsLoose):
                     self._run_ins_loose(i, a)
@@ -558,7 +560,7 @@ class Sim(object):
                         pos[:, -1] - d['ref_pos'][-1], vel[:, -1] - d['ref_vel'][-1]], axis=1)
                     self._mc[i]['end_err'] = err
                     self.err_stats[name] = engine.error_stats(engine.to_device(err)).cpu().numpy()
-            elif isinstance(a, Allan):
+            elif isinstance(a, (Allan, Psd)):
                 self._publish_allan(name, a, *a.run_batch(self.fs[0], self._logged_sets('accel'),
                                                           self._logged_sets('gyro')))
             elif isinstance(a, InsLoose):
@@ -799,9 +801,10 @@ class Sim(object):
         return max(1, min(max(hi - lo, 1), int(free_b / share // (n * bytes_per_sample)) or 1))
 
     def _publish_allan(self, name, algo, tau, accel, gyro):
-        """algo_time (the same tau for every run) and the plugin's accel and gyro outputs [R, ntau, 3] (ad_* for
-        Allan, hd_* for Hadamard) under run keys.  Allan and Hadamard plugins of one Sim share algo_time: each
-        replaces its own run keys in it and keeps the others'."""
+        """The plugin's first output, its abscissa (algo_time: the same tau for every run; algo_freq for Psd),
+        and its accel and gyro outputs [R, ntau, 3] (ad_* for Allan, hd_* for Hadamard, psd_* for Psd) under run
+        keys.  Plugins of one Sim with the same abscissa share it: each replaces its own run keys in it and keeps
+        the others'."""
         t, o_accel, o_gyro = algo.output
         prev = self.data.get(t)
         keep = {k: v for k, v in prev.items() if not k.startswith(name + '_')} if isinstance(prev, dict) else {}
@@ -816,15 +819,20 @@ class Sim(object):
         the only device memory is the decade-sum workspace (about 2 B per run-sample), so run blocks are
         rarely needed; otherwise K1 materialises the series (48 B per run-sample) for K4 (~2 B of workspace).
         Allan(overlapping=True) and Hadamard() always materialise: K4o needs its prefix workspace (about 48 B per
-        run-sample for the three series of one sensor) beside the series."""
+        run-sample for the three series of one sensor) beside the series.  Psd() materialises too, with K11's
+        chunk sums beside the series; its abscissa is the frequency grid instead of tau."""
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
+        spectral = isinstance(algo, Psd)
         overlapping = getattr(algo, 'overlapping', False)
-        fused = (not overlapping and self._vib_acc is None and self._vib_gyro is None and n > 5040
+        fused = (not spectral and not overlapping and self._vib_acc is None and self._vib_gyro is None and n > 5040
                  and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
-        tau = engine.allan_taus(n, self.fs[0])
+        tau = algo.frequencies(self.fs[0]) if spectral else engine.allan_taus(n, self.fs[0])
         if fused:
             block = self._allan_block(6 * 2, 2)
+        elif spectral:      # K1's 48 B per run-sample, then K11's chunk sums for the six series of a run
+            ws = engine.welch_workspace_bytes(n, 6, algo.nperseg, algo.noverlap)
+            block = self._allan_block(48 + max(ws, 0) / n, 3)
         elif overlapping:   # K1's 48 B per run-sample, then K4o's workspace for one sensor's 3 series
             block = self._allan_block(64 + engine.oallan_workspace_bytes(n, 3) / n, 3)
         else:

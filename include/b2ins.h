@@ -482,6 +482,28 @@ int b2ins_psd_series_f64(double fs, int64_t n, int64_t runs, int sensor, int tab
                          const double* freq, const double* sxx3, uint64_t seed,
                          int64_t run_offset, double* series, void* workspace, void* stream);
 
+/* ---- K11: Welch power spectral density ---------------------------------------------
+ * scipy.signal.welch(x, fs, window, nperseg, noverlap) with detrend='constant', scaling='density',
+ * average='mean', one-sided, nfft = nperseg, for `nseries` series at once.  N = nperseg, D = noverlap,
+ * S = N - D, K = (n - D) / S segments (samples after the last are unused), L = N / 2 + 1:
+ *   psd[k] = (1/K) sum_j c_k |DFT_N((x_j - mean x_j) w)[k]|^2 / (fs sum w^2), c_0 = c_{L-1} = 1, else 2;
+ *   freq[k] = k / (N (1/fs)), as np.fft.rfftfreq.
+ * N must be even, >= 16, and a power of two up to 16384 or at most 8192; 0 <= D < N; n >= N.
+ * Series addressing as b2ins_allan_f64.  window [N] (device): any finite window.  psd [nseries][L],
+ * freq [L] (device).  A NaN or +-inf sample inside a used segment makes every bin of its series NaN.
+ * Deterministic: a series gives the same bits whatever the batch, its position and its layout.
+ * b2ins_welch_workspace_bytes: device scratch for these arguments, negative if nperseg is not a
+ * length this transform takes (or noverlap, n do not give a segment). */
+int64_t b2ins_welch_workspace_bytes(int64_t n, int64_t nseries, int64_t nperseg, int64_t noverlap);
+int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x,
+                    int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                    int64_t nperseg, int64_t noverlap, const double* window,
+                    double* psd, double* freq, void* workspace, void* stream);
+int b2ins_welch_f64_host(double fs, int64_t n, int64_t nseries, const double* x,
+                         int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                         int64_t nperseg, int64_t noverlap, const double* window,
+                         double* psd, double* freq);
+
 /* ---- K6: GPS measurement generator ---------------------------------------------------
  * Replaces pathgen.gps_gen (gnss_ins_sim/pathgen/pathgen.py:596-625) and its call in loop A
  * (gnss_ins_sim/sim/ins_sim.py:497-500) for `runs` runs at once:
