@@ -7,9 +7,10 @@ import numpy as np
 import torch
 
 from . import engine
+from .series_analysis import SeriesEstimator
 
 
-class Allan(object):
+class Allan(SeriesEstimator):
     '''
     Allan deviation of the three accelerometer and three gyroscope channels.
 
@@ -26,51 +27,27 @@ class Allan(object):
     def __init__(self, overlapping=False):
         if not isinstance(overlapping, (bool, np.bool_)):
             raise TypeError('overlapping must be True or False, got %r' % (overlapping,))
+        super().__init__(['algo_time', 'ad_accel', 'ad_gyro'])
         self.overlapping = bool(overlapping)
-        self.input = ['fs', 'accel', 'gyro']
-        self.output = ['algo_time', 'ad_accel', 'ad_gyro']
-        self.batch = True
-        self.results = None
 
-    def run(self, set_of_input):
-        '''
-        set_of_input = [fs, accel (n,3), gyro (n,3)]
-        '''
-        fs = set_of_input[0]
-        tau, ad_a, ad_g = self.run_batch(fs, np.asarray(set_of_input[1])[None],
-                                         np.asarray(set_of_input[2])[None])
-        self.results = [tau, ad_a[0], ad_g[0]]
+    @property
+    def fused(self):
+        return not self.overlapping     # engine.allan_mc: K1 fused into K4
 
-    def run_batch(self, fs, accel, gyro, to_host=True, channel_major=False):
-        '''
-        accel, gyro: [R, n, 3] (the reference's per-run arrays) or, channel_major, [R, 3, n].
-        Returns tau [ntau], ad_accel [R, ntau, 3], ad_gyro [R, ntau, 3]
-        (Allan DEVIATION = sqrt(avar), allan_analysis.py:47-49).
-        '''
-        a = engine.to_device(accel)
-        g = engine.to_device(gyro)
-        var = self._variance()
-        out = []
-        for x in (a, g):
-            if channel_major:     # 3R contiguous series: the bulk-copy front end of K4
-                R, _, n = x.shape
-                avar, tau = var(fs, x, n, R * 3)
-            else:                 # 3R interleaved series, read in place (no copy)
-                R, n, _ = x.shape
-                avar, tau = var(fs, x, n, R * 3, inner=3, outer_stride=3 * n, sample_stride=3)
-            out.append(torch.sqrt(avar).reshape(R, 3, -1).permute(0, 2, 1).contiguous())
-        if to_host:
-            return tau.cpu().numpy(), out[0].cpu().numpy(), out[1].cpu().numpy()
-        return tau, out[0], out[1]
+    def _series(self, fs, x, n, nseries, **addressing):
+        var, tau = self._variance()(fs, x, n, nseries, **addressing)
+        return torch.sqrt(var), tau     # the DEVIATION, as allan_analysis.py:47-49
 
     def _variance(self):
         return engine.oallan if self.overlapping else engine.allan
 
-    def get_results(self):
-        return self.results
+    def abscissa(self, n, fs):
+        return engine.allan_taus(n, fs)
 
-    def reset(self):
-        pass
+    def run_bytes(self, n):
+        # 64 B per run-sample for K1's series (48 B) and K4's workspace; K4o adds its prefix workspace for the
+        # three series of one sensor
+        return 64 + engine.oallan_workspace_bytes(n, 3) / n if self.overlapping else 64
 
 
 class Hadamard(Allan):

@@ -239,13 +239,78 @@ struct DevBuf {
   double* d() const { return static_cast<double*>(p); }
 };
 
-struct Stream {
-  cudaStream_t s = nullptr;
-  ~Stream() {
-    if (s) cudaStreamDestroy(s);
+// One call of a device entry point from host memory (the *_host wrappers): a stream of its own, device copies
+// of the inputs queued on it, device room for the outputs and the scratch.  run() calls the device entry on
+// the stream, copies the outputs back and synchronises.  After the first failed CUDA call nothing more is
+// allocated or queued and run() reports that call; every buffer and the stream are released on every exit.
+class Staging {
+ public:
+  Staging() { note(cudaStreamCreateWithFlags(&s_, cudaStreamNonBlocking), "cudaStreamCreateWithFlags"); }
+  ~Staging() {
+    for (const Buf& b : bufs_) cudaFree(b.dev);
+    if (s_) cudaStreamDestroy(s_);
   }
-  cudaError_t create() { return cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
+  // a device copy of the `elems` doubles at host
+  const double* in(const double* host, int64_t elems) {
+    const size_t bytes = static_cast<size_t>(elems) * sizeof(double);
+    double* d = alloc(bytes, nullptr);
+    if (d && bytes) note(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, s_), "cudaMemcpyAsync");
+    return d;
+  }
+  // device room for `elems` doubles, copied back to host by run() unless host is null
+  double* out(double* host, int64_t elems) { return alloc(static_cast<size_t>(elems) * sizeof(double), host); }
+  void* scratch(int64_t bytes) { return alloc(static_cast<size_t>(bytes), nullptr); }
+
+  template <class DeviceCall>
+  int run(DeviceCall call) {
+    if (err_ != cudaSuccess) return fail(B2INS_ERR_CUDA, "%s: %s", what_, cudaGetErrorString(err_));
+    const int rc = call(s_);
+    if (rc != B2INS_OK) return rc;
+    for (const Buf& b : bufs_)
+      if (b.host && b.bytes) CU_CHECK(cudaMemcpyAsync(b.host, b.dev, b.bytes, cudaMemcpyDeviceToHost, s_));
+    CU_CHECK(cudaStreamSynchronize(s_));
+    return B2INS_OK;
+  }
+
+ private:
+  struct Buf {
+    void* dev;
+    void* host;
+    size_t bytes;
+  };
+  double* alloc(size_t bytes, void* host) {
+    void* p = nullptr;
+    if (err_ != cudaSuccess || !note(cudaMalloc(&p, bytes ? bytes : 16), "cudaMalloc")) return nullptr;
+    bufs_.push_back({p, host, bytes});
+    return static_cast<double*>(p);
+  }
+  bool note(cudaError_t e, const char* what) {
+    if (e != cudaSuccess && err_ == cudaSuccess) {
+      err_ = e;
+      what_ = what;
+    }
+    return e == cudaSuccess;
+  }
+  cudaStream_t s_ = nullptr;
+  cudaError_t err_ = cudaSuccess;
+  const char* what_ = "";
+  std::vector<Buf> bufs_;
 };
+
+// What K4, K4o and K11 check in common: the sample rate, the sizes and the addressing of the series
+// (series s, sample t at x[s / inner * outer_stride + (s % inner) + t * sample_stride])
+int series_check(double fs, int64_t n, int64_t nseries, int64_t inner, int64_t outer_stride, int64_t sample_stride) {
+  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
+  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
+  return B2INS_OK;
+}
+
+// elements of x from the first the series read to the last (0 without series): what a *_host wrapper stages
+int64_t series_elems(int64_t n, int64_t nseries, int64_t inner, int64_t outer_stride, int64_t sample_stride) {
+  if (nseries == 0) return 0;
+  const int64_t outer = (nseries + inner - 1) / inner;
+  return (outer - 1) * outer_stride + (inner - 1) + (n - 1) * sample_stride + 1;
+}
 
 // stream-ordered scratch: freed after the work queued on s before it, on every exit path; free() does it early
 // and returns the error
@@ -464,29 +529,18 @@ int b2ins_free_integration_f64_host(int ref_frame, double fs, int64_t runs, int6
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(gyro && accel && ini && att && pos && vel, "null buffer");
   ARG_CHECK(ini_sets >= 1 && (ini_rows == 9 || ini_rows == 10), "ini must be [sets>=1][9|10]");
-  const size_t bytes = static_cast<size_t>(runs) * n * 3 * sizeof(double);
-  const size_t ini_bytes = static_cast<size_t>(ini_sets) * ini_rows * sizeof(double);
-  DevBuf dg, da, di, oa, op, ov;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(dg.alloc(bytes));
-  CU_CHECK(da.alloc(bytes));
-  CU_CHECK(di.alloc(ini_bytes));
-  CU_CHECK(oa.alloc(bytes));
-  CU_CHECK(op.alloc(bytes));
-  CU_CHECK(ov.alloc(bytes));
-  CU_CHECK(cudaMemcpyAsync(dg.p, gyro, bytes, cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(da.p, accel, bytes, cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(di.p, ini, ini_bytes, cudaMemcpyHostToDevice, st.s));
-  const int rc = b2ins_free_integration_f64(ref_frame, fs, runs, n, dg.d(), da.d(), layout, di.d(),
-                                            ini_sets, ini_rows, run_offset, earth_rot, oa.d(),
-                                            op.d(), ov.d(), lanes_per_run, st.s);
-  if (rc != B2INS_OK) return rc;
-  CU_CHECK(cudaMemcpyAsync(att, oa.p, bytes, cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaMemcpyAsync(pos, op.p, bytes, cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaMemcpyAsync(vel, ov.p, bytes, cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
+  const int64_t elems = runs * n * 3;
+  Staging st;
+  const double* dg = st.in(gyro, elems);
+  const double* da = st.in(accel, elems);
+  const double* di = st.in(ini, int64_t(ini_sets) * ini_rows);
+  double* oa = st.out(att, elems);
+  double* op = st.out(pos, elems);
+  double* ov = st.out(vel, elems);
+  return st.run([&](cudaStream_t s) {
+    return b2ins_free_integration_f64(ref_frame, fs, runs, n, dg, da, layout, di, ini_sets, ini_rows, run_offset,
+                                      earth_rot, oa, op, ov, lanes_per_run, s);
+  });
 }
 
 // ---------------------------------------------------------------- K1 --------
@@ -705,28 +759,15 @@ int b2ins_magcal_fed_f64_host(int64_t runs, int64_t n, const int64_t* seg, const
   ARG_CHECK(run_stride >= 0 && sample_stride >= 3, "run_stride must be >= 0 and sample_stride >= 3");
   if (runs == 0) return B2INS_OK;
   ARG_CHECK(mag && soft_iron && hard_iron, "null buffer");
-  const int64_t elems = (runs - 1) * run_stride + (n - 1) * sample_stride + 3;
   const int64_t L = (seg[1] - seg[0]) + (seg[3] - seg[2]) + (seg[5] - seg[4]);
-  DevBuf dx, dsi, dhi, dcal;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(dx.alloc(static_cast<size_t>(elems) * sizeof(double)));
-  CU_CHECK(dsi.alloc(static_cast<size_t>(runs) * 9 * sizeof(double)));
-  CU_CHECK(dhi.alloc(static_cast<size_t>(runs) * 4 * sizeof(double)));
-  if (mag_cal) CU_CHECK(dcal.alloc(static_cast<size_t>(runs) * L * 3 * sizeof(double)));
-  CU_CHECK(cudaMemcpyAsync(dx.p, mag, static_cast<size_t>(elems) * sizeof(double), cudaMemcpyHostToDevice, st.s));
-  const int rc2 = b2ins_magcal_fed_f64(runs, n, seg, dx.d(), run_stride, sample_stride, dsi.d(), dhi.d(),
-                                       mag_cal ? dcal.d() : nullptr, st.s);
-  if (rc2 != B2INS_OK) return rc2;
-  CU_CHECK(cudaMemcpyAsync(soft_iron, dsi.p, static_cast<size_t>(runs) * 9 * sizeof(double), cudaMemcpyDeviceToHost,
-                           st.s));
-  CU_CHECK(cudaMemcpyAsync(hard_iron, dhi.p, static_cast<size_t>(runs) * 4 * sizeof(double), cudaMemcpyDeviceToHost,
-                           st.s));
-  if (mag_cal)
-    CU_CHECK(cudaMemcpyAsync(mag_cal, dcal.p, static_cast<size_t>(runs) * L * 3 * sizeof(double),
-                             cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
+  Staging st;
+  const double* dx = st.in(mag, (runs - 1) * run_stride + (n - 1) * sample_stride + 3);
+  double* dsi = st.out(soft_iron, runs * 9);
+  double* dhi = st.out(hard_iron, runs * 4);
+  double* dcal = mag_cal ? st.out(mag_cal, runs * L * 3) : nullptr;
+  return st.run([&](cudaStream_t s) {
+    return b2ins_magcal_fed_f64(runs, n, seg, dx, run_stride, sample_stride, dsi, dhi, dcal, s);
+  });
 }
 
 int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n, const double* ref_gyro,
@@ -740,27 +781,17 @@ int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n, const double* r
   ARG_CHECK(!(vib_gyro && vib_gyro->type == B2INS_VIB_SERIES) &&
                 !(vib_accel && vib_accel->type == B2INS_VIB_SERIES),
             "VIB_SERIES takes a device pointer: use the device entry point");
-  const size_t ref_bytes = static_cast<size_t>(n) * 3 * sizeof(double);
-  const size_t bytes = static_cast<size_t>(runs) * ref_bytes;
-  DevBuf rg, ra, og, oa, zd;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(rg.alloc(ref_bytes));
-  CU_CHECK(ra.alloc(ref_bytes));
-  CU_CHECK(og.alloc(bytes));
-  CU_CHECK(oa.alloc(bytes));
-  if (z_dump) CU_CHECK(zd.alloc(bytes * 4));
-  CU_CHECK(cudaMemcpyAsync(rg.p, ref_gyro, ref_bytes, cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(ra.p, ref_accel, ref_bytes, cudaMemcpyHostToDevice, st.s));
-  const int rc = b2ins_imu_noise_f64(fs, runs, n, rg.d(), ra.d(), gyro_err, accel_err, vib_gyro,
-                                     vib_accel, seed, run_offset, layout, og.d(), oa.d(),
-                                     z_dump ? zd.d() : nullptr, st.s);
-  if (rc != B2INS_OK) return rc;
-  CU_CHECK(cudaMemcpyAsync(gyro, og.p, bytes, cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaMemcpyAsync(accel, oa.p, bytes, cudaMemcpyDeviceToHost, st.s));
-  if (z_dump) CU_CHECK(cudaMemcpyAsync(z_dump, zd.p, bytes * 4, cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
+  const int64_t ref = n * 3, elems = runs * ref;
+  Staging st;
+  const double* rg = st.in(ref_gyro, ref);
+  const double* ra = st.in(ref_accel, ref);
+  double* og = st.out(gyro, elems);
+  double* oa = st.out(accel, elems);
+  double* zd = z_dump ? st.out(z_dump, elems * 4) : nullptr;
+  return st.run([&](cudaStream_t s) {
+    return b2ins_imu_noise_f64(fs, runs, n, rg, ra, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset,
+                               layout, og, oa, zd, s);
+  });
 }
 
 // ---------------------------------------------------------------- K12 -------
@@ -864,36 +895,23 @@ int b2ins_mc_free_integration_f64_host(const b2ins_mc_config* cfg, const double*
             "VIB_SERIES takes a device pointer: use the device entry point");
   ARG_CHECK(cfg->ini_sets >= 1 && (cfg->ini_rows == 9 || cfg->ini_rows == 10),
             "ini must be [sets>=1][9|10]");
-  const size_t ref_bytes = static_cast<size_t>(cfg->n) * 3 * sizeof(double);
-  const size_t ini_bytes = static_cast<size_t>(cfg->ini_sets) * cfg->ini_rows * sizeof(double);
-  const size_t err_bytes = static_cast<size_t>(cfg->runs) * 9 * sizeof(double);
-  DevBuf rg, ra, rn, di, de, ds, ws;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(rg.alloc(ref_bytes));
-  CU_CHECK(ra.alloc(ref_bytes));
-  CU_CHECK(rn.alloc(ref_bytes * 3));
-  CU_CHECK(di.alloc(ini_bytes));
-  CU_CHECK(de.alloc(err_bytes));
-  CU_CHECK(ds.alloc(27 * sizeof(double)));
-  CU_CHECK(ws.alloc(static_cast<size_t>(b2ins_error_stats_workspace_bytes(9))));
-  CU_CHECK(cudaMemcpyAsync(rg.p, ref_gyro, ref_bytes, cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(ra.p, ref_accel, ref_bytes, cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(rn.p, ref_nav, ref_bytes * 3, cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(di.p, ini, ini_bytes, cudaMemcpyHostToDevice, st.s));
+  const int64_t ref = cfg->n * 3;
+  Staging st;
+  const double* rg = st.in(ref_gyro, ref);
+  const double* ra = st.in(ref_accel, ref);
+  const double* rn = st.in(ref_nav, ref * 3);
+  const double* di = st.in(ini, int64_t(cfg->ini_sets) * cfg->ini_rows);
+  double* de = st.out(end_err, cfg->runs * 9);    // the statistics' input: on the device even if end_err is null
+  double* ds = st.out(stats, 27);
+  void* ws = st.scratch(b2ins_error_stats_workspace_bytes(9));
   b2ins_mc_config c = *cfg;
   c.stats_start = -1;
   c.dump_runs = 0;
-  int rc = b2ins_mc_free_integration_f64(&c, rg.d(), ra.d(), rn.d(), di.d(), de.d(), nullptr,
-                                         nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                         st.s);
-  if (rc != B2INS_OK) return rc;
-  rc = b2ins_error_stats_f64(cfg->runs, 9, de.d(), ds.d(), ws.d(), st.s);
-  if (rc != B2INS_OK) return rc;
-  if (end_err) CU_CHECK(cudaMemcpyAsync(end_err, de.p, err_bytes, cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaMemcpyAsync(stats, ds.p, 27 * sizeof(double), cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
+  return st.run([&](cudaStream_t s) {
+    const int rc = b2ins_mc_free_integration_f64(&c, rg, ra, rn, di, de, nullptr, nullptr, nullptr, nullptr,
+                                                 nullptr, nullptr, nullptr, s);
+    return rc != B2INS_OK ? rc : b2ins_error_stats_f64(cfg->runs, 9, de, ds, ws, s);
+  });
 }
 
 // ---------------------------------------------------------------- plan ------
@@ -1369,8 +1387,8 @@ int64_t b2ins_allan_workspace_bytes(int64_t n, int64_t nseries) {
 int b2ins_allan_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
                     int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
                     void* workspace, void* stream) {
-  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
-  ARG_CHECK(inner >= 1 && sample_stride >= 1, "bad strides");
+  const int chk = series_check(fs, n, nseries, inner, outer_stride, sample_stride);
+  if (chk != B2INS_OK) return chk;
   int64_t mult[128];
   const int ntau = b2ins_allan_num_tau(n, fs, mult, 128);
   if (ntau == 0 || nseries == 0) return B2INS_OK;
@@ -1415,34 +1433,32 @@ int b2ins_allan_mc_f64(double fs, int64_t n, int64_t runs, const double* ref_gyr
   return B2INS_OK;
 }
 
-int b2ins_allan_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
-                         int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
-  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
-  ARG_CHECK(inner >= 1 && sample_stride >= 1, "bad strides");
+// K4 and K4o's two forms from host memory: the device entry's checks, then only the span of x the series read
+typedef int (*VarianceEntry)(double, int64_t, int64_t, const double*, int64_t, int64_t, int64_t, double*, double*,
+                             void*, void*);
+
+static int variance_host(VarianceEntry entry, int64_t (*workspace_bytes)(int64_t, int64_t), double fs, int64_t n,
+                         int64_t nseries, const double* x, int64_t inner, int64_t outer_stride, int64_t sample_stride,
+                         double* var, double* tau) {
+  const int chk = series_check(fs, n, nseries, inner, outer_stride, sample_stride);
+  if (chk != B2INS_OK) return chk;
   const int ntau = b2ins_allan_num_tau(n, fs, nullptr, 0);
   if (ntau == 0 || nseries == 0) return B2INS_OK;
-  ARG_CHECK(x && avar && tau, "null buffer");
-  // extent of x touched
-  const int64_t outer = (nseries + inner - 1) / inner;
-  const int64_t elems = (outer - 1) * outer_stride + (inner - 1) + (n - 1) * sample_stride + 1;
-  DevBuf dx, dav, dtau, ws;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(dx.alloc(static_cast<size_t>(elems) * sizeof(double)));
-  CU_CHECK(dav.alloc(static_cast<size_t>(nseries) * ntau * sizeof(double)));
-  CU_CHECK(dtau.alloc(static_cast<size_t>(ntau) * sizeof(double)));
-  CU_CHECK(ws.alloc(static_cast<size_t>(allan_workspace_bytes(n, nseries))));
-  CU_CHECK(cudaMemcpyAsync(dx.p, x, static_cast<size_t>(elems) * sizeof(double),
-                           cudaMemcpyHostToDevice, st.s));
-  const int rc = b2ins_allan_f64(fs, n, nseries, dx.d(), inner, outer_stride, sample_stride,
-                                 dav.d(), dtau.d(), ws.p, st.s);
-  if (rc != B2INS_OK) return rc;
-  CU_CHECK(cudaMemcpyAsync(avar, dav.p, static_cast<size_t>(nseries) * ntau * sizeof(double),
-                           cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaMemcpyAsync(tau, dtau.p, static_cast<size_t>(ntau) * sizeof(double),
-                           cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
+  ARG_CHECK(x && var && tau, "null buffer");
+  Staging st;
+  const double* dx = st.in(x, series_elems(n, nseries, inner, outer_stride, sample_stride));
+  double* dvar = st.out(var, nseries * ntau);
+  double* dtau = st.out(tau, ntau);
+  void* ws = st.scratch(workspace_bytes(n, nseries));
+  return st.run([&](cudaStream_t s) {
+    return entry(fs, n, nseries, dx, inner, outer_stride, sample_stride, dvar, dtau, ws, s);
+  });
+}
+
+int b2ins_allan_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
+                         int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
+  return variance_host(b2ins_allan_f64, b2ins_allan_workspace_bytes, fs, n, nseries, x, inner, outer_stride,
+                       sample_stride, avar, tau);
 }
 
 // ---------------------------------------------------------------- K4o -------
@@ -1454,8 +1470,8 @@ int64_t b2ins_oallan_workspace_bytes(int64_t n, int64_t nseries) {
 static int oallan_f64(bool hadamard, double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
                       int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
                       void* workspace, void* stream) {
-  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
-  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
+  const int chk = series_check(fs, n, nseries, inner, outer_stride, sample_stride);
+  if (chk != B2INS_OK) return chk;
   int64_t mult[128];
   const int ntau = b2ins_allan_num_tau(n, fs, mult, 128);
   if (ntau == 0 || nseries == 0) return B2INS_OK;
@@ -1473,35 +1489,6 @@ static int oallan_f64(bool hadamard, double fs, int64_t n, int64_t nseries, cons
   return B2INS_OK;
 }
 
-static int oallan_f64_host(bool hadamard, double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
-                           int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
-  ARG_CHECK(fs > 0.0 && n >= 0 && nseries >= 0, "bad fs/n/nseries");
-  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
-  const int ntau = b2ins_allan_num_tau(n, fs, nullptr, 0);
-  if (ntau == 0 || nseries == 0) return B2INS_OK;
-  ARG_CHECK(x && avar && tau, "null buffer");
-  const int64_t outer = (nseries + inner - 1) / inner;
-  const int64_t elems = (outer - 1) * outer_stride + (inner - 1) + (n - 1) * sample_stride + 1;
-  DevBuf dx, dav, dtau, ws;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(dx.alloc(static_cast<size_t>(elems) * sizeof(double)));
-  CU_CHECK(dav.alloc(static_cast<size_t>(nseries) * ntau * sizeof(double)));
-  CU_CHECK(dtau.alloc(static_cast<size_t>(ntau) * sizeof(double)));
-  CU_CHECK(ws.alloc(static_cast<size_t>(oallan_workspace_bytes(n, nseries))));
-  CU_CHECK(cudaMemcpyAsync(dx.p, x, static_cast<size_t>(elems) * sizeof(double),
-                           cudaMemcpyHostToDevice, st.s));
-  const int rc = oallan_f64(hadamard, fs, n, nseries, dx.d(), inner, outer_stride, sample_stride,
-                            dav.d(), dtau.d(), ws.p, st.s);
-  if (rc != B2INS_OK) return rc;
-  CU_CHECK(cudaMemcpyAsync(avar, dav.p, static_cast<size_t>(nseries) * ntau * sizeof(double),
-                           cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaMemcpyAsync(tau, dtau.p, static_cast<size_t>(ntau) * sizeof(double),
-                           cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
-}
-
 int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
                      int64_t outer_stride, int64_t sample_stride, double* avar, double* tau,
                      void* workspace, void* stream) {
@@ -1510,7 +1497,8 @@ int b2ins_oallan_f64(double fs, int64_t n, int64_t nseries, const double* x, int
 
 int b2ins_oallan_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
                           int64_t outer_stride, int64_t sample_stride, double* avar, double* tau) {
-  return oallan_f64_host(false, fs, n, nseries, x, inner, outer_stride, sample_stride, avar, tau);
+  return variance_host(b2ins_oallan_f64, b2ins_oallan_workspace_bytes, fs, n, nseries, x, inner, outer_stride,
+                       sample_stride, avar, tau);
 }
 
 int b2ins_ohadamard_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
@@ -1521,7 +1509,8 @@ int b2ins_ohadamard_f64(double fs, int64_t n, int64_t nseries, const double* x, 
 
 int b2ins_ohadamard_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner,
                              int64_t outer_stride, int64_t sample_stride, double* hvar, double* tau) {
-  return oallan_f64_host(true, fs, n, nseries, x, inner, outer_stride, sample_stride, hvar, tau);
+  return variance_host(b2ins_ohadamard_f64, b2ins_oallan_workspace_bytes, fs, n, nseries, x, inner, outer_stride,
+                       sample_stride, hvar, tau);
 }
 
 // ---------------------------------------------------------------- K5 --------
@@ -1556,19 +1545,29 @@ int64_t b2ins_welch_workspace_bytes(int64_t n, int64_t nseries, int64_t nperseg,
   return welch_partial_offset(w) + parts;
 }
 
-int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner, int64_t outer_stride,
-                    int64_t sample_stride, int64_t nperseg, int64_t noverlap, const double* window, double* psd,
-                    double* freq, void* workspace, void* stream) {
+// K11's checks, shared by the device entry and its host wrapper.  K11 words its own rate and length rules, so
+// the common series check comes after them and only its stride rule can still fail there.
+static int welch_check(double fs, int64_t n, int64_t nseries, int64_t inner, int64_t outer_stride,
+                       int64_t sample_stride, int64_t nperseg, int64_t noverlap, WelchPlan* w) {
   ARG_CHECK(fs > 0.0 && std::isfinite(fs) && nseries >= 0, "bad fs/nseries");
-  ARG_CHECK(inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad strides");
   ARG_CHECK(noverlap >= 0 && noverlap < nperseg, "need 0 <= noverlap < nperseg, got noverlap=%lld, nperseg=%lld",
             static_cast<long long>(noverlap), static_cast<long long>(nperseg));
   ARG_CHECK(n >= nperseg, "a series of %lld samples is shorter than nperseg=%lld", static_cast<long long>(n),
             static_cast<long long>(nperseg));
-  WelchPlan w;
-  ARG_CHECK(welch_plan(n, nperseg, noverlap, &w),
+  const int chk = series_check(fs, n, nseries, inner, outer_stride, sample_stride);
+  if (chk != B2INS_OK) return chk;
+  ARG_CHECK(welch_plan(n, nperseg, noverlap, w),
             "nperseg=%lld: need an even length >= 16, a power of two up to 16384 or at most 8192",
             static_cast<long long>(nperseg));
+  return B2INS_OK;
+}
+
+int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner, int64_t outer_stride,
+                    int64_t sample_stride, int64_t nperseg, int64_t noverlap, const double* window, double* psd,
+                    double* freq, void* workspace, void* stream) {
+  WelchPlan w;
+  const int chk = welch_check(fs, n, nseries, inner, outer_stride, sample_stride, nperseg, noverlap, &w);
+  if (chk != B2INS_OK) return chk;
   ARG_CHECK(window && freq && workspace && (nseries == 0 || (x && psd)), "null buffer");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   WelchParams p;
@@ -1637,35 +1636,21 @@ int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x, int6
 int b2ins_welch_f64_host(double fs, int64_t n, int64_t nseries, const double* x, int64_t inner, int64_t outer_stride,
                          int64_t sample_stride, int64_t nperseg, int64_t noverlap, const double* window, double* psd,
                          double* freq) {
-  ARG_CHECK(nseries >= 0 && inner >= 1 && sample_stride >= 1 && outer_stride >= 0, "bad nseries/strides");
-  const int64_t wsb = b2ins_welch_workspace_bytes(n, nseries, nperseg, noverlap);
-  ARG_CHECK(wsb >= 0, "bad n/nperseg/noverlap (n=%lld, nperseg=%lld, noverlap=%lld)", static_cast<long long>(n),
-            static_cast<long long>(nperseg), static_cast<long long>(noverlap));
+  WelchPlan w;
+  const int chk = welch_check(fs, n, nseries, inner, outer_stride, sample_stride, nperseg, noverlap, &w);
+  if (chk != B2INS_OK) return chk;
   ARG_CHECK(window && freq && (nseries == 0 || (x && psd)), "null buffer");
   const int64_t L = nperseg / 2 + 1;
-  const int64_t outer = (nseries + inner - 1) / inner;
-  const int64_t elems = nseries == 0 ? 0 : (outer - 1) * outer_stride + (inner - 1) + (n - 1) * sample_stride + 1;
-  DevBuf dx, dw, dpsd, dfreq, ws;
-  Stream st;
-  CU_CHECK(st.create());
-  CU_CHECK(dx.alloc(static_cast<size_t>(elems > 0 ? elems : 1) * sizeof(double)));
-  CU_CHECK(dw.alloc(static_cast<size_t>(nperseg) * sizeof(double)));
-  CU_CHECK(dpsd.alloc(static_cast<size_t>(nseries > 0 ? nseries * L : 1) * sizeof(double)));
-  CU_CHECK(dfreq.alloc(static_cast<size_t>(L) * sizeof(double)));
-  CU_CHECK(ws.alloc(static_cast<size_t>(wsb)));
-  if (elems > 0)
-    CU_CHECK(cudaMemcpyAsync(dx.p, x, static_cast<size_t>(elems) * sizeof(double), cudaMemcpyHostToDevice, st.s));
-  CU_CHECK(cudaMemcpyAsync(dw.p, window, static_cast<size_t>(nperseg) * sizeof(double), cudaMemcpyHostToDevice,
-                           st.s));
-  const int rc = b2ins_welch_f64(fs, n, nseries, dx.d(), inner, outer_stride, sample_stride, nperseg, noverlap,
-                                 dw.d(), dpsd.d(), dfreq.d(), ws.p, st.s);
-  if (rc != B2INS_OK) return rc;
-  if (nseries > 0)
-    CU_CHECK(cudaMemcpyAsync(psd, dpsd.p, static_cast<size_t>(nseries * L) * sizeof(double), cudaMemcpyDeviceToHost,
-                             st.s));
-  CU_CHECK(cudaMemcpyAsync(freq, dfreq.p, static_cast<size_t>(L) * sizeof(double), cudaMemcpyDeviceToHost, st.s));
-  CU_CHECK(cudaStreamSynchronize(st.s));
-  return B2INS_OK;
+  Staging st;
+  const double* dx = st.in(x, series_elems(n, nseries, inner, outer_stride, sample_stride));
+  const double* dw = st.in(window, nperseg);
+  double* dpsd = st.out(psd, nseries * L);
+  double* dfreq = st.out(freq, L);
+  void* ws = st.scratch(b2ins_welch_workspace_bytes(n, nseries, nperseg, noverlap));
+  return st.run([&](cudaStream_t s) {
+    return b2ins_welch_f64(fs, n, nseries, dx, inner, outer_stride, sample_stride, nperseg, noverlap, dw, dpsd,
+                           dfreq, ws, s);
+  });
 }
 
 // ---------------------------------------------------------------- K1 plan ---

@@ -466,25 +466,37 @@ def allan_taus(n, fs):
     return np.asarray(allan_num_tau(n, fs), dtype=np.float64) / float(fs)
 
 
+def _outer_stride(n, inner, outer_stride, sample_stride):
+    """outer_stride of the series addressing when the caller gives none: series after series (inner == 1), or
+    groups of `inner` interleaved series after one another."""
+    if outer_stride is not None:
+        return outer_stride
+    return n * sample_stride if inner == 1 else n * inner
+
+
+def _variance(symbol, workspace_symbol, fs, x, n, nseries, inner, outer_stride, sample_stride):
+    """K4 or K4o's two forms through the C ABI entry `symbol`: var [nseries, ntau], tau [ntau] (CUDA)."""
+    _require_cuda()
+    lib = _lib.load()
+    outer_stride = _outer_stride(n, inner, outer_stride, sample_stride)
+    ntau = len(allan_num_tau(n, fs))
+    var = torch.zeros((nseries, ntau), dtype=torch.float64, device=x.device)
+    tau = torch.zeros((ntau,), dtype=torch.float64, device=x.device)
+    if ntau == 0 or nseries == 0:
+        return var, tau
+    ws = torch.empty(getattr(lib, workspace_symbol)(int(n), int(nseries)) // 8 + 1, dtype=torch.float64,
+                     device=x.device)
+    _lib.check(getattr(lib, symbol)(float(fs), int(n), int(nseries), _ptr(x), int(inner), int(outer_stride),
+                                    int(sample_stride), _ptr(var), _ptr(tau), _ptr(ws), _stream()))
+    return var, tau
+
+
 def allan(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
     """K4.  x: CUDA f64 buffer holding `nseries` series of n samples; series s, sample t at
     x.flat[(s // inner) * outer_stride + (s % inner) + t * sample_stride].
     Returns avar [nseries, ntau], tau [ntau] (CUDA)."""
-    _require_cuda()
-    lib = _lib.load()
-    if outer_stride is None:
-        outer_stride = n * sample_stride if inner == 1 else n * inner
-    ntau = len(allan_num_tau(n, fs))
-    avar = torch.zeros((nseries, ntau), dtype=torch.float64, device=x.device)
-    tau = torch.zeros((ntau,), dtype=torch.float64, device=x.device)
-    if ntau == 0 or nseries == 0:
-        return avar, tau
-    ws = torch.empty(lib.b2ins_allan_workspace_bytes(n, nseries) // 8 + 1, dtype=torch.float64,
-                     device=x.device)
-    _lib.check(lib.b2ins_allan_f64(float(fs), int(n), int(nseries), _ptr(x), int(inner),
-                                   int(outer_stride), int(sample_stride), _ptr(avar), _ptr(tau),
-                                   _ptr(ws), _stream()))
-    return avar, tau
+    return _variance('b2ins_allan_f64', 'b2ins_allan_workspace_bytes', fs, x, n, nseries, inner, outer_stride,
+                     sample_stride)
 
 
 def oallan_workspace_bytes(n, nseries):
@@ -496,7 +508,8 @@ def oallan(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
     """K4o: overlapping Allan variance on K4's tau grid, same addressing and outputs as allan():
     avar_o(m) = 1/(2 m^2 M) sum_{k<M} (S(k+m, m) - S(k, m))^2, M = n - 2m + 1.
     Returns avar [nseries, ntau], tau [ntau] (CUDA)."""
-    return _k4o('b2ins_oallan_f64', fs, x, n, nseries, inner, outer_stride, sample_stride)
+    return _variance('b2ins_oallan_f64', 'b2ins_oallan_workspace_bytes', fs, x, n, nseries, inner, outer_stride,
+                     sample_stride)
 
 
 def ohadamard(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
@@ -504,23 +517,8 @@ def ohadamard(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
     as allan(): hvar(m) = 1/(6 m^2 H) sum_{k<H} (S(k+2m, m) - 2 S(k+m, m) + S(k, m))^2, H = n - 3m + 1.
     A linear drift of the samples cancels; white noise gives sigma^2 / m, as avar_o does.
     Returns hvar [nseries, ntau], tau [ntau] (CUDA)."""
-    return _k4o('b2ins_ohadamard_f64', fs, x, n, nseries, inner, outer_stride, sample_stride)
-
-
-def _k4o(symbol, fs, x, n, nseries, inner, outer_stride, sample_stride):
-    _require_cuda()
-    fn = getattr(_lib.load(), symbol)
-    if outer_stride is None:
-        outer_stride = n * sample_stride if inner == 1 else n * inner
-    ntau = len(allan_num_tau(n, fs))
-    var = torch.zeros((nseries, ntau), dtype=torch.float64, device=x.device)
-    tau = torch.zeros((ntau,), dtype=torch.float64, device=x.device)
-    if ntau == 0 or nseries == 0:
-        return var, tau
-    ws = torch.empty(oallan_workspace_bytes(n, nseries) // 8 + 1, dtype=torch.float64, device=x.device)
-    _lib.check(fn(float(fs), int(n), int(nseries), _ptr(x), int(inner), int(outer_stride), int(sample_stride),
-                  _ptr(var), _ptr(tau), _ptr(ws), _stream()))
-    return var, tau
+    return _variance('b2ins_ohadamard_f64', 'b2ins_oallan_workspace_bytes', fs, x, n, nseries, inner, outer_stride,
+                     sample_stride)
 
 
 def welch_workspace_bytes(n, nseries, nperseg, noverlap):
@@ -534,8 +532,7 @@ def welch(fs, x, n, nseries, nperseg, noverlap, window, inner=1, outer_stride=No
     one-sided, nfft = nperseg) of `nseries` series of n samples, addressed as in allan().  window: [nperseg]
     floats.  Returns psd [nseries, nperseg // 2 + 1], freq [nperseg // 2 + 1] (CUDA)."""
     _require_cuda()
-    if outer_stride is None:
-        outer_stride = n * sample_stride if inner == 1 else n * inner
+    outer_stride = _outer_stride(n, inner, outer_stride, sample_stride)
     L = int(nperseg) // 2 + 1
     w = to_device(window, x.device)
     if w.shape != (int(nperseg),):

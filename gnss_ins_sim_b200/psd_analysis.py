@@ -4,9 +4,10 @@ scipy.signal.welch; the estimator itself is csrc/welch_kernel.cuh (K11)."""
 import numpy as np
 
 from . import engine
+from .series_analysis import SeriesEstimator
 
 
-class Psd(object):
+class Psd(SeriesEstimator):
     '''
     One-sided power spectral density of the three accelerometer and three gyroscope channels by Welch's
     method, as scipy.signal.welch(x, fs, window, nperseg, noverlap) computes it (detrend='constant',
@@ -48,49 +49,20 @@ class Psd(object):
             if not np.all(np.isfinite(w)):
                 raise ValueError('window values must be finite')
         self.window = w
-        self.input = ['fs', 'accel', 'gyro']
-        self.output = ['algo_freq', 'psd_accel', 'psd_gyro']
-        self.batch = True
-        self.results = None
+        super().__init__(['algo_freq', 'psd_accel', 'psd_gyro'])
 
-    def run(self, set_of_input):
-        '''
-        set_of_input = [fs, accel (n,3), gyro (n,3)]
-        '''
-        fs = set_of_input[0]
-        freq, p_a, p_g = self.run_batch(fs, np.asarray(set_of_input[1])[None], np.asarray(set_of_input[2])[None])
-        self.results = [freq, p_a[0], p_g[0]]
-
-    def run_batch(self, fs, accel, gyro, to_host=True, channel_major=False):
-        '''
-        accel, gyro: [R, n, 3] (the reference's per-run arrays, read in place) or, channel_major, [R, 3, n].
-        Returns freq [L], psd_accel [R, L, 3], psd_gyro [R, L, 3], L = nperseg // 2 + 1.
-        '''
-        a = engine.to_device(accel)
-        g = engine.to_device(gyro)
-        w = engine.to_device(self.window, a.device)
-        out = []
-        for x in (a, g):
-            if channel_major:
-                R, _, n = x.shape
-                kw = {}
-            else:
-                R, n, _ = x.shape
-                kw = dict(inner=3, outer_stride=3 * n, sample_stride=3)
-            if n < self.nperseg:
-                raise ValueError('a series of %d samples is shorter than nperseg=%d' % (n, self.nperseg))
-            psd, freq = engine.welch(fs, x, n, R * 3, self.nperseg, self.noverlap, w, **kw)
-            out.append(psd.reshape(R, 3, -1).permute(0, 2, 1).contiguous())
-        if to_host:
-            return freq.cpu().numpy(), out[0].cpu().numpy(), out[1].cpu().numpy()
-        return freq, out[0], out[1]
+    def _series(self, fs, x, n, nseries, **addressing):
+        if n < self.nperseg:
+            raise ValueError('a series of %d samples is shorter than nperseg=%d' % (n, self.nperseg))
+        return engine.welch(fs, x, n, nseries, self.nperseg, self.noverlap, self.window, **addressing)
 
     def frequencies(self, fs):
         '''freq [L] of run_batch for sample rate fs: k / (nperseg (1/fs)), as np.fft.rfftfreq.'''
         return np.arange(self.nperseg // 2 + 1) * (1.0 / (self.nperseg * (1.0 / fs)))
 
-    def get_results(self):
-        return self.results
+    def abscissa(self, n, fs):
+        return self.frequencies(fs)
 
-    def reset(self):
-        pass
+    def run_bytes(self, n):
+        # K1's 48 B per run-sample, then K11's chunk sums for the six series of a run
+        return 48 + max(engine.welch_workspace_bytes(n, 6, self.nperseg, self.noverlap), 0) / n

@@ -38,8 +38,7 @@ import torch
 from . import engine, dist, logged
 from .free_integration import FreeIntegration
 from .free_integration_odo import FreeIntegration as FreeIntegrationOdo
-from .allan_analysis import Allan
-from .psd_analysis import Psd
+from .series_analysis import SeriesEstimator
 from .ins_loose import InsLoose, gps_sample_index
 from .mag_calibrate import MagCal, check_segments
 
@@ -495,7 +494,7 @@ class Sim(object):
             for i, a in enumerate(self.algo):
                 if isinstance(a, FreeIntegration):     # incl. the odometer variant
                     self._run_free_integration(i, a)
-                elif isinstance(a, (Allan, Psd)):
+                elif isinstance(a, SeriesEstimator):
                     self._run_allan(i, a)
                 elif isinstance(a, InsLoose):
                     self._run_ins_loose(i, a)
@@ -560,7 +559,7 @@ class Sim(object):
                         pos[:, -1] - d['ref_pos'][-1], vel[:, -1] - d['ref_vel'][-1]], axis=1)
                     self._mc[i]['end_err'] = err
                     self.err_stats[name] = engine.error_stats(engine.to_device(err)).cpu().numpy()
-            elif isinstance(a, (Allan, Psd)):
+            elif isinstance(a, SeriesEstimator):
                 self._publish_allan(name, a, *a.run_batch(self.fs[0], self._logged_sets('accel'),
                                                           self._logged_sets('gyro')))
             elif isinstance(a, InsLoose):
@@ -823,20 +822,10 @@ class Sim(object):
         chunk sums beside the series; its abscissa is the frequency grid instead of tau."""
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
-        spectral = isinstance(algo, Psd)
-        overlapping = getattr(algo, 'overlapping', False)
-        fused = (not spectral and not overlapping and self._vib_acc is None and self._vib_gyro is None and n > 5040
+        fused = (algo.fused and self._vib_acc is None and self._vib_gyro is None and n > 5040
                  and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
-        tau = algo.frequencies(self.fs[0]) if spectral else engine.allan_taus(n, self.fs[0])
-        if fused:
-            block = self._allan_block(6 * 2, 2)
-        elif spectral:      # K1's 48 B per run-sample, then K11's chunk sums for the six series of a run
-            ws = engine.welch_workspace_bytes(n, 6, algo.nperseg, algo.noverlap)
-            block = self._allan_block(48 + max(ws, 0) / n, 3)
-        elif overlapping:   # K1's 48 B per run-sample, then K4o's workspace for one sensor's 3 series
-            block = self._allan_block(64 + engine.oallan_workspace_bytes(n, 3) / n, 3)
-        else:
-            block = self._allan_block(64, 3)
+        tau = algo.abscissa(n, self.fs[0])
+        block = self._allan_block(6 * 2, 2) if fused else self._allan_block(algo.run_bytes(n), 3)
         parts = []      # [runs, ntau, 6]: accel, gyro
         for r0 in range(lo, hi, block):
             r1 = min(hi, r0 + block)

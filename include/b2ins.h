@@ -427,6 +427,7 @@ int b2ins_error_stats_exchange_f64(int64_t runs, int ncomp, const double* err, i
  * Replaces allan.allan_var (allan/allan.py:18-59) for `nseries` series at once.
  * Series s, sample t lives at x[s / inner * outer_stride + (s % inner) + t * sample_stride]
  * (RUN_MAJOR accel [R][n][3]: inner = 3, outer_stride = 3n, sample_stride = 3).
+ * inner >= 1, sample_stride >= 1 and outer_stride >= 0, else B2INS_ERR_ARG (as for K4o and K11).
  * avar [nseries][ntau], tau [ntau], ntau = b2ins_allan_num_tau(n, fs).
  * workspace: device scratch of b2ins_allan_workspace_bytes(n, nseries) bytes. */
 int64_t b2ins_allan_workspace_bytes(int64_t n, int64_t nseries);

@@ -437,3 +437,160 @@ def test_lanes_per_run_choice():
     assert _lib.mc_shape(4, 0) == '6,1,0' and _lib.mc_shape(4, 1) == '6,2,0' and _lib.mc_shape(32) == '1,4,1'
     # every choice is a width the kernels are instantiated for
     assert all(pick(r, f) in (1, 2, 4, 8, 16, 32) for r in range(1, 60000, 997) for f in (0, 1))
+
+
+# ------------------------------------------------------------------ argument checks of the C ABI ---
+_PIN_BUF = 8192      # elements of every host buffer: larger than any nominal case below reads
+_PIN_KEEP = []       # the host buffers of the cases, alive while they run
+
+
+def _pin_calls():
+    """(case id, entry point, argument tuple) for every *_host entry point and the four series device
+    entries.  Host buffers are real (and large enough for the nominal sizes); device buffers are null, which
+    the device entries reject only after their other checks."""
+    from gnss_ins_sim_b200 import _lib
+    _PIN_KEEP[:] = [np.zeros(_PIN_BUF) for _ in range(8)]
+    h = [_lib.host_ptr(b) for b in _PIN_KEEP]
+    se = ctypes.byref(_lib.SensorErr())
+    vs = _lib.Vib()
+    vs.type = _lib.VIB_SERIES
+    seg_ok = (ctypes.c_int64 * 6)(0, 20, 20, 40, 40, 60)
+    seg_short = (ctypes.c_int64 * 6)(0, 20, 20, 22, 40, 60)
+    seg_out = (ctypes.c_int64 * 6)(0, 20, 20, 40, 40, 61)
+
+    def cfg(**kw):
+        c = _lib.McConfig()
+        c.ref_frame, c.fs, c.n, c.runs, c.ini_sets, c.ini_rows, c.stats_start = 1, 100.0, 10, 2, 1, 9, -1
+        for k, v in kw.items():
+            setattr(c, k, v)
+        return ctypes.byref(c)
+
+    calls = []
+
+    def add(entry, base, names, cases):
+        for cid, change in cases:
+            args = dict(zip(names, base))
+            args.update(change)
+            calls.append(('%s[%s]' % (entry, cid), 'b2ins_' + entry, tuple(args[k] for k in names)))
+
+    null_cases = lambda names: [('null_' + k, {k: None}) for k in names]     # noqa: E731
+    # K2
+    add('free_integration_f64_host', (1, 100.0, 2, 10, h[0], h[1], 0, h[2], 1, 9, 0, 1, h[3], h[4], h[5], 0),
+        ('rf', 'fs', 'runs', 'n', 'gyro', 'accel', 'layout', 'ini', 'sets', 'rows', 'off', 'er', 'att', 'pos',
+         'vel', 'lanes'),
+        [('valid', {}), ('runs_neg', {'runs': -1}), ('n_neg', {'n': -1}), ('runs_0', {'runs': 0}),
+         ('n_0', {'n': 0}), ('sets_0', {'sets': 0}), ('rows_8', {'rows': 8}), ('rows_11', {'rows': 11})]
+        + null_cases(('gyro', 'accel', 'ini', 'att', 'pos', 'vel')))
+    # K1
+    add('imu_noise_f64_host', (100.0, 2, 10, h[0], h[1], se, se, None, None, 7, 0, 0, h[2], h[3], None),
+        ('fs', 'runs', 'n', 'rg', 'ra', 'ge', 'ae', 'vg', 'va', 'seed', 'off', 'layout', 'gyro', 'accel', 'z'),
+        [('valid', {}), ('valid_z_dump', {'z': h[4]}), ('runs_neg', {'runs': -1}), ('n_neg', {'n': -1}),
+         ('runs_0', {'runs': 0}), ('n_0', {'n': 0}), ('vib_series_gyro', {'vg': ctypes.byref(vs)}),
+         ('vib_series_accel', {'va': ctypes.byref(vs)})] + null_cases(('rg', 'ra', 'gyro', 'accel')))
+    # K10
+    add('magcal_fed_f64_host', (2, 60, seg_ok, h[0], 180, 3, h[1], h[2], None),
+        ('runs', 'n', 'seg', 'mag', 'rs', 'ss', 'si', 'hi', 'cal'),
+        [('valid', {}), ('valid_cal', {'cal': h[3]}), ('runs_neg', {'runs': -1}), ('n_neg', {'n': -1}),
+         ('runs_0', {'runs': 0}), ('runs_2e31', {'runs': 1 << 31}), ('n_2e32', {'n': 1 << 32}),
+         ('seg_null', {'seg': None}), ('seg_short', {'seg': seg_short}), ('seg_out', {'seg': seg_out}),
+         ('run_stride_neg', {'rs': -1}), ('sample_stride_2', {'ss': 2})] + null_cases(('mag', 'si', 'hi')))
+    # K12
+    add('mc_free_integration_f64_host', (cfg(), h[0], h[1], h[2], h[3], None, h[4]),
+        ('cfg', 'rg', 'ra', 'rn', 'ini', 'end_err', 'stats'),
+        [('valid', {}), ('valid_end_err', {'end_err': h[5]}), ('cfg_null', {'cfg': None}),
+         ('runs_0', {'cfg': cfg(runs=0)}), ('n_0', {'cfg': cfg(n=0)}), ('runs_neg', {'cfg': cfg(runs=-1)}),
+         ('sets_0', {'cfg': cfg(ini_sets=0)}), ('rows_8', {'cfg': cfg(ini_rows=8)}),
+         ('vib_series', {'cfg': cfg(vib_gyro=vs)})] + null_cases(('rg', 'ra', 'rn', 'ini', 'stats')))
+    # K4, K4o and K4o's Hadamard form: interleaved [3, 2000] accel of one run (n = 2000 at 100 Hz: 20 tau)
+    series = [('valid', {}), ('fs_0', {'fs': 0.0}), ('fs_neg', {'fs': -1.0}), ('n_neg', {'n': -1}),
+              ('nseries_neg', {'ns': -1}), ('inner_0', {'inner': 0}), ('sample_stride_0', {'ss': 0}),
+              ('outer_stride_neg', {'os': -1}), ('n_short', {'n': 800}), ('n_0', {'n': 0}), ('nseries_0', {'ns': 0})]
+    names = ('fs', 'n', 'ns', 'x', 'inner', 'os', 'ss', 'var', 'tau')
+    for e in ('allan', 'oallan', 'ohadamard'):
+        add(e + '_f64_host', (100.0, 2000, 3, h[0], 3, 6000, 3, h[1], h[2]), names,
+            series + null_cases(('x', 'var', 'tau')))
+        add(e + '_f64', (100.0, 2000, 3, None, 3, 6000, 3, None, None, None, None), names + ('ws', 'stream'),
+            series[1:] + [('null_device', {})])
+    # K11
+    names = ('fs', 'n', 'ns', 'x', 'inner', 'os', 'ss', 'nperseg', 'noverlap', 'win', 'psd', 'freq')
+    welch = [('nseries_neg', {'ns': -1}), ('inner_0', {'inner': 0}), ('sample_stride_0', {'ss': 0}),
+             ('outer_stride_neg', {'os': -1}), ('noverlap_neg', {'noverlap': -1}),
+             ('noverlap_nperseg', {'noverlap': 256}), ('nperseg_15', {'nperseg': 15, 'noverlap': 7}),
+             ('nperseg_8', {'nperseg': 8, 'noverlap': 4}), ('nperseg_9000', {'nperseg': 9000, 'noverlap': 0, 'n': 9000}),
+             ('n_short', {'n': 255}), ('n_neg', {'n': -1})]
+    add('welch_f64_host', (100.0, 2000, 3, h[0], 3, 6000, 3, 256, 128, h[1], h[2], h[3]), names,
+        [('valid', {}), ('valid_nseries_0', {'ns': 0, 'x': None, 'psd': None})] + welch
+        + null_cases(('x', 'win', 'psd', 'freq')))
+    add('welch_f64', (100.0, 2000, 3, None, 3, 6000, 3, 256, 128, None, None, None, None, None),
+        names + ('ws', 'stream'),
+        [('fs_0', {'fs': 0.0}), ('fs_inf', {'fs': float('inf')}), ('fs_nan', {'fs': float('nan')})] + welch
+        + [('null_device', {}), ('null_device_nseries_0', {'ns': 0})])
+    return calls
+
+
+_SERIES_PINS = {'fs_0': 'bad fs/n/nseries', 'fs_neg': 'bad fs/n/nseries', 'n_neg': 'bad fs/n/nseries',
+                'nseries_neg': 'bad fs/n/nseries', 'inner_0': 'bad strides', 'sample_stride_0': 'bad strides',
+                'outer_stride_neg': 'bad strides', 'n_short': None, 'n_0': None, 'nseries_0': None,
+                'null_x': 'null buffer', 'null_var': 'null buffer', 'null_tau': 'null buffer',
+                'null_device': 'null buffer'}
+_WELCH_PINS = {'fs_0': 'bad fs/nseries', 'fs_inf': 'bad fs/nseries', 'fs_nan': 'bad fs/nseries',
+               'nseries_neg': 'bad fs/nseries', 'inner_0': 'bad strides', 'sample_stride_0': 'bad strides',
+               'outer_stride_neg': 'bad strides',
+               'noverlap_neg': 'need 0 <= noverlap < nperseg, got noverlap=-1, nperseg=256',
+               'noverlap_nperseg': 'need 0 <= noverlap < nperseg, got noverlap=256, nperseg=256',
+               'nperseg_15': 'nperseg=15: need an even length >= 16, a power of two up to 16384 or at most 8192',
+               'nperseg_8': 'nperseg=8: need an even length >= 16, a power of two up to 16384 or at most 8192',
+               'nperseg_9000': 'nperseg=9000: need an even length >= 16, a power of two up to 16384 or at most 8192',
+               'n_short': 'a series of 255 samples is shorter than nperseg=256',
+               'n_neg': 'a series of -1 samples is shorter than nperseg=256',
+               'null_x': 'null buffer', 'null_win': 'null buffer', 'null_psd': 'null buffer', 'null_freq': 'null buffer',
+               'null_device': 'null buffer', 'null_device_nseries_0': 'null buffer'}
+_RUNS_N = 'runs and n must be non-negative'
+_INI = 'ini must be [sets>=1][9|10]'
+_VIB = 'VIB_SERIES takes a device pointer: use the device entry point'
+_SEG = 'segment %d [%d, %d) must hold at least 3 rows inside [0, 60)'
+_PINS = {
+    'free_integration_f64_host': dict({'runs_neg': _RUNS_N, 'n_neg': _RUNS_N, 'runs_0': None, 'n_0': None,
+                                       'sets_0': _INI, 'rows_8': _INI, 'rows_11': _INI},
+                                      **{'null_' + k: 'null buffer' for k in ('gyro', 'accel', 'ini', 'att', 'pos', 'vel')}),
+    'imu_noise_f64_host': dict({'runs_neg': _RUNS_N, 'n_neg': _RUNS_N, 'runs_0': None, 'n_0': None,
+                                'vib_series_gyro': _VIB, 'vib_series_accel': _VIB},
+                               **{'null_' + k: 'null buffer' for k in ('rg', 'ra', 'gyro', 'accel')}),
+    'magcal_fed_f64_host': dict({'runs_neg': _RUNS_N, 'n_neg': _RUNS_N, 'runs_0': None,
+                                 'runs_2e31': 'runs must be < 2^31', 'n_2e32': 'n must be < 2^32',
+                                 'seg_null': 'null segments', 'seg_short': _SEG % (1, 20, 22),
+                                 'seg_out': _SEG % (2, 40, 61),
+                                 'run_stride_neg': 'run_stride must be >= 0 and sample_stride >= 3',
+                                 'sample_stride_2': 'run_stride must be >= 0 and sample_stride >= 3'},
+                                **{'null_' + k: 'null buffer' for k in ('mag', 'si', 'hi')}),
+    'mc_free_integration_f64_host': dict({'cfg_null': 'cfg is null', 'runs_0': 'runs and n must be positive',
+                                          'n_0': 'runs and n must be positive',
+                                          'runs_neg': 'runs and n must be positive', 'sets_0': _INI,
+                                          'rows_8': _INI, 'vib_series': _VIB},
+                                         **{'null_' + k: 'null buffer' for k in ('rg', 'ra', 'rn', 'ini', 'stats')}),
+    'welch_f64_host': _WELCH_PINS, 'welch_f64': _WELCH_PINS,
+}
+for _e in ('allan', 'oallan', 'ohadamard'):
+    _PINS[_e + '_f64_host'] = _PINS[_e + '_f64'] = _SERIES_PINS
+
+
+def test_c_abi_argument_checks_are_pinned():
+    """Every *_host entry point and the four series device entries: each bad argument gives B2INS_ERR_ARG and
+    the same b2ins_last_error() text, decided before any CUDA call; a call with nothing to compute (no runs, no
+    samples, no series, a series too short for one tau) returns B2INS_OK before any CUDA call; valid arguments
+    reach CUDA (B2INS_ERR_CUDA without a device).  None in the tables marks an early B2INS_OK."""
+    from gnss_ins_sim_b200 import _lib
+    lib = _lib.load()
+    has_device = lib.b2ins_device_count() > 0
+    for cid, fn, args in _pin_calls():
+        entry, case = cid[:-1].split('[')
+        if case.startswith('valid'):
+            if not has_device:
+                assert getattr(lib, fn)(*args) == _lib.ERR_CUDA, cid
+            continue
+        want = _PINS[entry][case]
+        rc = getattr(lib, fn)(*args)
+        if want is None:
+            assert rc == _lib.OK, (cid, rc, lib.b2ins_last_error())
+        else:
+            assert (rc, lib.b2ins_last_error().decode()) == (_lib.ERR_ARG, want), cid

@@ -334,6 +334,48 @@ def test_host_entry_points(eng):
     avar, tau = np.empty(38), np.empty(38)
     _lib.check(lib.b2ins_allan_f64_host(100.0, x.size, 1, hp(x), 1, x.size, 1, hp(avar), hp(tau)))
     assert_close(avar, ga['avar'], 1e-9, 0.0, 'avar')
+    # K1 with the Gaussian draws dumped: bit for bit the device entry
+    zo = np.empty((R, n, 12))
+    _lib.check(lib.b2ins_imu_noise_f64_host(100.0, R, n, hp(rg), hp(ra), ctypes.byref(se_g), ctypes.byref(se_a),
+                                            None, None, int(g['seed']), 0, 0, hp(go), hp(ao), hp(zo)))
+    dg, da, dz = eng.imu_noise(100.0, R, _dev(rg), _dev(ra), ge, ae, int(g['seed']), dump_z=True)
+    for host, dev in ((go, dg), (ao, da), (zo, dz)):
+        assert np.array_equal(host, dev.cpu().numpy())
+    # K10 on supplied samples, mag_cal not requested
+    rng = np.random.default_rng(5)
+    b0, ang = np.array([20.0, -5.0, 42.0]), np.linspace(0.0, 2.2 * np.pi, 400)
+    c, s = np.cos(ang), np.sin(ang)
+    rows = []
+    for i, j in ((1, 2), (2, 0), (0, 1)):       # one rotation about each axis
+        b = np.tile(b0, (ang.size, 1))
+        b[:, i], b[:, j] = c * b0[i] + s * b0[j], -s * b0[i] + c * b0[j]
+        rows.append(b + 0.3 * rng.standard_normal(b.shape))
+    mag = np.ascontiguousarray(np.stack([np.concatenate(rows)] * 2))
+    seg = ((0, 400), (400, 800), (800, 1200))
+    si, hi = np.empty((2, 3, 3)), np.empty((2, 4))
+    _lib.check(lib.b2ins_magcal_fed_f64_host(2, 1200, (ctypes.c_int64 * 6)(*np.ravel(seg)), hp(mag), 3600, 3, hp(si),
+                                             hp(hi), None))
+    res = eng.mag_calibrate(seg, _dev(mag))
+    assert np.array_equal(si, res.soft_iron.cpu().numpy()) and np.array_equal(hi, res.hard_iron.cpu().numpy())
+    # K4o, its Hadamard form and K11 on interleaved [R, n, 3] runs that lie outer_stride > 3n apart
+    Rs, ns, pad, fs = 2, 6000, 7, 100.0
+    buf = np.zeros((Rs, 3 * ns + pad))
+    buf[:, :3 * ns] = (1e-4 * np.arange(3 * ns) + rng.standard_normal((Rs, 3 * ns)))
+    dbuf, os_ = _dev(buf), 3 * ns + pad
+    ntau = len(eng.allan_num_tau(ns, fs))
+    for entry, dev_fn in (('b2ins_oallan_f64_host', eng.oallan), ('b2ins_ohadamard_f64_host', eng.ohadamard)):
+        var, tau = np.empty((3 * Rs, ntau)), np.empty(ntau)
+        _lib.check(getattr(lib, entry)(fs, ns, 3 * Rs, hp(buf), 3, os_, 3, hp(var), hp(tau)))
+        dvar, dtau = dev_fn(fs, dbuf, ns, 3 * Rs, inner=3, outer_stride=os_, sample_stride=3)
+        assert np.array_equal(var, dvar.cpu().numpy()) and np.array_equal(tau, dtau.cpu().numpy()), entry
+    win = 0.5 - 0.5 * np.cos(2.0 * np.pi * np.arange(256) / 256)
+    psd, freq = np.empty((3 * Rs, 129)), np.empty(129)
+    _lib.check(lib.b2ins_welch_f64_host(fs, ns, 3 * Rs, hp(buf), 3, os_, 3, 256, 128, hp(win), hp(psd), hp(freq)))
+    dpsd, dfreq = eng.welch(fs, dbuf, ns, 3 * Rs, 256, 128, win, inner=3, outer_stride=os_, sample_stride=3)
+    assert np.array_equal(psd, dpsd.cpu().numpy()) and np.array_equal(freq, dfreq.cpu().numpy())
+    freq0 = np.full(129, np.nan)          # no series: the frequency grid only
+    _lib.check(lib.b2ins_welch_f64_host(fs, ns, 0, None, 3, os_, 3, 256, 128, hp(win), None, hp(freq0)))
+    assert np.array_equal(freq0, freq)
 
 
 def test_argument_errors(eng):
