@@ -107,6 +107,8 @@ SIGNATURES = {
     'b2ins_oallan_f64_host': (_I, [_D, _L, _L, _P, _L, _L, _L, _P, _P]),
     'b2ins_ohadamard_f64': (_I, [_D, _L, _L, _P, _L, _L, _L, _P, _P, _P, _P]),
     'b2ins_ohadamard_f64_host': (_I, [_D, _L, _L, _P, _L, _L, _L, _P, _P]),
+    'b2ins_allan_fit_f64': (_I, [_D, _L, _L, _P, _L, _L, _P, _P]),
+    'b2ins_allan_fit_f64_host': (_I, [_D, _L, _L, _P, _L, _L, _P]),
     'b2ins_psd_series_len': (_I, [_L]),
     'b2ins_psd_workspace_bytes': (_L, [_L, _L]),
     'b2ins_psd_series_f64': (_I, [_D, _L, _L, _I, _I, _P, _P, _U64, _L, _P, _P, _P]),

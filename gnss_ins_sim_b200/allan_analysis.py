@@ -1,7 +1,8 @@
 """Allan plugin -- device-backed mirror of demo_algorithms/allan_analysis.py:15-61
 (input ['fs','accel','gyro'], output ['algo_time','ad_accel','ad_gyro']); the variance
 itself is csrc/allan_kernel.cuh (K4, allan.allan_var allan.py:18-59) or, overlapping,
-csrc/oallan_kernel.cuh (K4o).  Hadamard: the overlapping Hadamard deviation on the same
+csrc/oallan_kernel.cuh (K4o); fit=True adds the IEEE Std 952 noise terms of every curve
+(csrc/allanfit_kernel.cuh, K13) as ['noise_accel','noise_gyro'].  Hadamard: the overlapping Hadamard deviation on the same
 tau grid (K4o's Hadamard form), output ['algo_time','hd_accel','hd_gyro']."""
 import numpy as np
 import torch
@@ -22,13 +23,30 @@ class Allan(SeriesEstimator):
     with S(k, m) the sum of the m samples from k.  It has many more degrees of freedom at long tau,
     where bias instability and rate random walk are read.  Both use the same tau grid
     (m = j*10^k <= n/9), so the two curves can be laid over each other.
+
+    fit=True also identifies the IEEE Std 952-1997 noise terms of every curve on the device (engine.allan_fit,
+    K13), from the variance before its square root: outputs noise_accel and noise_gyro, [R, 3, 6] from run_batch
+    and [3, 6] per run, rows the axes x, y, z and columns
+        Q      quantisation                      rad            (accel m/s)
+        N      angle / velocity random walk      rad/s/sqrt(Hz) (m/s^2/sqrt(Hz)), the IMU model's arw / vrw
+        B      bias instability                  rad/s          (m/s^2)
+        K      rate random walk                  rad/s^2/sqrt(Hz) (m/s^3/sqrt(Hz))
+        R      rate ramp                         rad/s^2        (m/s^3)
+        B_min  minimum deviation / 0.664         rad/s          (m/s^2), the datasheet bias-instability figure.
+    The fit is the weighted non-negative least-squares fit of sigma^2 = sum_p C_p tau^p (p = -2..2) with relative
+    residuals, each bin weighted by floor(n / m) - 1, the number of squared differences allan_var averages there.
+    The overlapping curve is fitted with the same weights: it has more degrees of freedom than that at long tau,
+    so for it the weights are a conservative proxy, not its degrees of freedom.
     '''
 
-    def __init__(self, overlapping=False):
+    def __init__(self, overlapping=False, fit=False):
         if not isinstance(overlapping, (bool, np.bool_)):
             raise TypeError('overlapping must be True or False, got %r' % (overlapping,))
-        super().__init__(['algo_time', 'ad_accel', 'ad_gyro'])
+        if not isinstance(fit, (bool, np.bool_)):
+            raise TypeError('fit must be True or False, got %r' % (fit,))
+        super().__init__(['algo_time', 'ad_accel', 'ad_gyro'] + (['noise_accel', 'noise_gyro'] if fit else []))
         self.overlapping = bool(overlapping)
+        self.fit = bool(fit)
 
     @property
     def fused(self):
@@ -36,6 +54,8 @@ class Allan(SeriesEstimator):
 
     def _series(self, fs, x, n, nseries, **addressing):
         var, tau = self._variance()(fs, x, n, nseries, **addressing)
+        if self.fit:
+            return torch.sqrt(var), tau, engine.allan_fit(fs, n, var)
         return torch.sqrt(var), tau     # the DEVIATION, as allan_analysis.py:47-49
 
     def _variance(self):

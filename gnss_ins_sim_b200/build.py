@@ -27,7 +27,7 @@ LIB = os.environ.get('B2INS_LIB') or os.path.join(CSRC, 'libb2ins.so')
 UNITS = ['b2ins_api.cu', 'mc_plain_rf0.cu', 'mc_plain_rf1.cu', 'mc_spec_rf0.cu', 'mc_spec_rf1.cu']
 DEPS = UNITS + ['internal.h', 'mc_plain_launch.cuh', 'mc_spec_launch.cuh', 'common.cuh', 'fastmath64.cuh',
                 'mech.cuh', 'mc_kernel.cuh', 'mc_spec_kernel.cuh', 'mc_av_kernel.cuh', 'noise_kernel.cuh', 'stats_kernel.cuh',
-                'allan_kernel.cuh', 'oallan_kernel.cuh', 'psd_kernel.cuh', 'welch_kernel.cuh', 'gps_kernel.cuh', 'mag_kernel.cuh', 'magcal_kernel.cuh',
+                'allan_kernel.cuh', 'allanfit_kernel.cuh', 'oallan_kernel.cuh', 'psd_kernel.cuh', 'welch_kernel.cuh', 'gps_kernel.cuh', 'mag_kernel.cuh', 'magcal_kernel.cuh',
                 'sensor_stats_kernel.cuh',
                 'ekf_kernel.cuh', 'pathgen_host.h',
                 os.path.join('..', '..', 'include', 'b2ins.h')]

@@ -22,6 +22,7 @@
 #include "ekf_kernel.cuh"
 #include "stats_kernel.cuh"
 #include "sensor_stats_kernel.cuh"
+#include "allanfit_kernel.cuh"
 
 #ifdef B2INS_SINGLE_TU
 #define B2_RF 0
@@ -1511,6 +1512,62 @@ int b2ins_ohadamard_f64_host(double fs, int64_t n, int64_t nseries, const double
                              int64_t outer_stride, int64_t sample_stride, double* hvar, double* tau) {
   return variance_host(b2ins_ohadamard_f64, b2ins_oallan_workspace_bytes, fs, n, nseries, x, inner, outer_stride,
                        sample_stride, hvar, tau);
+}
+
+// ---------------------------------------------------------------- K13 -------
+// K13's checks, shared by the device entry and its host wrapper; nseries = 0 is left to the caller.  The grid
+// and the weights go to *p, from (n, fs) by K4's own grid function.
+static int allan_fit_check(double fs, int64_t n, int64_t nseries, int64_t series_stride, int64_t bin_stride,
+                           AllanFitParams* p) {
+  ARG_CHECK(fs > 0.0 && std::isfinite(fs) && n >= 0 && nseries >= 0, "bad fs/n/nseries");
+  ARG_CHECK(series_stride >= 0 && bin_stride >= 1, "bad strides");
+  ARG_CHECK(nseries / kFitWarps + (nseries % kFitWarps != 0) <= INT32_MAX, "too many series for one call");
+  int64_t mult[kFitMaxBins];
+  const int ntau = b2ins_allan_num_tau(n, fs, mult, kFitMaxBins);
+  ARG_CHECK(ntau <= kFitMaxBins, "too many tau");
+  p->ntau = ntau;
+  for (int k = 0; k < ntau; ++k) {
+    p->tau[k] = static_cast<double>(mult[k]) * (1.0 / fs);
+    p->w[k] = static_cast<double>(n / mult[k] - 1);
+  }
+  return B2INS_OK;
+}
+
+int b2ins_allan_fit_f64(double fs, int64_t n, int64_t nseries, const double* var, int64_t series_stride,
+                        int64_t bin_stride, double* out, void* stream) {
+  AllanFitParams p;
+  std::memset(&p, 0, sizeof(p));
+  const int chk = allan_fit_check(fs, n, nseries, series_stride, bin_stride, &p);
+  if (chk != B2INS_OK) return chk;
+  if (nseries == 0) return B2INS_OK;
+  ARG_CHECK(out && (var || p.ntau == 0), "null buffer");
+  p.var = var;
+  p.out = out;
+  p.nseries = nseries;
+  p.series_stride = series_stride;
+  p.bin_stride = bin_stride;
+  p.b_scale = std::sqrt(kPi / (2.0 * std::log(2.0)));
+  p.nan = std::numeric_limits<double>::quiet_NaN();
+  const int64_t ctas = (nseries + kFitWarps - 1) / kFitWarps;
+  allan_fit_kernel<<<static_cast<unsigned>(ctas), kFitWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
+int b2ins_allan_fit_f64_host(double fs, int64_t n, int64_t nseries, const double* var, int64_t series_stride,
+                             int64_t bin_stride, double* out) {
+  AllanFitParams p;
+  const int chk = allan_fit_check(fs, n, nseries, series_stride, bin_stride, &p);
+  if (chk != B2INS_OK) return chk;
+  if (nseries == 0) return B2INS_OK;
+  ARG_CHECK(out && (var || p.ntau == 0), "null buffer");
+  Staging st;
+  const double* dv =
+      p.ntau == 0 ? nullptr : st.in(var, (nseries - 1) * series_stride + (p.ntau - 1) * bin_stride + 1);
+  double* dout = st.out(out, nseries * 6);
+  return st.run([&](cudaStream_t s) {
+    return b2ins_allan_fit_f64(fs, n, nseries, dv, series_stride, bin_stride, dout, s);
+  });
 }
 
 // ---------------------------------------------------------------- K5 --------

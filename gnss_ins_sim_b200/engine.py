@@ -521,6 +521,28 @@ def ohadamard(fs, x, n, nseries, inner=1, outer_stride=None, sample_stride=1):
                      sample_stride)
 
 
+def allan_fit(fs, n, var, series_stride=None, bin_stride=1, nseries=None):
+    """K13: the IEEE Std 952 noise coefficients of Allan variance curves on the grid of n samples at fs, as
+    allan / oallan / allan_mc return them (the variance, read in place).  var: CUDA f64, curve s, bin k at
+    var.flat[s * series_stride + k * bin_stride] (series_stride None: ntau, so [nseries, ntau] and [runs, 6, ntau]
+    are read as they are); nseries None: var.numel() // ntau (with ntau = 0: the product of var's leading
+    dimensions).  Returns [nseries, 6] (CUDA): Q, N, B, K, R and B_min (include/b2ins.h, DESIGN.md section 3.13).
+    Asynchronous on the current stream."""
+    _require_cuda()
+    ntau = len(allan_num_tau(n, fs))
+    if nseries is None:
+        nseries = var.numel() // ntau if ntau else int(np.prod(var.shape[:-1]))
+    nseries = int(nseries)
+    series_stride = ntau if series_stride is None else int(series_stride)
+    if nseries and ntau and (nseries - 1) * series_stride + (ntau - 1) * int(bin_stride) >= var.numel():
+        raise ValueError('%d curves of %d bins with strides (%d, %d) do not fit in %d values'
+                         % (nseries, ntau, series_stride, bin_stride, var.numel()))
+    out = torch.empty((nseries, 6), dtype=torch.float64, device=var.device)
+    _lib.check(_lib.load().b2ins_allan_fit_f64(float(fs), int(n), nseries, _ptr(var) if ntau else None,
+                                               int(series_stride), int(bin_stride), _ptr(out), _stream()))
+    return out
+
+
 def welch_workspace_bytes(n, nseries, nperseg, noverlap):
     """Device scratch of engine.welch; negative if nperseg is not a length K11 transforms (or noverlap and n
     give no segment)."""

@@ -140,6 +140,9 @@ def read_data_dir(path, ref_frame):
 # ---- writing: Sim_data.save_to_file (sim_data.py:117-165) -----------------------------------------
 # name -> (column legends, internal units, units written to the file)
 _ANG3, _DEG3 = ['rad'] * 3, ['deg'] * 3
+_NOISE = ['Q', 'N', 'B', 'K', 'R', 'B_min']
+_NOISE_GYRO = ['rad', 'rad/s/sqrt(Hz)', 'rad/s', 'rad/s^2/sqrt(Hz)', 'rad/s^2', 'rad/s']
+_NOISE_ACCEL = ['m/s', 'm/s^2/sqrt(Hz)', 'm/s^2', 'm/s^3/sqrt(Hz)', 'm/s^3', 'm/s^2']
 OUTPUT_FORMAT = {
     'time': (['time'], ['sec'], ['sec']),
     'gps_time': (['gps_time'], ['sec'], ['sec']),
@@ -172,6 +175,9 @@ OUTPUT_FORMAT = {
     'algo_freq': (['algo_freq'], ['Hz'], ['Hz']),
     'psd_accel': (['PSD_accel_x', 'PSD_accel_y', 'PSD_accel_z'], ['m^2/s^4/Hz'] * 3, ['m^2/s^4/Hz'] * 3),
     'psd_gyro': (['PSD_gyro_x', 'PSD_gyro_y', 'PSD_gyro_z'], ['rad^2/s^2/Hz'] * 3, ['rad^2/s^2/Hz'] * 3),
+    # Allan(fit=True): one row per axis (x, y, z), the IEEE Std 952 terms in SI units, written as they are
+    'noise_gyro': (_NOISE, _NOISE_GYRO, _NOISE_GYRO),
+    'noise_accel': (_NOISE, _NOISE_ACCEL, _NOISE_ACCEL),
 }
 
 

@@ -17,7 +17,8 @@ Dispatch on `algorithm`:
     process-error statistics) leave the device.  Per-run histories are materialised
     lazily: counter-based Philox makes any run reproducible in isolation, so
     get_data(['pos'])[0]['algo0_7'] re-runs just run 7 with history output on.
-  * gnss_ins_sim_b200 Allan            -> K1 (noise) + K4 (Allan variance) per run block.
+  * gnss_ins_sim_b200 Allan            -> K1 (noise) + K4 (Allan variance) per run block; fit=True adds
+                                         K13 (noise identification) on the device curves.
   * gnss_ins_sim_b200 Psd              -> K1 (noise) + K11 (Welch power spectral density) per run block.
   * gnss_ins_sim_b200 MagCal           -> K8's samples regenerated inside K10 (magnetometer calibration).
   * any other reference-style plugin   -> K1 generates gyro/accel (K8 the magnetometer of a
@@ -244,6 +245,19 @@ class _DataDict(dict):
 
     def get(self, key, default=None):
         return self[key] if key in self else default
+
+
+def _gather_allan(curves, noise, total):
+    """Every rank's Allan results in one gather: its curves [R_local, L, 6] and, with the fit, its noise terms
+    [R_local, 6, 6] (None without) go as rows [R_local, 6 L (+ 36)].  Returns ([total, L, 6], [total, 6, 6] or
+    None) in run order on every rank."""
+    R, L = curves.shape[0], curves.shape[1]
+    rows = curves.reshape(R, L * 6)
+    if noise is not None:
+        rows = np.concatenate([rows, noise.reshape(R, 36)], axis=1)
+    rows = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(rows)), total)
+    return (rows[:, :L * 6].reshape(total, L, 6),
+            None if noise is None else rows[:, L * 6:].reshape(total, 6, 6))
 
 
 def _keyed(name, per_run):
@@ -799,17 +813,20 @@ class Sim(object):
             free_b = 2 ** 31
         return max(1, min(max(hi - lo, 1), int(free_b / share // (n * bytes_per_sample)) or 1))
 
-    def _publish_allan(self, name, algo, tau, accel, gyro):
+    def _publish_allan(self, name, algo, tau, accel, gyro, *per_series):
         """The plugin's first output, its abscissa (algo_time: the same tau for every run; algo_freq for Psd),
         and its accel and gyro outputs [R, ntau, 3] (ad_* for Allan, hd_* for Hadamard, psd_* for Psd) under run
-        keys.  Plugins of one Sim with the same abscissa share it: each replaces its own run keys in it and keeps
-        the others'."""
-        t, o_accel, o_gyro = algo.output
+        keys, then its per-series outputs in output order (Allan(fit=True): noise_accel, noise_gyro [R, 3, 6]).
+        Plugins of one Sim with the same abscissa share it: each replaces its own run keys in it and keeps the
+        others'."""
+        t, o_accel, o_gyro, *o_rest = algo.output
         prev = self.data.get(t)
         keep = {k: v for k, v in prev.items() if not k.startswith(name + '_')} if isinstance(prev, dict) else {}
         self.data[t] = dict(keep, **_keyed(name, [tau] * len(accel)))
         self.data[o_accel] = _keyed(name, accel)
         self.data[o_gyro] = _keyed(name, gyro)
+        for o, v in zip(o_rest, per_series):
+            self.data[o] = _keyed(name, v)
 
     def _run_allan(self, i, algo):
         """The Allan deviations of this rank's shard of the runs, in run blocks sized to the free device
@@ -819,31 +836,39 @@ class Sim(object):
         rarely needed; otherwise K1 materialises the series (48 B per run-sample) for K4 (~2 B of workspace).
         Allan(overlapping=True) and Hadamard() always materialise: K4o needs its prefix workspace (about 48 B per
         run-sample for the three series of one sensor) beside the series.  Psd() materialises too, with K11's
-        chunk sums beside the series; its abscissa is the frequency grid instead of tau."""
+        chunk sums beside the series; its abscissa is the frequency grid instead of tau.  Allan(fit=True) fits
+        every block's curves on the device (K13, engine.allan_fit) before they are copied back; the [R, 6, 6]
+        noise terms (channels accel x y z, gyro x y z) are gathered with the curves."""
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
         fused = (algo.fused and self._vib_acc is None and self._vib_gyro is None and n > 5040
                  and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
+        fit = getattr(algo, 'fit', False)
         tau = algo.abscissa(n, self.fs[0])
         block = self._allan_block(6 * 2, 2) if fused else self._allan_block(algo.run_bytes(n), 3)
-        parts = []      # [runs, ntau, 6]: accel, gyro
+        parts, fits = [], []      # [runs, ntau, 6]: accel, gyro; [runs, 6, 6]: the noise terms of each channel
         for r0 in range(lo, hi, block):
             r1 = min(hi, r0 + block)
             if fused:
                 d = self._dev
                 avar, _ = engine.allan_mc(self.fs[0], r1 - r0, d['ref_gyro'], d['ref_accel'], self.imu.gyro_err,
                                           self.imu.accel_err, self.seed, run_offset=self.run_base + r0)
+                if fit:
+                    fits.append(engine.allan_fit(self.fs[0], n, avar).reshape(r1 - r0, 6, 6).cpu().numpy())
                 parts.append(torch.sqrt(avar).permute(0, 2, 1).contiguous().cpu().numpy())
             else:
                 # every channel a contiguous series: K4 then streams them with bulk copies
                 gyro, accel = self._noise_block(r0, r1, engine.LAYOUT_CHANNEL_MAJOR)
-                tau, a, g = algo.run_batch(self.fs[0], accel, gyro, channel_major=True)
+                tau, a, g, *noise = algo.run_batch(self.fs[0], accel, gyro, channel_major=True)
                 parts.append(np.concatenate([a, g], axis=2))
+                if fit:
+                    fits.append(np.concatenate(noise, axis=1))
         both = np.concatenate(parts) if parts else np.zeros((0, len(tau), 6))
+        noise = (np.concatenate(fits) if fits else np.zeros((0, 6, 6))) if fit else None
         if dist.world() > 1:
-            both = dist.gather_rows(torch.from_numpy(np.ascontiguousarray(both.reshape(hi - lo, -1))),
-                                    self.sim_count).reshape(self.sim_count, len(tau), 6)
-        self._publish_allan(self.algo_name(i), algo, tau, both[:, :, 0:3], both[:, :, 3:6])
+            both, noise = _gather_allan(both, noise, self.sim_count)
+        per_series = (noise[:, 0:3], noise[:, 3:6]) if fit else ()
+        self._publish_allan(self.algo_name(i), algo, tau, both[:, :, 0:3], both[:, :, 3:6], *per_series)
 
     # ---- magnetometer calibration (K10) ---------------------------------------------------------
     def _publish_magcal(self, name, soft_iron, hard_iron):

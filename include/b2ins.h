@@ -469,6 +469,25 @@ int b2ins_ohadamard_f64_host(double fs, int64_t n, int64_t nseries, const double
                              int64_t inner, int64_t outer_stride, int64_t sample_stride,
                              double* hvar, double* tau);
 
+/* ---- K13: Allan noise identification (IEEE Std 952-1997 Annex C) ----------------------
+ * Fits sigma^2(tau) = C_-2 tau^-2 + C_-1 tau^-1 + C_0 + C_1 tau + C_2 tau^2 (every C_p >= 0) to the Allan
+ * variance curves of `nseries` series of n samples at fs, as K4 or K4o computed them (the variance, not the
+ * deviation), on their grid: tau_k = m_k / fs with m_k from b2ins_allan_num_tau(n, fs), weights
+ * w_k = floor(n / m_k) - 1.  Objective sum_k w_k (model(tau_k) / v_k - 1)^2 over the bins with v_k > 0, minimised
+ * exactly over the non-negative coefficients by enumerating the 31 supports (DESIGN.md section 3.13).
+ * var: v of series s, bin k at var[s * series_stride + k * bin_stride] (device; K4's [nseries][ntau] is
+ * series_stride = ntau, bin_stride = 1; may be null when ntau = 0).  out [nseries][6] (device):
+ *   Q = sqrt(C_-2 / 3), N = sqrt(C_-1), B = sqrt(C_0 pi / (2 ln 2)), K = sqrt(3 C_1), R = sqrt(2 C_2),
+ *   B_min = sqrt(min_k v_k) / sqrt(2 ln 2 / pi).
+ * A NaN, +-inf or negative v_k, or ntau = 0, gives six NaNs; a zero bin is left out of the fit but counts for
+ * B_min; all-zero bins give six zeros.  fs > 0 and finite, n >= 0, nseries >= 0, series_stride >= 0 and
+ * bin_stride >= 1, else B2INS_ERR_ARG; nseries = 0 returns B2INS_OK.  Deterministic: a series gives the same
+ * bits whatever the batch and its position in it. */
+int b2ins_allan_fit_f64(double fs, int64_t n, int64_t nseries, const double* var, int64_t series_stride,
+                        int64_t bin_stride, double* out, void* stream);
+int b2ins_allan_fit_f64_host(double fs, int64_t n, int64_t nseries, const double* var, int64_t series_stride,
+                             int64_t bin_stride, double* out);
+
 /* ---- K5: vibration series from a PSD -------------------------------------------
  * Replaces time_series_from_psd (gnss_ins_sim/psd/time_series_from_psd.py:17-65) as called
  * three times per sensor and run by acc_gen / gyro_gen (pathgen.py:478-485, :541-548).

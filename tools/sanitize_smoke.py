@@ -25,10 +25,13 @@ def main():
         avar, tau = engine.allan(100.0, x, n, nser)
         assert torch.isfinite(avar).all()
     x = engine.to_device(rng.randn(2, 12000, 3))
-    engine.allan(100.0, x, 12000, 6, inner=3, outer_stride=36000, sample_stride=3)
+    avar, _ = engine.allan(100.0, x, 12000, 6, inner=3, outer_stride=36000, sample_stride=3)
     # K4o's Hadamard form on the interleaved triads (ragged scan and output tiles)
     hvar, _ = engine.ohadamard(100.0, x, 12000, 6, inner=3, outer_stride=36000, sample_stride=3)
     assert torch.isfinite(hvar).all()
+    # K13 on the transposed curves (bin stride 6, a ragged last CTA of two series)
+    noise = engine.allan_fit(100.0, 12000, avar.t().contiguous(), series_stride=1, bin_stride=6)
+    assert torch.isfinite(noise).all()
     # K1 (plain and time-segmented), K12 (wide and narrow groups, both frames), K3, K6
     g = {rf: dict(np.load(os.path.join(ROOT, 'tests', 'golden', 'traj_90deg_turn_100hz_rf%d.npz' % rf)))
          for rf in (0, 1)}
