@@ -22,6 +22,10 @@ class SensorErr(ctypes.Structure):
                 ('b_corr', ctypes.c_double * 3), ('rw', ctypes.c_double * 3)]
 
 
+class NoiseTerms(ctypes.Structure):
+    _fields_ = [('q', ctypes.c_double * 3), ('k', ctypes.c_double * 3), ('r', ctypes.c_double * 3)]
+
+
 class Vib(ctypes.Structure):
     _fields_ = [('type', ctypes.c_int32), ('series_len', ctypes.c_int32),
                 ('amp', ctypes.c_double * 3), ('freq', ctypes.c_double),
@@ -66,6 +70,7 @@ class B2insError(RuntimeError):
 
 _I, _L, _D, _P, _U64 = ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p, ctypes.c_uint64
 _SE, _VB, _MC = ctypes.POINTER(SensorErr), ctypes.POINTER(Vib), ctypes.POINTER(McConfig)
+_NT = ctypes.POINTER(NoiseTerms)
 
 # name -> (restype, argtypes); every symbol include/b2ins.h declares
 SIGNATURES = {
@@ -78,12 +83,15 @@ SIGNATURES = {
     'b2ins_free_integration_f64_host': (_I, [_I, _D, _L, _L, _P, _P, _I, _P, _I, _I, _L, _I, _P, _P, _P, _I]),
     'b2ins_imu_noise_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P, _P]),
     'b2ins_imu_noise_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
+    'b2ins_imu_noise_ex_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _I, _P, _P, _P, _P]),
+    'b2ins_imu_noise_ex_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
     'b2ins_gps_noise_f64': (_I, [_L, _L, _P, _P, _P, _I, _U64, _L, _P, _P]),
     'b2ins_mag_noise_f64': (_I, [_L, _L, _P, _P, _P, _P, _U64, _L, _P, _P]),
     'b2ins_magcal_f64': (_I, [_L, _L, c_int64_p, _P, _P, _P, _P, _U64, _L, _P, _P, _P, _P]),
     'b2ins_magcal_fed_f64': (_I, [_L, _L, c_int64_p, _P, _L, _L, _P, _P, _P, _P]),
     'b2ins_magcal_fed_f64_host': (_I, [_L, _L, c_int64_p, _P, _L, _L, _P, _P, _P]),
     'b2ins_imu_err_stats_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _L, _P, _P, _P]),
+    'b2ins_imu_err_stats_ex_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _L, _P, _P, _P]),
     'b2ins_proc_stats_f64': (_I, [_L, _L, _I, _P, _P, _L, _P, _P, _P]),
     'b2ins_mc_free_integration_f64': (_I, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2ins_mc_free_integration_ex_f64': (_I, [_MC, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -130,6 +138,7 @@ SIGNATURES = {
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),
     'b2ins_diag_psd_plan': (_I, [_L, ctypes.POINTER(ctypes.c_int)]),
     'b2ins_diag_noise_plan': (_I, [_D, _L, _L, _SE, _SE, _I, c_double_p, c_int64_p]),
+    'b2ins_diag_noise_plan_ex': (_I, [_D, _L, _L, _SE, _SE, _NT, _NT, _I, c_double_p, c_int64_p]),
     'b2ins_diag_fastmath_f64': (_I, [_I, _L, _P, _P, _P, _P]),
     'b2ins_diag_philox': (_I, [_L, _P, _P]),
     'b2ins_diag_normal_from_words': (_I, [_L, _P, _P]),
@@ -203,9 +212,9 @@ def noise_plan(fs, runs, n, gyro_err, accel_err, sm_count=0):
     ge, ae = sensor_err(gyro_err, 'arw'), sensor_err(accel_err, 'vrw')
     coef = np.zeros(18)
     plan = np.zeros(3, dtype=np.int64)
-    check(load().b2ins_diag_noise_plan(float(fs), int(runs), int(n), ctypes.byref(ge), ctypes.byref(ae),
-                                        int(sm_count), coef.ctypes.data_as(c_double_p),
-                                        plan.ctypes.data_as(c_int64_p)))
+    check(load().b2ins_diag_noise_plan_ex(float(fs), int(runs), int(n), ctypes.byref(ge), ctypes.byref(ae),
+                                           noise_terms(gyro_err), noise_terms(accel_err), int(sm_count),
+                                           coef.ctypes.data_as(c_double_p), plan.ctypes.data_as(c_int64_p)))
     return {'gm_a': coef[0:6], 'gm_b': coef[6:12], 'wd': coef[12:18], 'nseg': int(plan[0]),
             'seg_len': int(plan[1]), 'pass1_len': int(plan[2])}
 
@@ -231,6 +240,27 @@ def sensor_err(err, white_key):
     a = np.array([err['b'], err['b_drift'], err['b_corr'], err[white_key]], dtype=np.float64)   # [4][3] = the struct
     assert a.shape == (4, 3)
     return SensorErr.from_buffer_copy(a)
+
+
+TERM_KEYS = ('q', 'rrw', 'rr')     # an imu_model dict's IEEE Std 952 terms (Q, K, R), SI units
+
+
+def set_terms(err):
+    """The IEEE Std 952 terms an imu_model dict sets: its keys among TERM_KEYS with a non-zero value."""
+    return [k for k in TERM_KEYS if k in err and np.any(np.asarray(err[k], dtype=np.float64) != 0.0)]
+
+
+def noise_terms(err):
+    """imu_model dict -> NoiseTerms (absent keys: zero), or None when it has no non-zero term: the _ex entry
+    points then run the kernels without terms."""
+    if not set_terms(err):
+        return None
+    t = NoiseTerms()
+    for f, k in zip(('q', 'k', 'r'), TERM_KEYS):
+        v = np.broadcast_to(np.asarray(err.get(k, 0.0), dtype=np.float64), (3,))
+        for c in range(3):
+            getattr(t, f)[c] = float(v[c])
+    return t
 
 
 def vib(vib_def, series_ptr=None, series_len=0):

@@ -336,7 +336,7 @@ struct AsyncBuf {
 // pass 1 reduces every segment to its zero-state end value, a tiny serial kernel chains them, pass 0
 // regenerates (counter-based Philox: nothing is stored) and writes.  Costs the noise twice, so it is only used
 // when one CTA per run would leave most of the GPU idle.
-void noise_plan(NoiseParams* out, int sms) {
+void noise_plan(NoiseParams* out, int sms, bool walk = false) {
   NoiseParams& p = *out;
   int nseg = 1;
   const int64_t want_ctas = static_cast<int64_t>(sms) * 2;
@@ -357,7 +357,7 @@ void noise_plan(NoiseParams* out, int sms) {
   // pass 1 only needs the drives that still matter at the segment end: |a|^L < 1e-20.  The rule is on |a|:
   // tau < dt gives a <= 0 (-1 at tau = dt / 2), whose drives decay as |a|^k; a = 0 keeps
   // none; |a| >= 1 never decays and needs the whole segment.
-  int64_t keep = 1;
+  int64_t keep = walk ? len : 1;     // a rate random walk never decays
   for (int c = 0; c < 6; ++c) {
     const double a = std::fabs((c < 3) ? p.accel.gm_a[c] : p.gyro.gm_a[c - 3]);
     if (a >= 1.0) {
@@ -371,12 +371,36 @@ void noise_plan(NoiseParams* out, int sms) {
   p.pass1_len = keep < len ? keep : len;
 }
 
+// the IEEE Std 952 terms of the two triads for the device (K1's channel order: accel, then gyro), checked; *any
+// is false when every term is zero or absent, and the _ex entry points then launch the kernels without them
+int digest_terms(const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms, double fs,
+                 NoiseTerms* x, bool* any, bool* walk) {
+  std::memset(x, 0, sizeof(*x));
+  *any = *walk = false;
+  const b2ins_noise_terms* t[2] = {accel_terms, gyro_terms};
+  for (int s = 0; s < 2; ++s) {
+    if (!t[s]) continue;
+    for (int c = 0; c < 3; ++c) {
+      ARG_CHECK(std::isfinite(t[s]->q[c]) && t[s]->q[c] >= 0.0 && std::isfinite(t[s]->k[c]) && t[s]->k[c] >= 0.0 &&
+                    std::isfinite(t[s]->r[c]),
+                "noise terms: q and k must be finite and >= 0, r finite");
+      x->q[3 * s + c] = t[s]->q[c] * std::sqrt(12.0);
+      x->k[3 * s + c] = t[s]->k[c] * std::sqrt(1.0 / fs);
+      x->r[3 * s + c] = t[s]->r[c];
+      *any = *any || t[s]->q[c] != 0.0 || t[s]->k[c] != 0.0 || t[s]->r[c] != 0.0;
+      *walk = *walk || t[s]->k[c] != 0.0;
+    }
+  }
+  return B2INS_OK;
+}
+
 // K1's parameters and time segmentation, shared by K1 and K9; with segments, pass 1 and the carry chain are
-// launched here and *scratch holds their buffers until the caller has queued pass 0 on s.
+// launched here and *scratch holds their buffers until the caller has queued pass 0 on s.  x (nullable): the
+// IEEE Std 952 terms, whose rate random walk is carried across the segments like the drift, with a = 1.
 int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
                   const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
                   const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, cudaStream_t s, NoiseParams* out,
-                  AsyncBuf* scratch) {
+                  AsyncBuf* scratch, NoiseTerms* x = nullptr, bool walk = false) {
   NoiseParams& p = *out;
   std::memset(&p, 0, sizeof(p));
   p.n = n;
@@ -391,17 +415,29 @@ int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, co
   if (rc != B2INS_OK) return rc;
   p.ref_gyro = ref_gyro;
   p.ref_accel = ref_accel;
-  noise_plan(&p, sm_count());
+  noise_plan(&p, sm_count(), walk);
   p.pass = 0;
   p.seg_carry = nullptr;
   p.seg_end = nullptr;
   if (p.nseg > 1) {
-    CU_CHECK(scratch->alloc(sizeof(double) * runs * p.nseg * 12));
+    CU_CHECK(scratch->alloc(sizeof(double) * runs * p.nseg * (x ? 24 : 12)));
     p.seg_end = scratch->p;
     p.seg_carry = scratch->p + runs * p.nseg * 6;
     p.pass = 1;
-    imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
-    noise_carry_kernel<<<static_cast<unsigned>((runs * 6 + 127) / 128), 128, 0, s>>>(p);
+    const unsigned ctas = static_cast<unsigned>((runs * 6 + 127) / 128);
+    if (x) {
+      x->seg_end = scratch->p + runs * p.nseg * 12;
+      x->seg_carry = scratch->p + runs * p.nseg * 18;
+      imu_noise_ex_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p, *x);
+      NoiseParams pw = p;      // the walk's carry chain: noise_carry_kernel with a = 1
+      for (int c = 0; c < 3; ++c) pw.accel.gm_a[c] = pw.gyro.gm_a[c] = 1.0;
+      pw.seg_end = x->seg_end;
+      pw.seg_carry = x->seg_carry;
+      noise_carry_kernel<<<ctas, 128, 0, s>>>(pw);
+    } else {
+      imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
+    }
+    noise_carry_kernel<<<ctas, 128, 0, s>>>(p);
     p.pass = 0;
   }
   CU_CHECK(cudaGetLastError());
@@ -545,41 +581,64 @@ int b2ins_free_integration_f64_host(int ref_frame, double fs, int64_t runs, int6
 }
 
 // ---------------------------------------------------------------- K1 --------
-int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
-                        const double* ref_accel, const b2ins_sensor_err* gyro_err,
-                        const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
-                        const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, int layout,
-                        double* gyro, double* accel, double* z_dump, void* stream) {
+int b2ins_imu_noise_ex_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
+                           const double* ref_accel, const b2ins_sensor_err* gyro_err,
+                           const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                           const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro,
+                           const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, int layout,
+                           double* gyro, double* accel, double* z_dump, void* stream) {
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   ARG_CHECK(layout >= 0 && layout <= 2, "layout must be B2INS_LAYOUT_*");
+  NoiseTerms x;
+  bool terms = false, walk = false;
+  int rc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
+  if (rc != B2INS_OK) return rc;
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && gyro && accel, "null buffer");
   ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
   NoiseParams p;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AsyncBuf scratch(s);
-  const int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed,
-                               run_offset, s, &p, &scratch);
+  rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset, s,
+                     &p, &scratch, terms ? &x : nullptr, walk);
   if (rc != B2INS_OK) return rc;
   p.out_gyro = gyro;
   p.out_accel = accel;
   layout_strides(layout, runs, n, &p.osr, &p.ost, &p.osc);
   p.z_dump = z_dump;
-  imu_noise_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p);
+  if (terms)
+    imu_noise_ex_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p, x);
+  else
+    imu_noise_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p);
   CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
 }
 
+int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
+                        const double* ref_accel, const b2ins_sensor_err* gyro_err,
+                        const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
+                        const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, int layout,
+                        double* gyro, double* accel, double* z_dump, void* stream) {
+  return b2ins_imu_noise_ex_f64(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, nullptr, nullptr, vib_gyro,
+                                vib_accel, seed, run_offset, layout, gyro, accel, z_dump, stream);
+}
+
 // ---------------------------------------------------------------- K9 --------
-int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
-                            const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
-                            const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
-                            int64_t stats_start, double* end_err, double* proc_stats, void* stream) {
+int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
+                               const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                               const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                               const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel, uint64_t seed,
+                               int64_t run_offset, int64_t stats_start, double* end_err, double* proc_stats,
+                               void* stream) {
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   ARG_CHECK(stats_start < n || n == 0, "stats_start must be < n");
+  NoiseTerms x;
+  bool terms = false, walk = false;
+  const int trc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
+  if (trc != B2INS_OK) return trc;
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && end_err, "null buffer");
   ARG_CHECK(stats_start < 0 || proc_stats, "stats_start >= 0 needs proc_stats");
@@ -589,7 +648,7 @@ int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* re
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AsyncBuf scratch(s), partial(s);
   const int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed,
-                               run_offset, s, &P.np, &scratch);
+                               run_offset, s, &P.np, &scratch, terms ? &x : nullptr, walk);
   if (rc != B2INS_OK) return rc;
   P.stats_start = stats_start;
   P.end_err = end_err;
@@ -600,7 +659,10 @@ int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* re
       return fail(B2INS_ERR_CUDA, "cudaMallocAsync of the segment partials: %s", cudaGetErrorString(e));
     P.partial = partial.p;
   }
-  imu_err_stats_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P);
+  if (terms)
+    imu_err_stats_ex_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P, x);
+  else
+    imu_err_stats_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P);
   if (partial.p) {
     err_stats_fold_kernel<<<static_cast<unsigned>((runs * kErrCh + 127) / 128), 128, 0, s>>>(P);
     CU_CHECK(partial.free());
@@ -608,6 +670,14 @@ int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* re
   CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
+}
+
+int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
+                            const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                            const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
+                            int64_t stats_start, double* end_err, double* proc_stats, void* stream) {
+  return b2ins_imu_err_stats_ex_f64(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, nullptr, nullptr, vib_gyro,
+                                    vib_accel, seed, run_offset, stats_start, end_err, proc_stats, stream);
 }
 
 // ---------------------------------------------------------------- K3p -------
@@ -776,6 +846,16 @@ int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n, const double* r
                              const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
                              const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
                              int layout, double* gyro, double* accel, double* z_dump) {
+  return b2ins_imu_noise_ex_f64_host(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, nullptr, nullptr,
+                                     vib_gyro, vib_accel, seed, run_offset, layout, gyro, accel, z_dump);
+}
+
+int b2ins_imu_noise_ex_f64_host(double fs, int64_t runs, int64_t n, const double* ref_gyro,
+                                const double* ref_accel, const b2ins_sensor_err* gyro_err,
+                                const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                                const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro,
+                                const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
+                                int layout, double* gyro, double* accel, double* z_dump) {
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(ref_gyro && ref_accel && gyro && accel, "null buffer");
@@ -790,8 +870,8 @@ int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n, const double* r
   double* oa = st.out(accel, elems);
   double* zd = z_dump ? st.out(z_dump, elems * 4) : nullptr;
   return st.run([&](cudaStream_t s) {
-    return b2ins_imu_noise_f64(fs, runs, n, rg, ra, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset,
-                               layout, og, oa, zd, s);
+    return b2ins_imu_noise_ex_f64(fs, runs, n, rg, ra, gyro_err, accel_err, gyro_terms, accel_terms, vib_gyro,
+                                  vib_accel, seed, run_offset, layout, og, oa, zd, s);
   });
 }
 
@@ -1713,9 +1793,19 @@ int b2ins_welch_f64_host(double fs, int64_t n, int64_t nseries, const double* x,
 // ---------------------------------------------------------------- K1 plan ---
 int b2ins_diag_noise_plan(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
                           const b2ins_sensor_err* accel_err, int sm_count_arg, double* coef, int64_t* plan) {
+  return b2ins_diag_noise_plan_ex(fs, runs, n, gyro_err, accel_err, nullptr, nullptr, sm_count_arg, coef, plan);
+}
+
+int b2ins_diag_noise_plan_ex(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
+                             const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                             const b2ins_noise_terms* accel_terms, int sm_count_arg, double* coef, int64_t* plan) {
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs > 0 && n > 0, "runs and n must be positive");
   ARG_CHECK(gyro_err && accel_err && coef && plan, "null buffer");
+  NoiseTerms x;
+  bool terms = false, walk = false;
+  const int trc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
+  if (trc != B2INS_OK) return trc;
   NoiseParams p;
   std::memset(&p, 0, sizeof(p));
   p.n = n;
@@ -1724,7 +1814,7 @@ int b2ins_diag_noise_plan(double fs, int64_t runs, int64_t n, const b2ins_sensor
   if (rc != B2INS_OK) return rc;
   rc = digest_triad(accel_err, nullptr, fs, &p.accel);
   if (rc != B2INS_OK) return rc;
-  noise_plan(&p, sm_count_arg > 0 ? sm_count_arg : sm_count());
+  noise_plan(&p, sm_count_arg > 0 ? sm_count_arg : sm_count(), walk);
   for (int c = 0; c < 6; ++c) {
     const TriadNoise& e = (c < 3) ? p.accel : p.gyro;
     coef[c] = e.gm_a[c % 3];

@@ -36,6 +36,8 @@ constexpr uint32_t kDrawPhase = 9;  // +axis, t = 0xFFFFFFFF: sinusoidal gyro-vi
 constexpr uint32_t kDrawOdo = 12;   // odometer white noise (z0)
 constexpr uint32_t kDrawMag = 13;   // magnetometer: 13 (x, y), 14 (z from z0)
 constexpr uint32_t kDrawPsd = 16;   // +3*sensor+axis, t = bin index: PSD random phases
+constexpr uint32_t kDrawRrw = 32;   // +3*sensor+axis: rate random walk drive (z0)
+constexpr uint32_t kDrawQuant = 38; // +3*sensor+axis: quantisation uniform (words x1:x0, as uniform01)
 
 struct PhiloxOut {
   uint32_t x0, x1, x2, x3;

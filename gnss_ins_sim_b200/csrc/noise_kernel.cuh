@@ -69,6 +69,39 @@ __device__ __forceinline__ void triad_sample(const NoiseParams& p, const TriadNo
   }
 }
 
+// The IEEE Std 952 terms of b2ins_noise_terms, digested per channel in K1's order (accel x y z, gyro x y z)
+struct NoiseTerms {
+  double q[6];          // Q sqrt(12): the angle / velocity quantisation error is q (u - 1/2)
+  double k[6];          // K sqrt(dt): the rate random walk's step per unit normal
+  double r[6];          // R: the rate ramp R (t dt)
+  double* seg_carry;    // time segments: the walk at every segment start [runs][nseg][6] (all zero for seg 0)
+  double* seg_end;      //                pass 1: the zero-state walk at every segment end [runs][nseg][6]
+};
+
+// the terms of one triad of sample t, added to the measurement m3: the stretch's zero-state walk rk (then
+// advanced by one sample), the quantisation rate error (e[t+1] - e[t]) / dt (qe: e[t], then e[t+1]) and the ramp.
+// drives_only (pass 1): only the walk advances.  A channel whose k (q) is zero makes no walk (quantisation) draw:
+// the branches are uniform over the launch, so a ramp alone costs no Philox.
+template <int SENSOR>
+__device__ __forceinline__ void terms_sample(const NoiseParams& p, const NoiseTerms& x, int64_t t, uint32_t run_lo,
+                                             uint32_t run_hi, bool drives_only, double* rk, double* qe, double* m3) {
+  const uint32_t t32 = static_cast<uint32_t>(t);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int ch = 3 * SENSOR + c;
+    if (!drives_only) {
+      double qr = 0.0;
+      if (x.q[ch] != 0.0) {
+        const double e1 = x.q[ch] * (uniform01(t32 + 1u, kDrawQuant + ch, run_lo, run_hi, p.k0, p.k1) - 0.5);
+        qr = (e1 - qe[c]) / p.dt;
+        qe[c] = e1;
+      }
+      m3[c] += rk[c] + (qr + x.r[ch] * (static_cast<double>(t) * p.dt));
+    }
+    if (x.k[ch] != 0.0) rk[c] = fma(x.k[ch], normal_pair(t32, kDrawRrw + ch, run_lo, run_hi, p.k0, p.k1).z0, rk[c]);
+  }
+}
+
 // the prologue of a K1 or K9 CTA, before its first __syncthreads: a^q per channel into apow[kNoisePer + 1][6],
 // the run's sinusoidal gyro-vibration phase and, with carry_in, the Gauss-Markov state at the segment start
 // (zero without)
@@ -99,9 +132,14 @@ __device__ __forceinline__ void noise_prologue(const NoiseParams& p, double (*ap
   }
 }
 
-__global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __grid_constant__ NoiseParams p) {
+// K1's body.  TERMS adds the IEEE Std 952 terms of x (DESIGN.md section 4): the rate random walk k runs as six
+// more channels of the affine scan with A = 1, the quantisation error carries e[t+1] along the thread's stretch
+// (one extra uniform at its start), the rate ramp is R t dt.  Without TERMS this is K1 as it always was.
+template <bool TERMS>
+__device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const NoiseTerms* x) {
+  constexpr int C = TERMS ? 12 : 6;               // scanned channels: drift (accel, gyro), then the walk
   __shared__ double stage[2][kNoiseTile * 3];     // accel, gyro of the tile, [sample][axis]
-  __shared__ double wtot[6][kNoiseWarps][2];      // (A, E) of every warp's stretch, per channel
+  __shared__ double wtot[C][kNoiseWarps][2];      // (A, E) of every warp's stretch, per channel
   __shared__ double apow[kNoisePer + 1][6];       // a^q per channel
   const int segs = (p.pass == 1) ? p.nseg - 1 : p.nseg;
   const int64_t run = blockIdx.x / segs;
@@ -111,16 +149,31 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __gri
   const int64_t grun = p.run_offset + run;
   const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  double phase[3], carry[6];                      // carry: d at the first sample of the tile
-  noise_prologue(p, apow, run, seg, run_lo, run_hi, p.pass == 0, phase, carry);
+  double phase[3], carry[C];                      // carry: d (and k) at the first sample of the tile
+  noise_prologue(p, apow, run, seg, run_lo, run_hi, p.pass == 0, phase, *reinterpret_cast<double(*)[6]>(carry));
+  if constexpr (TERMS) {
+#pragma unroll
+    for (int c = 0; c < 6; ++c) carry[6 + c] = (p.pass == 0 && x->seg_carry) ? x->seg_carry[(run * p.nseg + seg) * 6 + c] : 0.0;
+  }
   __syncthreads();
 
   for (int64_t tile0 = seg_lo; tile0 < seg_hi; tile0 += kNoiseTile) {
     const int cnt = static_cast<int>(min64(kNoiseTile, seg_hi - tile0));
     // ---- the thread's stretch: one sensor triad at a time (three Box-Muller chains in flight) -------
-    double r[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    double r[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) r[c] = 0.0;
     int mine = cnt - tid * kNoisePer;                 // live samples of this thread's stretch
     mine = mine < 0 ? 0 : (mine > kNoisePer ? kNoisePer : mine);
+    double qe[TERMS ? 6 : 1];                         // TERMS: the quantisation error e[t] of each channel
+    if constexpr (TERMS) {
+      if (mine > 0 && p.pass == 0) {
+        const uint32_t t0 = static_cast<uint32_t>(tile0 + tid * kNoisePer);
+#pragma unroll
+        for (int c = 0; c < 6; ++c)
+          qe[c] = x->q[c] != 0.0 ? x->q[c] * (uniform01(t0, kDrawQuant + c, run_lo, run_hi, p.k0, p.k1) - 0.5) : 0.0;
+      }
+    }
 #pragma unroll 1
     for (int q = 0; q < mine; ++q) {
       const int el = tid * kNoisePer + q;
@@ -128,24 +181,26 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __gri
       double m3[3];
       triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase,
                       p.pass == 1, r, m3);
+      if constexpr (TERMS) terms_sample<0>(p, *x, t, run_lo, run_hi, p.pass == 1, r + 6, qe, m3);
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
       triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase,
                       p.pass == 1, r + 3, m3);
+      if constexpr (TERMS) terms_sample<1>(p, *x, t, run_lo, run_hi, p.pass == 1, r + 9, qe + 3, m3);
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
     }
     // ---- affine scan over the threads, six channels: (A, E) o (A', E') = (A A', A' E + E') -------
-    double sA[6], sE[6];
+    double sA[C], sE[C];
 #pragma unroll
-    for (int c = 0; c < 6; ++c) {
-      sA[c] = apow[mine][c];
+    for (int c = 0; c < C; ++c) {
+      sA[c] = c < 6 ? apow[mine][c] : 1.0;
       sE[c] = r[c];
     }
-    affine_scan_warp<6, kNoiseWarps>(sA, sE, wtot, lane, warp);
+    affine_scan_warp<C, kNoiseWarps>(sA, sE, wtot, lane, warp);
     __syncthreads();   // warp totals; the staged tile is complete
-    double S[6];       // drift at the first sample of this thread's stretch
-    affine_scan_block<6, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
+    double S[C];       // drift at the first sample of this thread's stretch
+    affine_scan_block<C, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
     if (p.pass == 0) {
       // ---- + a^q S on the thread's own samples, then the tile leaves in the caller's layout -------
 #pragma unroll 1
@@ -155,6 +210,10 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __gri
         for (int c = 0; c < 3; ++c) {
           stage[0][el * 3 + c] += apow[q][c] * S[c];
           stage[1][el * 3 + c] += apow[q][3 + c] * S[3 + c];
+          if constexpr (TERMS) {      // the walk at the stretch start
+            stage[0][el * 3 + c] += S[6 + c];
+            stage[1][el * 3 + c] += S[9 + c];
+          }
         }
       }
       __syncthreads();
@@ -196,7 +255,20 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __gri
     // segment, whose end value is never used
 #pragma unroll
     for (int c = 0; c < 6; ++c) p.seg_end[(run * p.nseg + seg) * 6 + c] = carry[c];
+    if constexpr (TERMS) {
+#pragma unroll
+      for (int c = 0; c < 6; ++c) x->seg_end[(run * p.nseg + seg) * 6 + c] = carry[6 + c];
+    }
   }
+}
+
+__global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __grid_constant__ NoiseParams p) {
+  imu_noise_body<false>(p, nullptr);
+}
+
+__global__ void __launch_bounds__(kNoiseThreads, 3) imu_noise_ex_kernel(const __grid_constant__ NoiseParams p,
+                                                                      const __grid_constant__ NoiseTerms x) {
+  imu_noise_body<true>(p, &x);
 }
 
 // carry-in of every segment from the zero-state segment responses: c[s+1] = a^L c[s] + E[s]

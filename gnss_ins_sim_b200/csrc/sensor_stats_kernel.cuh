@@ -60,10 +60,13 @@ __device__ __forceinline__ void write_stats(double* ps, int c, int nc, double n,
   ps[2 * nc + c] = n > 0.0 ? sqrt(m2 / n) : none;
 }
 
-__global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const __grid_constant__ ErrStatsParams P) {
+// K9's body; TERMS: with the IEEE Std 952 terms of x, generated as K1's imu_noise_body<true> makes them
+template <bool TERMS>
+__device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, const NoiseTerms* x) {
+  constexpr int C = TERMS ? 12 : 6;
   const NoiseParams& p = P.np;
   __shared__ double stage[2][kNoiseTile * 3];     // accel, gyro of the tile, [sample][axis]
-  __shared__ double wtot[6][kNoiseWarps][2];
+  __shared__ double wtot[C][kNoiseWarps][2];
   __shared__ double apow[kNoisePer + 1][6];
   const int64_t run = blockIdx.x / p.nseg;
   const int seg = static_cast<int>(blockIdx.x % p.nseg);
@@ -73,8 +76,12 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
   const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool want_stats = P.stats_start >= 0;
-  double phase[3], carry[6];
-  noise_prologue(p, apow, run, seg, run_lo, run_hi, true, phase, carry);
+  double phase[3], carry[C];
+  noise_prologue(p, apow, run, seg, run_lo, run_hi, true, phase, *reinterpret_cast<double(*)[6]>(carry));
+  if constexpr (TERMS) {
+#pragma unroll
+    for (int c = 0; c < 6; ++c) carry[6 + c] = x->seg_carry ? x->seg_carry[(run * p.nseg + seg) * 6 + c] : 0.0;
+  }
   double an = 0.0, am[6], a2[6], ax[6];           // the thread's running statistics
 #pragma unroll
   for (int c = 0; c < 6; ++c) am[c] = a2[c] = ax[c] = 0.0;
@@ -82,9 +89,20 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
 
   for (int64_t tile0 = seg_lo; tile0 < seg_hi; tile0 += kNoiseTile) {
     const int cnt = static_cast<int>(min64(kNoiseTile, seg_hi - tile0));
-    double r[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    double r[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) r[c] = 0.0;
     int mine = cnt - tid * kNoisePer;
     mine = mine < 0 ? 0 : (mine > kNoisePer ? kNoisePer : mine);
+    double qe[TERMS ? 6 : 1];
+    if constexpr (TERMS) {
+      if (mine > 0) {
+        const uint32_t t0 = static_cast<uint32_t>(tile0 + tid * kNoisePer);
+#pragma unroll
+        for (int c = 0; c < 6; ++c)
+          qe[c] = x->q[c] != 0.0 ? x->q[c] * (uniform01(t0, kDrawQuant + c, run_lo, run_hi, p.k0, p.k1) - 0.5) : 0.0;
+      }
+    }
 #pragma unroll 1
     for (int q = 0; q < mine; ++q) {
       const int el = tid * kNoisePer + q;
@@ -92,24 +110,26 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
       double m3[3];
       triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase, false,
                       r, m3);
+      if constexpr (TERMS) terms_sample<0>(p, *x, t, run_lo, run_hi, false, r + 6, qe, m3);
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
       triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase, false,
                       r + 3, m3);
+      if constexpr (TERMS) terms_sample<1>(p, *x, t, run_lo, run_hi, false, r + 9, qe + 3, m3);
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
     }
     // ---- the affine scan of K1 ------------------------------------------------------------------
-    double sA[6], sE[6];
+    double sA[C], sE[C];
 #pragma unroll
-    for (int c = 0; c < 6; ++c) {
-      sA[c] = apow[mine][c];
+    for (int c = 0; c < C; ++c) {
+      sA[c] = c < 6 ? apow[mine][c] : 1.0;
       sE[c] = r[c];
     }
-    affine_scan_warp<6, kNoiseWarps>(sA, sE, wtot, lane, warp);
+    affine_scan_warp<C, kNoiseWarps>(sA, sE, wtot, lane, warp);
     __syncthreads();
-    double S[6];
-    affine_scan_block<6, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
+    double S[C];
+    affine_scan_block<C, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
     // ---- the thread's own samples: the measurement exactly as K1 stores it, minus the truth --------
     // pass A: e (kept in the stage), the end-point error, sum and max over the samples >= stats_start
     const int64_t t_lo = tile0 + tid * kNoisePer;
@@ -125,8 +145,12 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
       double e[6];
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        const double ma = fma(apow[q][c], S[c], stage[0][el * 3 + c]);
-        const double mg = fma(apow[q][3 + c], S[3 + c], stage[1][el * 3 + c]);
+        double ma = fma(apow[q][c], S[c], stage[0][el * 3 + c]);
+        double mg = fma(apow[q][3 + c], S[3 + c], stage[1][el * 3 + c]);
+        if constexpr (TERMS) {      // the walk at the stretch start
+          ma += S[6 + c];
+          mg += S[9 + c];
+        }
         e[c] = ma - p.ref_accel[t * 3 + c];
         e[3 + c] = mg - p.ref_gyro[t * 3 + c];
         stage[0][el * 3 + c] = e[c];
@@ -215,6 +239,15 @@ __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const _
       o[13 + c] = mx;
     }
   }
+}
+
+__global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const __grid_constant__ ErrStatsParams P) {
+  imu_err_stats_body<false>(P, nullptr);
+}
+
+__global__ void __launch_bounds__(kNoiseThreads, 3) imu_err_stats_ex_kernel(const __grid_constant__ ErrStatsParams P,
+                                                                          const __grid_constant__ NoiseTerms x) {
+  imu_err_stats_body<true>(P, &x);
 }
 
 // the segments of every run, merged in segment order: one thread per (run, channel)

@@ -103,7 +103,8 @@ def free_integration_odo(ref_frame, fs, gyro, odo, ini, earth_rot=True, layout=L
 
 def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0,
               vib_gyro=None, vib_accel=None, layout=LAYOUT_RUN_MAJOR, dump_z=False):
-    """K1.  ref_gyro/ref_accel: CUDA f64 [n,3]; *_err: imu_model dicts.
+    """K1.  ref_gyro/ref_accel: CUDA f64 [n,3]; *_err: imu_model dicts (with a non-zero 'q', 'rrw' or 'rr':
+    K1 with the IEEE Std 952 terms, b2ins_imu_noise_ex_f64).
     Returns gyro, accel ([R,n,3], [n,3,R] or, LAYOUT_CHANNEL_MAJOR, [R,3,n]) and, if dump_z,
     z [R,n,12]."""
     _require_cuda()
@@ -117,10 +118,17 @@ def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offs
     ge, ae = _lib.sensor_err(gyro_err, 'arw'), _lib.sensor_err(accel_err, 'vrw')
     vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
-    _lib.check(lib.b2ins_imu_noise_f64(
-        float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
-        ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
-        _ptr(gyro), _ptr(accel), _ptr(z), _stream()))
+    tg, ta = _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err)
+    if tg is None and ta is None:
+        _lib.check(lib.b2ins_imu_noise_f64(
+            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
+            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
+            _ptr(gyro), _ptr(accel), _ptr(z), _stream()))
+    else:
+        _lib.check(lib.b2ins_imu_noise_ex_f64(
+            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
+            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
+            _ptr(gyro), _ptr(accel), _ptr(z), _stream()))
     return (gyro, accel, z) if dump_z else (gyro, accel)
 
 
@@ -227,10 +235,17 @@ def imu_err_stats(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_
     ge, ae = _lib.sensor_err(gyro_err, 'arw'), _lib.sensor_err(accel_err, 'vrw')
     vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
-    _lib.check(lib.b2ins_imu_err_stats_f64(
-        float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
-        ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
-        _ptr(end_err), _ptr(proc), _stream()))
+    tg, ta = _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err)
+    if tg is None and ta is None:
+        _lib.check(lib.b2ins_imu_err_stats_f64(
+            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
+            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
+            _ptr(end_err), _ptr(proc), _stream()))
+    else:
+        _lib.check(lib.b2ins_imu_err_stats_ex_f64(
+            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
+            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
+            _ptr(end_err), _ptr(proc), _stream()))
     return end_err, proc
 
 

@@ -11,6 +11,10 @@ so building a second IMU silently changes the first.  Here every IMU owns privat
 Units (as in the reference after its conversions, imu_model.py:138-143):
   gyro  b, b_drift [rad/s], arw [rad/s/sqrt(Hz)], b_corr [s]
   accel b, b_drift [m/s^2], vrw [m/s^2/sqrt(Hz)], b_corr [s]
+and, only where a dict accuracy gives them, the IEEE Std 952 terms the reference does not model (the columns Q, K
+and R of Allan(fit=True)'s noise_gyro / noise_accel):
+  gyro  q [rad], rrw [rad/s^2/sqrt(Hz)], rr [rad/s^2]
+  accel q [m/s], rrw [m/s^3/sqrt(Hz)], rr [m/s^3]
 """
 import math
 
@@ -60,6 +64,28 @@ def odo_profile():
 
 
 _REQUIRED = ('gyro_b', 'gyro_b_stability', 'gyro_arw', 'accel_b', 'accel_b_stability', 'accel_vrw')
+# optional IEEE Std 952 terms: accuracy key -> (stored key, factor from the datasheet unit to SI)
+_TERMS = {
+    'gyro': {'gyro_q': ('q', D2R),                       # deg -> rad
+             'gyro_rrw': ('rrw', D2R / 3600.0 / 60.0),    # deg/h/sqrt(h) -> rad/s^2/sqrt(Hz)
+             'gyro_rr': ('rr', D2R / 3600.0 / 3600.0)},   # deg/h^2 -> rad/s^2
+    'accel': {'accel_q': ('q', 1.0),                     # m/s
+              'accel_rrw': ('rrw', 1.0 / 60.0),          # m/s^2/sqrt(h) -> m/s^3/sqrt(Hz)
+              'accel_rr': ('rr', 1.0 / 3600.0)},         # m/s^2/h -> m/s^3
+}
+_TERM_KEYS = ('q', 'rrw', 'rr')
+
+
+def _terms(accuracy, sensor):
+    """The IEEE Std 952 terms of one sensor an accuracy dict gives, in SI units (absent keys are not stored)."""
+    out = {}
+    for key, (stored, scale) in _TERMS[sensor].items():
+        if key in accuracy:
+            v = np.broadcast_to(np.array(accuracy[key], dtype=np.float64), (3,)) * scale
+            if not np.all(np.isfinite(v)) or (stored != 'rr' and np.any(v < 0.0)):
+                raise ValueError('%s must be finite%s' % (key, '' if stored == 'rr' else ' and >= 0'))
+            out[stored] = v
+    return out
 
 
 class IMU(object):
@@ -67,7 +93,9 @@ class IMU(object):
     'mid-accuracy' | 'high-accuracy' | dict with gyro_b [deg/h], gyro_arw [deg/sqrt(h)],
     gyro_b_stability [deg/h], accel_b [m/s^2], accel_vrw [m/s/sqrt(h)],
     accel_b_stability [m/s^2] and optionally gyro_b_corr / accel_b_corr [s] (missing ->
-    inf -> white bias drift), mag_si, mag_hi, mag_std."""
+    inf -> white bias drift), mag_si, mag_hi, mag_std, and the IEEE Std 952 terms gyro_q [deg],
+    gyro_rrw [deg/h/sqrt(h)], gyro_rr [deg/h^2], accel_q [m/s], accel_rrw [m/s^2/sqrt(h)],
+    accel_rr [m/s^2/h] (missing -> zero; stored as gyro_err / accel_err 'q', 'rrw', 'rr' in SI units)."""
 
     def __init__(self, accuracy='low-accuracy', axis=6, gps=True, gps_opt=None,
                  odo=False, odo_opt=None):
@@ -102,6 +130,8 @@ class IMU(object):
                 'b_corr': as_arr(accuracy['accel_b_corr']) if 'accel_b_corr' in accuracy
                 else inf3.copy(),
                 'vrw': as_arr(accuracy['accel_vrw']) / 60.0}
+            self.gyro_err.update(_terms(accuracy, 'gyro'))
+            self.accel_err.update(_terms(accuracy, 'accel'))
             self.mag_err = mag_profile('low-accuracy')
             if self.magnetometer:
                 if 'mag_std' not in accuracy:
@@ -145,7 +175,7 @@ class IMU(object):
             return profiles(value)
         if isinstance(value, dict):
             for k in value:
-                if k not in current:
+                if k not in current and k not in _TERM_KEYS:
                     raise ValueError('unsupported key: %s in %s' % (k, what))
                 current[k] = value[k]
             return current
@@ -153,11 +183,12 @@ class IMU(object):
 
     def set_gyro_error(self, gyro_error='low-accuracy'):
         """imu_model.py:207-236: grade string, or dict of {'b','arw','b_drift','b_corr'}
-        IN THE STORED (SI) UNITS, exactly as the reference assigns them."""
+        IN THE STORED (SI) UNITS, exactly as the reference assigns them, and of 'q', 'rrw', 'rr'
+        (Allan(fit=True)'s Q, K and R of a gyro axis: columns 0, 3 and 4 of noise_gyro)."""
         self.gyro_err = self._set(self.gyro_err, gyro_error, gyro_profile, 'gyro_error')
 
     def set_accel_error(self, accel_error='low-accuracy'):
-        """imu_model.py:238-267"""
+        """imu_model.py:238-267; also 'q', 'rrw', 'rr' as for set_gyro_error (noise_accel's columns)."""
         self.accel_err = self._set(self.accel_err, accel_error, accel_profile, 'accel_error')
 
     def set_mag_error(self, mag_error='low-accuracy'):

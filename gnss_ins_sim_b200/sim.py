@@ -36,7 +36,7 @@ from collections.abc import Mapping
 import numpy as np
 import torch
 
-from . import engine, dist, logged
+from . import _lib, engine, dist, logged
 from .free_integration import FreeIntegration
 from .free_integration_odo import FreeIntegration as FreeIntegrationOdo
 from .series_analysis import SeriesEstimator
@@ -401,6 +401,7 @@ class Sim(object):
         self.seed = int(seed)
         self.lanes_per_run = int(lanes_per_run)
         self.history_block = int(history_block)
+        self._force_fed = False    # tests: run free integration as K1 then K2 even without the IMU's extra terms
         self.run_base = int(run_base)
         self.wmm_file, self.wmm_date = wmm_file, wmm_date
         self.data_src = motion_def
@@ -477,6 +478,11 @@ class Sim(object):
             return self._run_logged()
         if self.imu is None:
             raise ValueError('imu must be an IMU model when data are generated from a trajectory')
+        terms = self._imu_terms()
+        for a in self.algo or []:       # refused before anything of the Sim is reset
+            if terms and isinstance(a, (InsLoose, FreeIntegrationOdo)):
+                raise ValueError('%s generates its IMU inside its kernel, which makes no quantisation, rate '
+                                 'random walk or rate ramp: the IMU sets %s' % (type(a).__name__, terms))
         self._blocks = {}        # (block, name) -> [runs of the block, ...] host histories (_history)
         self._proc = {}          # (algo index, start [s], position frame) -> [R, 3, 9] process statistics
         self._sens = {}          # (source, first row) -> sensor error statistics (_sensor_launch)
@@ -720,12 +726,53 @@ class Sim(object):
     def _uses_psd(self):
         return any(v is not None and v['type'] == 'psd' for v in (self._vib_acc, self._vib_gyro))
 
+    def _imu_terms(self):
+        """The IEEE Std 952 terms the IMU sets (non-zero 'q', 'rrw', 'rr'), e.g. ['gyro rrw']; [] for none."""
+        return ['%s %s' % (s, k) for s, err in (('gyro', self.imu.gyro_err), ('accel', self.imu.accel_err))
+                for k in _lib.set_terms(err)]
+
+    def _fed(self, ai):
+        """True if free-integration plugin ai runs as K1 then K2 on the materialised series (the IMU has terms
+        K12's generator does not make) instead of K12."""
+        return not isinstance(self.algo[ai], FreeIntegrationOdo) and (self._force_fed or bool(self._imu_terms()))
+
+    def _fed_blocks(self, ai, lo, hi):
+        """K1 (with the IMU's terms) then K2 for experiment runs [lo, hi) of free-integration plugin ai, in run
+        blocks sized to the free device memory (120 B per run-sample: the series and the histories): yields
+        (r0, att, pos, vel, gyro, accel), CUDA [runs, n, 3].  Philox makes a block's rerun identical."""
+        algo = self.algo[ai]
+        block = max(1, min(hi - lo, self._allan_block(120, 3)))
+        for r0 in range(lo, hi, block):
+            r1 = min(hi, r0 + block)
+            gyro, accel = self._noise_block(r0, r1)
+            att, pos, vel = engine.free_integration(self.ref_frame, self.fs[0], gyro, accel, algo.ini_device(),
+                                                    earth_rot=algo.earth_rot,
+                                                    run_offset=self._mc[ai]['base'] + r0)
+            yield r0, att, pos, vel, gyro, accel
+            del att, pos, vel, gyro, accel
+
+    def _fed_errors(self, att, pos, vel, frame=0, rows=slice(None)):
+        """[runs, rows, 9] host errors of K2 history rows against the trajectory's: attitude wrapped to [-pi, pi),
+        position in the frame's units (engine.POS_FRAME_*), velocity."""
+        ref = {k: self._traj[k][rows] for k in ('ref_att', 'ref_pos', 'ref_vel')}
+        ea = (att[:, rows].cpu().numpy() - ref['ref_att'][None] + math.pi) % (2.0 * math.pi) - math.pi
+        x = pos[:, rows].cpu().numpy()
+        ep = np.stack([lla_error_metres(xr, ref['ref_pos'], frame) for xr in x]) if frame else x - ref['ref_pos'][None]
+        return np.concatenate([ea, ep, vel[:, rows].cpu().numpy() - ref['ref_vel'][None]], axis=2)
+
     def _run_free_integration(self, i, algo):
         name = self.algo_name(i)
         lo, hi = self._shard
         self._mc[i] = {'base': algo.run_times, 'end_err': None}   # plugin's run counter at run 0
         err, stats = np.zeros((0, 9)), np.zeros((3, 9))
-        if not isinstance(algo, FreeIntegrationOdo):
+        if self._fed(i):
+            if hi > lo:
+                err = np.concatenate([self._fed_errors(a, p, v, rows=slice(-1, None))[:, 0]
+                                      for _, a, p, v, _, _ in self._fed_blocks(i, lo, hi)])
+                stats = engine.error_stats(engine.to_device(err)).cpu().numpy()
+            self._mc[i]['end_err'] = err
+            self.err_stats[name] = dist.combine_local_stats(stats, hi - lo)
+        elif not isinstance(algo, FreeIntegrationOdo):
             # the plan path on this rank's shard (pinned staging, one H2D, K12, K3, one D2H);
             # with several ranks the [3][9] shard statistics are merged by one all_gather
             # the exchange path is chosen from the LARGEST shard, a rank-independent quantity (shards
@@ -842,7 +889,7 @@ class Sim(object):
         lo, hi = self._shard
         n = self._traj['ref_gyro'].shape[0]
         fused = (algo.fused and self._vib_acc is None and self._vib_gyro is None and n > 5040
-                 and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
+                 and not self._imu_terms() and os.environ.get('B2INS_ALLAN_FUSED', '1') != '0')
         fit = getattr(algo, 'fit', False)
         tau = algo.abscissa(n, self.fs[0])
         block = self._allan_block(6 * 2, 2) if fused else self._allan_block(algo.run_bytes(n), 3)
@@ -1019,6 +1066,13 @@ class Sim(object):
             res = self._ekf_launch(self.algo[name[0]], r0, runs, dump_runs=runs)
             return {(name[0], k): v.cpu().numpy() for k, v in (('att_euler', res.att), ('pos', res.pos),
                                                                ('vel', res.vel), ('wb', res.wb), ('ab', res.ab))}
+        if isinstance(name, tuple) and self._fed(name[0]):
+            out = {}
+            for b0, att, pos, vel, gyro, accel in self._fed_blocks(name[0], r0, r0 + runs):
+                for k, v in (((name[0], 'att_euler'), att), ((name[0], 'pos'), pos), ((name[0], 'vel'), vel),
+                             ('gyro', gyro), ('accel', accel)):
+                    out.setdefault(k, []).append(v.cpu().numpy())
+            return {k: np.concatenate(v) for k, v in out.items()}
         if isinstance(name, tuple):
             res = self._mc_launch(name[0], r0, runs, dump_runs=runs, dump_nav=True, dump_imu=True)
             out = {(name[0], k): v.cpu().numpy() for k, v in (('att_euler', res.att), ('pos', res.pos),
@@ -1055,6 +1109,21 @@ class Sim(object):
             n = self._traj['ref_gyro'].shape[0]
             return {k: np.zeros((0, n, 3)) for k in ('att_euler', 'pos', 'vel')}
         stride = max(1, int(stride))
+        if self._fed(algo_index):
+            parts = {}
+            for _, att, pos, vel, gyro, accel in self._fed_blocks(algo_index, lo, hi):
+                names = [('att_euler', att), ('pos', pos), ('vel', vel)] + ([('gyro', gyro), ('accel', accel)]
+                                                                             if imu else [])
+                for k, t in names:
+                    parts.setdefault(k, []).append(t[:, ::stride].cpu().numpy())
+            out = {k: np.concatenate(v) for k, v in parts.items()}
+            if quat:
+                out['att_quat'] = np.stack([euler2quat_zyx(a) for a in out['att_euler']])
+            if stride == 1:
+                self._all_hist = (algo_index, lo, out)
+            else:
+                out['time'] = self.data['time'][::stride]
+            return out
         pool = _hist_pool(self)      # device + pinned buffers: this Sim's, or a dead Sim's (never a live one's)
         res = self._mc_launch(algo_index, lo, runs, dump_runs=runs, dump_stride=stride, dump_nav=True,
                               dump_imu=imu, out=pool.get('res'), dump_quat=quat)
@@ -1346,6 +1415,11 @@ class Sim(object):
                     ps = torch.cat([r.proc_stats for r in self._ekf_blocks(algo, proc_start=start,
                                                                            proc_pos_frame=frame)])
                     ps = ps.reshape(hi - lo, 27)
+                elif hi > lo and self._fed(algo_index):
+                    # K2's histories of each block, reduced on the host as for logged results
+                    ps = torch.from_numpy(np.concatenate([
+                        np.stack([_host_stats(e) for e in self._fed_errors(a, p, v, frame, slice(start, None))])
+                        for _, a, p, v, _, _ in self._fed_blocks(algo_index, lo, hi)]).reshape(hi - lo, 27))
                 elif hi > lo:
                     ps = self._mc_launch(algo_index, lo, hi - lo, stats_start=start,
                                          proc_pos_frame=frame).proc_stats.reshape(hi - lo, 27)

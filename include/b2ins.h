@@ -63,6 +63,18 @@ typedef struct b2ins_sensor_err {
   double rw[3];      /* 'arw' [rad/s/sqrt(Hz)] or 'vrw' [m/s^2/sqrt(Hz)] */
 } b2ins_sensor_err;
 
+/* The IEEE Std 952 terms of one triad that b2ins_sensor_err does not hold (DESIGN.md section 4), in the units of
+ * the Allan noise identification's columns Q, K and R (b2ins_allan_fit_f64).  Per axis c, sample t, dt = 1/fs:
+ *   q: quantisation [rad; accel m/s]: e[t] = q sqrt(12) (u[t] - 1/2), u uniform in [0, 1); rate error (e[t+1] - e[t]) / dt
+ *   k: rate random walk [rad/s^2/sqrt(Hz); accel m/s^3/sqrt(Hz)]: w[0] = 0, w[t+1] = w[t] + k sqrt(dt) z[t]
+ *   r: rate ramp [rad/s^2; accel m/s^3]: r t dt, the same in every run
+ * q and k must be finite and >= 0, r finite. */
+typedef struct b2ins_noise_terms {
+  double q[3];
+  double k[3];
+  double r[3];
+} b2ins_noise_terms;
+
 /* Vibration model of one triad: Sim.__parse_env output (ins_sim.py:642-701). */
 typedef struct b2ins_vib {
   int32_t type; /* B2INS_VIB_* */
@@ -320,6 +332,24 @@ int b2ins_imu_noise_f64_host(double fs, int64_t runs, int64_t n,
                              const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
                              uint64_t seed, int64_t run_offset, int layout,
                              double* gyro, double* accel, double* z_dump);
+
+/* K1 with the terms of b2ins_noise_terms added to every measurement (gyro_terms / accel_terms nullable: none).
+ * Sensor 0 is accel, sensor 1 gyro; the walk of axis c draws pair 32 + 3 sensor + c (z0), the quantisation
+ * uniform of sample t draw 38 + 3 sensor + c.  With every term zero these are b2ins_imu_noise_f64[_host]. */
+int b2ins_imu_noise_ex_f64(double fs, int64_t runs, int64_t n,
+                           const double* ref_gyro, const double* ref_accel,
+                           const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                           const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                           const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                           uint64_t seed, int64_t run_offset, int layout,
+                           double* gyro, double* accel, double* z_dump, void* stream);
+int b2ins_imu_noise_ex_f64_host(double fs, int64_t runs, int64_t n,
+                                const double* ref_gyro, const double* ref_accel,
+                                const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                                const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                                const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                                uint64_t seed, int64_t run_offset, int layout,
+                                double* gyro, double* accel, double* z_dump);
 
 /* ---- K12: fused Monte-Carlo run (noise -> integration -> per-run errors) --
  * Replaces loop A (ins_sim.py:490-496) + loop B (ins_algo_manager.py:73-95) + the per-run
@@ -587,6 +617,14 @@ int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n,
                             const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
                             uint64_t seed, int64_t run_offset, int64_t stats_start,
                             double* end_err, double* proc_stats, void* stream);
+/* K9 of the measurements b2ins_imu_noise_ex_f64 makes (same arguments); with every term zero, K9 itself. */
+int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n,
+                               const double* ref_gyro, const double* ref_accel,
+                               const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                               const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                               const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                               uint64_t seed, int64_t run_offset, int64_t stats_start,
+                               double* end_err, double* proc_stats, void* stream);
 
 /* ---- K3p: per-run error statistics of a device array ----------------------------------
  * x [runs][m][ncomp] against the shared ref [m][ncomp] (device), e = x - ref:
@@ -660,6 +698,11 @@ int b2ins_diag_psd_plan(int64_t n, int* P);
  * Pure host logic: the function the launch calls. */
 int b2ins_diag_noise_plan(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
                           const b2ins_sensor_err* accel_err, int sm_count, double* coef, int64_t* plan);
+/* The plan of the _ex entry points: as above; a non-zero rate random walk (k) never decays, so pass 1 then
+ * covers whole segments (pass1_len = seg_len). */
+int b2ins_diag_noise_plan_ex(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
+                             const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                             const b2ins_noise_terms* accel_terms, int sm_count, double* coef, int64_t* plan);
 
 /* The device's own FP64 primitives (csrc/fastmath64.cuh, and mech.cuh's sincos_angle), applied
  * elementwise to n arguments: out0[i] = f(a[i]) (div: a[i] / b[i]); the sin/cos functions write

@@ -118,6 +118,11 @@ def main():
     engine.imu_err_stats(100.0, 5, rg, ra, MID_G, MID_A, 1, stats_start=250)
     engine.imu_err_stats(100.0, 5, rg, ra, MID_G, MID_A, 1)
     engine.imu_err_stats(100.0, 1, long_g, long_g, MID_G, MID_A, 1, stats_start=1000)
+    # K1-ex and K9-ex with the IEEE Std 952 terms: a segmented plan with a ragged last tile (n = 300 001)
+    tg, ta = dict(MID_G, q=np.full(3, 1e-6), rrw=np.full(3, 2e-6), rr=np.full(3, 1e-7)), dict(MID_A, rrw=np.full(3, 1e-4))
+    long_r = engine.to_device(np.zeros((300001, 3)))
+    engine.imu_noise(100.0, 1, long_r, long_r, tg, ta, 1)
+    engine.imu_err_stats(100.0, 1, long_r, long_r, tg, ta, 1, stats_start=1000)
     engine.proc_stats(mag, ref_mag, 7)
     torch.cuda.synchronize()
     print('sanitize smoke ok')
