@@ -26,6 +26,10 @@ class NoiseTerms(ctypes.Structure):
     _fields_ = [('q', ctypes.c_double * 3), ('k', ctypes.c_double * 3), ('r', ctypes.c_double * 3)]
 
 
+class RunErr(ctypes.Structure):
+    _fields_ = [('b', ctypes.c_double * 3), ('sf', ctypes.c_double * 3), ('ma', (ctypes.c_double * 3) * 3)]
+
+
 class Vib(ctypes.Structure):
     _fields_ = [('type', ctypes.c_int32), ('series_len', ctypes.c_int32),
                 ('amp', ctypes.c_double * 3), ('freq', ctypes.c_double),
@@ -70,7 +74,7 @@ class B2insError(RuntimeError):
 
 _I, _L, _D, _P, _U64 = ctypes.c_int, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p, ctypes.c_uint64
 _SE, _VB, _MC = ctypes.POINTER(SensorErr), ctypes.POINTER(Vib), ctypes.POINTER(McConfig)
-_NT = ctypes.POINTER(NoiseTerms)
+_NT, _RE = ctypes.POINTER(NoiseTerms), ctypes.POINTER(RunErr)
 
 # name -> (restype, argtypes); every symbol include/b2ins.h declares
 SIGNATURES = {
@@ -85,6 +89,11 @@ SIGNATURES = {
     'b2ins_imu_noise_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
     'b2ins_imu_noise_ex_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _I, _P, _P, _P, _P]),
     'b2ins_imu_noise_ex_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _I, _P, _P, _P]),
+    'b2ins_imu_noise_rx_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _I, _P, _P, _P, _RE,
+                                    _RE, _P]),
+    'b2ins_imu_noise_rx_f64_host': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _I, _P, _P, _P,
+                                         _RE, _RE]),
+    'b2ins_imu_run_err_f64': (_I, [_U64, _L, _L, _RE, _RE, _P, _P]),
     'b2ins_gps_noise_f64': (_I, [_L, _L, _P, _P, _P, _I, _U64, _L, _P, _P]),
     'b2ins_mag_noise_f64': (_I, [_L, _L, _P, _P, _P, _P, _U64, _L, _P, _P]),
     'b2ins_magcal_f64': (_I, [_L, _L, c_int64_p, _P, _P, _P, _P, _U64, _L, _P, _P, _P, _P]),
@@ -92,6 +101,8 @@ SIGNATURES = {
     'b2ins_magcal_fed_f64_host': (_I, [_L, _L, c_int64_p, _P, _L, _L, _P, _P, _P]),
     'b2ins_imu_err_stats_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _VB, _VB, _U64, _L, _L, _P, _P, _P]),
     'b2ins_imu_err_stats_ex_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _L, _P, _P, _P]),
+    'b2ins_imu_err_stats_rx_f64': (_I, [_D, _L, _L, _P, _P, _SE, _SE, _NT, _NT, _VB, _VB, _U64, _L, _L, _P, _P, _RE,
+                                        _RE, _P]),
     'b2ins_proc_stats_f64': (_I, [_L, _L, _I, _P, _P, _L, _P, _P, _P]),
     'b2ins_mc_free_integration_f64': (_I, [_MC, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'b2ins_mc_free_integration_ex_f64': (_I, [_MC, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
@@ -261,6 +272,32 @@ def noise_terms(err):
         for c in range(3):
             getattr(t, f)[c] = float(v[c])
     return t
+
+
+RUN_ERR_KEYS = ('b_std', 'sf', 'ma')    # an imu_model dict's run-to-run errors (1 sigma, SI units)
+
+
+def set_run_errors(err):
+    """The run-to-run errors an imu_model dict sets: its keys among RUN_ERR_KEYS with a non-zero value."""
+    return [k for k in RUN_ERR_KEYS if k in err and np.any(np.asarray(err[k], dtype=np.float64) != 0.0)]
+
+
+def run_err(err):
+    """imu_model dict -> RunErr (absent keys: zero; 'ma' a scalar for every off-diagonal or 3x3), or None when it
+    has no non-zero run error: the _rx entry points then launch what the _ex ones do."""
+    if not set_run_errors(err):
+        return None
+    e = RunErr()
+    for f, k in (('b', 'b_std'), ('sf', 'sf')):
+        v = np.broadcast_to(np.asarray(err.get(k, 0.0), dtype=np.float64), (3,))
+        for c in range(3):
+            getattr(e, f)[c] = float(v[c])
+    ma = np.asarray(err.get('ma', 0.0), dtype=np.float64)
+    ma = ma * (1.0 - np.eye(3)) if ma.ndim == 0 else ma.reshape(3, 3)
+    for i in range(3):
+        for j in range(3):
+            e.ma[i][j] = float(ma[i, j])
+    return e
 
 
 def vib(vib_def, series_ptr=None, series_len=0):

@@ -394,6 +394,33 @@ int digest_terms(const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* a
   return B2INS_OK;
 }
 
+// the run-to-run errors of the two triads for the device (accel, then gyro), checked; *any is false when both are
+// null or all zero, and the _rx entry points then launch exactly what the _ex ones launch
+int digest_run_err(const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, RunErrs* re, bool* any) {
+  std::memset(re, 0, sizeof(*re));
+  *any = false;
+  const b2ins_run_err* e[2] = {accel_run, gyro_run};
+  for (int s = 0; s < 2; ++s) {
+    if (!e[s]) continue;
+    for (int c = 0; c < 3; ++c) {
+      ARG_CHECK(std::isfinite(e[s]->b[c]) && e[s]->b[c] >= 0.0 && std::isfinite(e[s]->sf[c]) && e[s]->sf[c] >= 0.0,
+                "run errors: b, sf and ma must be finite and >= 0");
+      for (int j = 0; j < 3; ++j)
+        ARG_CHECK(std::isfinite(e[s]->ma[c][j]) && e[s]->ma[c][j] >= 0.0,
+                  "run errors: b, sf and ma must be finite and >= 0");
+      ARG_CHECK(e[s]->ma[c][c] == 0.0, "run errors: the diagonal of ma must be 0");
+      re->s[s].b[c] = e[s]->b[c];
+      re->s[s].sf[c] = e[s]->sf[c];
+      *any = *any || e[s]->b[c] != 0.0 || e[s]->sf[c] != 0.0;
+      for (int j = 0; j < 3; ++j) {
+        re->s[s].ma[c][j] = e[s]->ma[c][j];
+        *any = *any || e[s]->ma[c][j] != 0.0;
+      }
+    }
+  }
+  return B2INS_OK;
+}
+
 // K1's parameters and time segmentation, shared by K1 and K9; with segments, pass 1 and the carry chain are
 // launched here and *scratch holds their buffers until the caller has queued pass 0 on s.  x (nullable): the
 // IEEE Std 952 terms, whose rate random walk is carried across the segments like the drift, with a = 1.
@@ -581,18 +608,23 @@ int b2ins_free_integration_f64_host(int ref_frame, double fs, int64_t runs, int6
 }
 
 // ---------------------------------------------------------------- K1 --------
-int b2ins_imu_noise_ex_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
+int b2ins_imu_noise_rx_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
                            const double* ref_accel, const b2ins_sensor_err* gyro_err,
                            const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
                            const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro,
                            const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, int layout,
-                           double* gyro, double* accel, double* z_dump, void* stream) {
+                           double* gyro, double* accel, double* z_dump, const b2ins_run_err* gyro_run,
+                           const b2ins_run_err* accel_run, void* stream) {
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   ARG_CHECK(layout >= 0 && layout <= 2, "layout must be B2INS_LAYOUT_*");
   NoiseTerms x;
   bool terms = false, walk = false;
   int rc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
+  if (rc != B2INS_OK) return rc;
+  RunErrs re;
+  bool runerr = false;
+  rc = digest_run_err(gyro_run, accel_run, &re, &runerr);
   if (rc != B2INS_OK) return rc;
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && gyro && accel, "null buffer");
@@ -607,13 +639,29 @@ int b2ins_imu_noise_ex_f64(double fs, int64_t runs, int64_t n, const double* ref
   p.out_accel = accel;
   layout_strides(layout, runs, n, &p.osr, &p.ost, &p.osc);
   p.z_dump = z_dump;
-  if (terms)
-    imu_noise_ex_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p, x);
+  const unsigned ctas = static_cast<unsigned>(runs * p.nseg);
+  if (terms && runerr)
+    imu_noise_ex_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(p, x, re);
+  else if (terms)
+    imu_noise_ex_kernel<<<ctas, kNoiseThreads, 0, s>>>(p, x);
+  else if (runerr)
+    imu_noise_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(p, re);
   else
-    imu_noise_kernel<<<static_cast<unsigned>(runs * p.nseg), kNoiseThreads, 0, s>>>(p);
+    imu_noise_kernel<<<ctas, kNoiseThreads, 0, s>>>(p);
   CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
+}
+
+int b2ins_imu_noise_ex_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
+                           const double* ref_accel, const b2ins_sensor_err* gyro_err,
+                           const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                           const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro,
+                           const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, int layout,
+                           double* gyro, double* accel, double* z_dump, void* stream) {
+  return b2ins_imu_noise_rx_f64(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, gyro_terms, accel_terms,
+                                vib_gyro, vib_accel, seed, run_offset, layout, gyro, accel, z_dump, nullptr, nullptr,
+                                stream);
 }
 
 int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro,
@@ -625,13 +673,28 @@ int b2ins_imu_noise_f64(double fs, int64_t runs, int64_t n, const double* ref_gy
                                 vib_accel, seed, run_offset, layout, gyro, accel, z_dump, stream);
 }
 
+int b2ins_imu_run_err_f64(uint64_t seed, int64_t runs, int64_t run_offset, const b2ins_run_err* gyro_run,
+                          const b2ins_run_err* accel_run, double* out, void* stream) {
+  ARG_CHECK(runs >= 0, "runs must be non-negative");
+  RunErrs re;
+  bool any = false;
+  const int rc = digest_run_err(gyro_run, accel_run, &re, &any);
+  if (rc != B2INS_OK) return rc;
+  if (runs == 0) return B2INS_OK;
+  ARG_CHECK(out, "null buffer");
+  imu_run_err_kernel<<<static_cast<unsigned>((runs * 2 + 127) / 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+      re, runs, run_offset, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32), out);
+  CU_CHECK(cudaGetLastError());
+  return B2INS_OK;
+}
+
 // ---------------------------------------------------------------- K9 --------
-int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
+int b2ins_imu_err_stats_rx_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
                                const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
                                const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
                                const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel, uint64_t seed,
                                int64_t run_offset, int64_t stats_start, double* end_err, double* proc_stats,
-                               void* stream) {
+                               const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, void* stream) {
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   ARG_CHECK(stats_start < n || n == 0, "stats_start must be < n");
@@ -639,6 +702,10 @@ int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n, const double*
   bool terms = false, walk = false;
   const int trc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
   if (trc != B2INS_OK) return trc;
+  RunErrs re;
+  bool runerr = false;
+  const int xrc = digest_run_err(gyro_run, accel_run, &re, &runerr);
+  if (xrc != B2INS_OK) return xrc;
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && end_err, "null buffer");
   ARG_CHECK(stats_start < 0 || proc_stats, "stats_start >= 0 needs proc_stats");
@@ -659,10 +726,15 @@ int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n, const double*
       return fail(B2INS_ERR_CUDA, "cudaMallocAsync of the segment partials: %s", cudaGetErrorString(e));
     P.partial = partial.p;
   }
-  if (terms)
-    imu_err_stats_ex_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P, x);
+  const unsigned ctas = static_cast<unsigned>(runs * P.np.nseg);
+  if (terms && runerr)
+    imu_err_stats_ex_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, x, re);
+  else if (terms)
+    imu_err_stats_ex_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, x);
+  else if (runerr)
+    imu_err_stats_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, re);
   else
-    imu_err_stats_kernel<<<static_cast<unsigned>(runs * P.np.nseg), kNoiseThreads, 0, s>>>(P);
+    imu_err_stats_kernel<<<ctas, kNoiseThreads, 0, s>>>(P);
   if (partial.p) {
     err_stats_fold_kernel<<<static_cast<unsigned>((runs * kErrCh + 127) / 128), 128, 0, s>>>(P);
     CU_CHECK(partial.free());
@@ -670,6 +742,17 @@ int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n, const double*
   CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
+}
+
+int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
+                               const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                               const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                               const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel, uint64_t seed,
+                               int64_t run_offset, int64_t stats_start, double* end_err, double* proc_stats,
+                               void* stream) {
+  return b2ins_imu_err_stats_rx_f64(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, gyro_terms, accel_terms,
+                                    vib_gyro, vib_accel, seed, run_offset, stats_start, end_err, proc_stats, nullptr,
+                                    nullptr, stream);
 }
 
 int b2ins_imu_err_stats_f64(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
@@ -856,7 +939,23 @@ int b2ins_imu_noise_ex_f64_host(double fs, int64_t runs, int64_t n, const double
                                 const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro,
                                 const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
                                 int layout, double* gyro, double* accel, double* z_dump) {
+  return b2ins_imu_noise_rx_f64_host(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, gyro_terms, accel_terms,
+                                     vib_gyro, vib_accel, seed, run_offset, layout, gyro, accel, z_dump, nullptr,
+                                     nullptr);
+}
+
+int b2ins_imu_noise_rx_f64_host(double fs, int64_t runs, int64_t n, const double* ref_gyro,
+                                const double* ref_accel, const b2ins_sensor_err* gyro_err,
+                                const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                                const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro,
+                                const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset,
+                                int layout, double* gyro, double* accel, double* z_dump,
+                                const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run) {
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
+  RunErrs re;
+  bool runerr = false;
+  const int rc = digest_run_err(gyro_run, accel_run, &re, &runerr);
+  if (rc != B2INS_OK) return rc;
   if (runs == 0 || n == 0) return B2INS_OK;
   ARG_CHECK(ref_gyro && ref_accel && gyro && accel, "null buffer");
   ARG_CHECK(!(vib_gyro && vib_gyro->type == B2INS_VIB_SERIES) &&
@@ -870,8 +969,8 @@ int b2ins_imu_noise_ex_f64_host(double fs, int64_t runs, int64_t n, const double
   double* oa = st.out(accel, elems);
   double* zd = z_dump ? st.out(z_dump, elems * 4) : nullptr;
   return st.run([&](cudaStream_t s) {
-    return b2ins_imu_noise_ex_f64(fs, runs, n, rg, ra, gyro_err, accel_err, gyro_terms, accel_terms, vib_gyro,
-                                  vib_accel, seed, run_offset, layout, og, oa, zd, s);
+    return b2ins_imu_noise_rx_f64(fs, runs, n, rg, ra, gyro_err, accel_err, gyro_terms, accel_terms, vib_gyro,
+                                  vib_accel, seed, run_offset, layout, og, oa, zd, gyro_run, accel_run, s);
   });
 }
 

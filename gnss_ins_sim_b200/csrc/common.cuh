@@ -38,6 +38,8 @@ constexpr uint32_t kDrawMag = 13;   // magnetometer: 13 (x, y), 14 (z from z0)
 constexpr uint32_t kDrawPsd = 16;   // +3*sensor+axis, t = bin index: PSD random phases
 constexpr uint32_t kDrawRrw = 32;   // +3*sensor+axis: rate random walk drive (z0)
 constexpr uint32_t kDrawQuant = 38; // +3*sensor+axis: quantisation uniform (words x1:x0, as uniform01)
+constexpr uint32_t kDrawRunErr = 44;        // +6*sensor+j, t = kRunErrT: run-to-run bias, scale factor, misalignment
+constexpr uint32_t kRunErrT = 0xFFFFFFFDu;  // the run errors' counter (0xFFFFFFFF: phases, 0xFFFFFFFE: filter state)
 
 struct PhiloxOut {
   uint32_t x0, x1, x2, x3;

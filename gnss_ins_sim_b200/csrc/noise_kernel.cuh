@@ -102,6 +102,43 @@ __device__ __forceinline__ void terms_sample(const NoiseParams& p, const NoiseTe
   }
 }
 
+// The run-to-run errors of b2ins_run_err (DESIGN.md section 4): the 1-sigma values of one sensor, SI units
+struct RunErrSigma {
+  double b[3];          // turn-on bias
+  double sf[3];         // scale factor
+  double ma[3][3];      // misalignment: sensitivity of sensor axis i to true axis j (zero diagonal)
+};
+struct RunErrs {
+  RunErrSigma s[2];     // accel, gyro
+};
+
+// pair j (0..5) of one sensor's run errors, drawn from the global run id: e12 = (S row-major [9], b_run [3]) with
+// S = diag(sf) + ma.  j < 3: (z0, z1) -> (b_run[j], sf[j]); j >= 3: the off-diagonals of row j - 3 in column order.
+// K1's and K9's prologues (one thread per pair) and imu_run_err_kernel (one thread per sensor) share it.
+__device__ __forceinline__ void run_err_pair(const RunErrSigma& s, int sensor, int j, uint32_t run_lo,
+                                             uint32_t run_hi, uint32_t k0, uint32_t k1, double* e12) {
+  const Normal2 z = normal_pair(kRunErrT, kDrawRunErr + 6 * sensor + j, run_lo, run_hi, k0, k1);
+  if (j < 3) {
+    e12[9 + j] = s.b[j] * z.z0;
+    e12[4 * j] = s.sf[j] * z.z1;
+  } else {
+    const int i = j - 3, c0 = (i == 0) ? 1 : 0, c1 = (i == 2) ? 1 : 2;
+    e12[3 * i + c0] = s.ma[i][c0] * z.z0;
+    e12[3 * i + c1] = s.ma[i][c1] * z.z1;
+  }
+}
+
+// + delta[c] = b_run[c] + sum_j S[c][j] ref[j] on one triad; e12 in shared memory (broadcast reads)
+__device__ __forceinline__ void run_err_add(const double* e12, const double* ref3, double* m3) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    double d = e12[9 + c];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) d = fma(e12[3 * c + j], ref3[j], d);
+    m3[c] += d;
+  }
+}
+
 // the prologue of a K1 or K9 CTA, before its first __syncthreads: a^q per channel into apow[kNoisePer + 1][6],
 // the run's sinusoidal gyro-vibration phase and, with carry_in, the Gauss-Markov state at the segment start
 // (zero without)
@@ -134,13 +171,17 @@ __device__ __forceinline__ void noise_prologue(const NoiseParams& p, double (*ap
 
 // K1's body.  TERMS adds the IEEE Std 952 terms of x (DESIGN.md section 4): the rate random walk k runs as six
 // more channels of the affine scan with A = 1, the quantisation error carries e[t+1] along the thread's stretch
-// (one extra uniform at its start), the rate ramp is R t dt.  Without TERMS this is K1 as it always was.
-template <bool TERMS>
-__device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const NoiseTerms* x) {
+// (one extra uniform at its start), the rate ramp is R t dt.  RUNERR adds the run-to-run errors of re: the CTA's
+// run makes its (S, b_run) of both sensors in the prologue into shared memory (12 threads, one pair each), and
+// every triad gets delta = b_run + S ref from there; it has no state in time, so segments carry nothing for it.
+// Without TERMS and RUNERR this is K1 as it always was.
+template <bool TERMS, bool RUNERR>
+__device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const NoiseTerms* x, const RunErrs* re) {
   constexpr int C = TERMS ? 12 : 6;               // scanned channels: drift (accel, gyro), then the walk
   __shared__ double stage[2][kNoiseTile * 3];     // accel, gyro of the tile, [sample][axis]
   __shared__ double wtot[C][kNoiseWarps][2];      // (A, E) of every warp's stretch, per channel
   __shared__ double apow[kNoisePer + 1][6];       // a^q per channel
+  __shared__ double rerr[RUNERR ? 2 : 1][12];     // RUNERR: (S row-major, b_run) of accel, gyro for this run
   const int segs = (p.pass == 1) ? p.nseg - 1 : p.nseg;
   const int64_t run = blockIdx.x / segs;
   const int seg = static_cast<int>(blockIdx.x % segs);
@@ -154,6 +195,9 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
   if constexpr (TERMS) {
 #pragma unroll
     for (int c = 0; c < 6; ++c) carry[6 + c] = (p.pass == 0 && x->seg_carry) ? x->seg_carry[(run * p.nseg + seg) * 6 + c] : 0.0;
+  }
+  if constexpr (RUNERR) {
+    if (tid < 12) run_err_pair(re->s[tid / 6], tid / 6, tid % 6, run_lo, run_hi, p.k0, p.k1, rerr[tid / 6]);
   }
   __syncthreads();
 
@@ -182,11 +226,17 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
       triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase,
                       p.pass == 1, r, m3);
       if constexpr (TERMS) terms_sample<0>(p, *x, t, run_lo, run_hi, p.pass == 1, r + 6, qe, m3);
+      if constexpr (RUNERR) {
+        if (p.pass == 0) run_err_add(rerr[0], p.ref_accel + t * 3, m3);
+      }
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
       triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase,
                       p.pass == 1, r + 3, m3);
       if constexpr (TERMS) terms_sample<1>(p, *x, t, run_lo, run_hi, p.pass == 1, r + 9, qe + 3, m3);
+      if constexpr (RUNERR) {
+        if (p.pass == 0) run_err_add(rerr[1], p.ref_gyro + t * 3, m3);
+      }
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
     }
@@ -263,12 +313,35 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
 }
 
 __global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_kernel(const __grid_constant__ NoiseParams p) {
-  imu_noise_body<false>(p, nullptr);
+  imu_noise_body<false, false>(p, nullptr, nullptr);
 }
 
 __global__ void __launch_bounds__(kNoiseThreads, 3) imu_noise_ex_kernel(const __grid_constant__ NoiseParams p,
                                                                       const __grid_constant__ NoiseTerms x) {
-  imu_noise_body<true>(p, &x);
+  imu_noise_body<true, false>(p, &x, nullptr);
+}
+
+// K1-rx: the run-to-run errors alone, and with the IEEE Std 952 terms
+__global__ void __launch_bounds__(kNoiseThreads, 4) imu_noise_rx_kernel(const __grid_constant__ NoiseParams p,
+                                                                      const __grid_constant__ RunErrs re) {
+  imu_noise_body<false, true>(p, nullptr, &re);
+}
+
+__global__ void __launch_bounds__(kNoiseThreads, 3) imu_noise_ex_rx_kernel(const __grid_constant__ NoiseParams p,
+                                                                         const __grid_constant__ NoiseTerms x,
+                                                                         const __grid_constant__ RunErrs re) {
+  imu_noise_body<true, true>(p, &x, &re);
+}
+
+// the run-error table: one thread per (run, sensor) writes out[run][sensor][12] = (S row-major, b_run)
+__global__ void imu_run_err_kernel(const __grid_constant__ RunErrs re, int64_t runs, int64_t run_offset, uint32_t k0,
+                                   uint32_t k1, double* out) {
+  const int64_t idx = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= runs * 2) return;
+  const int sensor = static_cast<int>(idx % 2);
+  const int64_t grun = run_offset + idx / 2;
+  const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
+  for (int j = 0; j < 6; ++j) run_err_pair(re.s[sensor], sensor, j, run_lo, run_hi, k0, k1, out + idx * 12);
 }
 
 // carry-in of every segment from the zero-state segment responses: c[s+1] = a^L c[s] + E[s]

@@ -60,14 +60,16 @@ __device__ __forceinline__ void write_stats(double* ps, int c, int nc, double n,
   ps[2 * nc + c] = n > 0.0 ? sqrt(m2 / n) : none;
 }
 
-// K9's body; TERMS: with the IEEE Std 952 terms of x, generated as K1's imu_noise_body<true> makes them
-template <bool TERMS>
-__device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, const NoiseTerms* x) {
+// K9's body; TERMS: with the IEEE Std 952 terms of x, RUNERR: with the run-to-run errors of re, generated as K1's
+// imu_noise_body<TERMS, RUNERR> makes them
+template <bool TERMS, bool RUNERR>
+__device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, const NoiseTerms* x, const RunErrs* re) {
   constexpr int C = TERMS ? 12 : 6;
   const NoiseParams& p = P.np;
   __shared__ double stage[2][kNoiseTile * 3];     // accel, gyro of the tile, [sample][axis]
   __shared__ double wtot[C][kNoiseWarps][2];
   __shared__ double apow[kNoisePer + 1][6];
+  __shared__ double rerr[RUNERR ? 2 : 1][12];     // RUNERR: (S row-major, b_run) of accel, gyro for this run
   const int64_t run = blockIdx.x / p.nseg;
   const int seg = static_cast<int>(blockIdx.x % p.nseg);
   const int64_t seg_hi = min64(p.n, (seg + 1) * p.seg_len);
@@ -81,6 +83,9 @@ __device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, cons
   if constexpr (TERMS) {
 #pragma unroll
     for (int c = 0; c < 6; ++c) carry[6 + c] = x->seg_carry ? x->seg_carry[(run * p.nseg + seg) * 6 + c] : 0.0;
+  }
+  if constexpr (RUNERR) {
+    if (tid < 12) run_err_pair(re->s[tid / 6], tid / 6, tid % 6, run_lo, run_hi, p.k0, p.k1, rerr[tid / 6]);
   }
   double an = 0.0, am[6], a2[6], ax[6];           // the thread's running statistics
 #pragma unroll
@@ -111,11 +116,13 @@ __device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, cons
       triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase, false,
                       r, m3);
       if constexpr (TERMS) terms_sample<0>(p, *x, t, run_lo, run_hi, false, r + 6, qe, m3);
+      if constexpr (RUNERR) run_err_add(rerr[0], p.ref_accel + t * 3, m3);
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
       triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase, false,
                       r + 3, m3);
       if constexpr (TERMS) terms_sample<1>(p, *x, t, run_lo, run_hi, false, r + 9, qe + 3, m3);
+      if constexpr (RUNERR) run_err_add(rerr[1], p.ref_gyro + t * 3, m3);
 #pragma unroll
       for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
     }
@@ -242,12 +249,24 @@ __device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, cons
 }
 
 __global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_kernel(const __grid_constant__ ErrStatsParams P) {
-  imu_err_stats_body<false>(P, nullptr);
+  imu_err_stats_body<false, false>(P, nullptr, nullptr);
 }
 
 __global__ void __launch_bounds__(kNoiseThreads, 3) imu_err_stats_ex_kernel(const __grid_constant__ ErrStatsParams P,
                                                                           const __grid_constant__ NoiseTerms x) {
-  imu_err_stats_body<true>(P, &x);
+  imu_err_stats_body<true, false>(P, &x, nullptr);
+}
+
+// K9-rx: the run-to-run errors alone, and with the IEEE Std 952 terms
+__global__ void __launch_bounds__(kNoiseThreads, 4) imu_err_stats_rx_kernel(const __grid_constant__ ErrStatsParams P,
+                                                                          const __grid_constant__ RunErrs re) {
+  imu_err_stats_body<false, true>(P, nullptr, &re);
+}
+
+__global__ void __launch_bounds__(kNoiseThreads, 3)
+    imu_err_stats_ex_rx_kernel(const __grid_constant__ ErrStatsParams P, const __grid_constant__ NoiseTerms x,
+                               const __grid_constant__ RunErrs re) {
+  imu_err_stats_body<true, true>(P, &x, &re);
 }
 
 // the segments of every run, merged in segment order: one thread per (run, channel)

@@ -104,7 +104,8 @@ def free_integration_odo(ref_frame, fs, gyro, odo, ini, earth_rot=True, layout=L
 def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0,
               vib_gyro=None, vib_accel=None, layout=LAYOUT_RUN_MAJOR, dump_z=False):
     """K1.  ref_gyro/ref_accel: CUDA f64 [n,3]; *_err: imu_model dicts (with a non-zero 'q', 'rrw' or 'rr':
-    K1 with the IEEE Std 952 terms, b2ins_imu_noise_ex_f64).
+    K1 with the IEEE Std 952 terms, b2ins_imu_noise_ex_f64; with a non-zero 'b_std', 'sf' or 'ma': K1 with the
+    run-to-run errors, b2ins_imu_noise_rx_f64).
     Returns gyro, accel ([R,n,3], [n,3,R] or, LAYOUT_CHANNEL_MAJOR, [R,3,n]) and, if dump_z,
     z [R,n,12]."""
     _require_cuda()
@@ -119,7 +120,13 @@ def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offs
     vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
     tg, ta = _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err)
-    if tg is None and ta is None:
+    xg, xa = _lib.run_err(gyro_err), _lib.run_err(accel_err)
+    if xg is not None or xa is not None:
+        _lib.check(lib.b2ins_imu_noise_rx_f64(
+            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
+            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
+            _ptr(gyro), _ptr(accel), _ptr(z), xg, xa, _stream()))
+    elif tg is None and ta is None:
         _lib.check(lib.b2ins_imu_noise_f64(
             float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
             ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
@@ -130,6 +137,18 @@ def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offs
             ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
             _ptr(gyro), _ptr(accel), _ptr(z), _stream()))
     return (gyro, accel, z) if dump_z else (gyro, accel)
+
+
+def imu_run_errors(runs, gyro_err, accel_err, seed, run_offset=0):
+    """The run-to-run errors K1 and K9 draw for runs run_offset .. run_offset + runs - 1 (b2ins_imu_run_err_f64),
+    from the imu_model dicts' 'b_std', 'sf', 'ma' (absent: zero).  Returns CUDA f64 [R, 2, 3, 4]: sensor 0 accel,
+    1 gyro; row i = (S[i][0], S[i][1], S[i][2], b_run[i]) with S = diag(sf) + ma."""
+    _require_cuda()
+    lib = _lib.load()
+    out = torch.zeros((runs, 2, 12), dtype=torch.float64, device='cuda')
+    _lib.check(lib.b2ins_imu_run_err_f64(int(seed) & 0xFFFFFFFFFFFFFFFF, int(runs), int(run_offset),
+                                         _lib.run_err(gyro_err), _lib.run_err(accel_err), _ptr(out), _stream()))
+    return torch.cat([out[:, :, :9].reshape(runs, 2, 3, 3), out[:, :, 9:].reshape(runs, 2, 3, 1)], dim=3)
 
 
 def gps_noise(runs, ref_gps, gps_err, gps_type, seed, run_offset=0):
@@ -236,7 +255,13 @@ def imu_err_stats(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_
     vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
     va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
     tg, ta = _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err)
-    if tg is None and ta is None:
+    xg, xa = _lib.run_err(gyro_err), _lib.run_err(accel_err)
+    if xg is not None or xa is not None:
+        _lib.check(lib.b2ins_imu_err_stats_rx_f64(
+            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
+            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
+            _ptr(end_err), _ptr(proc), xg, xa, _stream()))
+    elif tg is None and ta is None:
         _lib.check(lib.b2ins_imu_err_stats_f64(
             float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
             ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),

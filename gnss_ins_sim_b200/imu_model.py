@@ -15,6 +15,9 @@ and, only where a dict accuracy gives them, the IEEE Std 952 terms the reference
 and R of Allan(fit=True)'s noise_gyro / noise_accel):
   gyro  q [rad], rrw [rad/s^2/sqrt(Hz)], rr [rad/s^2]
   accel q [m/s], rrw [m/s^3/sqrt(Hz)], rr [m/s^3]
+and the run-to-run errors (1 sigma, drawn once per Monte-Carlo run; DESIGN.md section 4):
+  gyro  b_std [rad/s], sf [-], ma [rad] (3x3, zero diagonal)
+  accel b_std [m/s^2], sf [-], ma [rad] (3x3, zero diagonal)
 """
 import math
 
@@ -74,6 +77,16 @@ _TERMS = {
               'accel_rr': ('rr', 1.0 / 3600.0)},         # m/s^2/h -> m/s^3
 }
 _TERM_KEYS = ('q', 'rrw', 'rr')
+# optional run-to-run errors (1 sigma): accuracy key -> (stored key, factor from the datasheet unit to SI)
+_RUN_ERRS = {
+    'gyro': {'gyro_b_std': ('b_std', D2R / 3600.0),       # deg/h -> rad/s
+             'gyro_sf': ('sf', 1e-6),                     # ppm
+             'gyro_ma': ('ma', D2R)},                     # deg -> rad
+    'accel': {'accel_b_std': ('b_std', 1.0),             # m/s^2
+              'accel_sf': ('sf', 1e-6),                   # ppm
+              'accel_ma': ('ma', D2R)},                   # deg -> rad
+}
+_RUN_ERR_KEYS = ('b_std', 'sf', 'ma')
 
 
 def _terms(accuracy, sensor):
@@ -88,6 +101,27 @@ def _terms(accuracy, sensor):
     return out
 
 
+def _run_err_value(key, stored, value):
+    """One run-to-run error in SI units, checked: b_std and sf [3], ma 3x3 (a scalar is every off-diagonal) with a
+    zero diagonal; every value finite and >= 0."""
+    v = np.array(value, dtype=np.float64)
+    if stored == 'ma':
+        v = v * (1.0 - np.eye(3)) if v.ndim == 0 else v.reshape(3, 3)
+        if np.any(np.diag(v) != 0.0):
+            raise ValueError('%s must have a zero diagonal' % key)
+    else:
+        v = np.broadcast_to(v, (3,)).copy()
+    if not np.all(np.isfinite(v)) or np.any(v < 0.0):
+        raise ValueError('%s must be finite and >= 0' % key)
+    return v
+
+
+def _run_errs(accuracy, sensor):
+    """The run-to-run errors of one sensor an accuracy dict gives, in SI units (absent keys are not stored)."""
+    return {stored: _run_err_value(key, stored, np.array(accuracy[key], dtype=np.float64) * scale)
+            for key, (stored, scale) in _RUN_ERRS[sensor].items() if key in accuracy}
+
+
 class IMU(object):
     """IMU error model; see the module docstring.  accuracy: 'low-accuracy' |
     'mid-accuracy' | 'high-accuracy' | dict with gyro_b [deg/h], gyro_arw [deg/sqrt(h)],
@@ -95,7 +129,10 @@ class IMU(object):
     accel_b_stability [m/s^2] and optionally gyro_b_corr / accel_b_corr [s] (missing ->
     inf -> white bias drift), mag_si, mag_hi, mag_std, and the IEEE Std 952 terms gyro_q [deg],
     gyro_rrw [deg/h/sqrt(h)], gyro_rr [deg/h^2], accel_q [m/s], accel_rrw [m/s^2/sqrt(h)],
-    accel_rr [m/s^2/h] (missing -> zero; stored as gyro_err / accel_err 'q', 'rrw', 'rr' in SI units)."""
+    accel_rr [m/s^2/h] (missing -> zero; stored as gyro_err / accel_err 'q', 'rrw', 'rr' in SI units), and the
+    run-to-run errors (1 sigma) gyro_b_std [deg/h], accel_b_std [m/s^2], gyro_sf / accel_sf [ppm], gyro_ma /
+    accel_ma [deg] (a scalar for every off-diagonal, or 3x3 with a zero diagonal) (missing -> zero; stored as
+    'b_std', 'sf', 'ma' in SI units)."""
 
     def __init__(self, accuracy='low-accuracy', axis=6, gps=True, gps_opt=None,
                  odo=False, odo_opt=None):
@@ -132,6 +169,8 @@ class IMU(object):
                 'vrw': as_arr(accuracy['accel_vrw']) / 60.0}
             self.gyro_err.update(_terms(accuracy, 'gyro'))
             self.accel_err.update(_terms(accuracy, 'accel'))
+            self.gyro_err.update(_run_errs(accuracy, 'gyro'))
+            self.accel_err.update(_run_errs(accuracy, 'accel'))
             self.mag_err = mag_profile('low-accuracy')
             if self.magnetometer:
                 if 'mag_std' not in accuracy:
@@ -175,20 +214,22 @@ class IMU(object):
             return profiles(value)
         if isinstance(value, dict):
             for k in value:
-                if k not in current and k not in _TERM_KEYS:
+                if k not in current and k not in _TERM_KEYS and k not in _RUN_ERR_KEYS:
                     raise ValueError('unsupported key: %s in %s' % (k, what))
-                current[k] = value[k]
+                current[k] = _run_err_value(k, k, value[k]) if k in _RUN_ERR_KEYS else value[k]
             return current
         raise TypeError('%s is not valid.' % what)
 
     def set_gyro_error(self, gyro_error='low-accuracy'):
         """imu_model.py:207-236: grade string, or dict of {'b','arw','b_drift','b_corr'}
         IN THE STORED (SI) UNITS, exactly as the reference assigns them, and of 'q', 'rrw', 'rr'
-        (Allan(fit=True)'s Q, K and R of a gyro axis: columns 0, 3 and 4 of noise_gyro)."""
+        (Allan(fit=True)'s Q, K and R of a gyro axis: columns 0, 3 and 4 of noise_gyro), and of the run-to-run
+        errors 'b_std' [rad/s], 'sf' [-], 'ma' [rad] (checked as IMU(accuracy=dict) checks them)."""
         self.gyro_err = self._set(self.gyro_err, gyro_error, gyro_profile, 'gyro_error')
 
     def set_accel_error(self, accel_error='low-accuracy'):
-        """imu_model.py:238-267; also 'q', 'rrw', 'rr' as for set_gyro_error (noise_accel's columns)."""
+        """imu_model.py:238-267; also 'q', 'rrw', 'rr' as for set_gyro_error (noise_accel's columns), and
+        'b_std' [m/s^2], 'sf', 'ma'."""
         self.accel_err = self._set(self.accel_err, accel_error, accel_profile, 'accel_error')
 
     def set_mag_error(self, mag_error='low-accuracy'):

@@ -482,7 +482,8 @@ class Sim(object):
         for a in self.algo or []:       # refused before anything of the Sim is reset
             if terms and isinstance(a, (InsLoose, FreeIntegrationOdo)):
                 raise ValueError('%s generates its IMU inside its kernel, which makes no quantisation, rate '
-                                 'random walk or rate ramp: the IMU sets %s' % (type(a).__name__, terms))
+                                 'random walk, rate ramp or run-to-run bias, scale-factor or misalignment error: '
+                                 'the IMU sets %s' % (type(a).__name__, terms))
         self._blocks = {}        # (block, name) -> [runs of the block, ...] host histories (_history)
         self._proc = {}          # (algo index, start [s], position frame) -> [R, 3, 9] process statistics
         self._sens = {}          # (source, first row) -> sensor error statistics (_sensor_launch)
@@ -727,9 +728,22 @@ class Sim(object):
         return any(v is not None and v['type'] == 'psd' for v in (self._vib_acc, self._vib_gyro))
 
     def _imu_terms(self):
-        """The IEEE Std 952 terms the IMU sets (non-zero 'q', 'rrw', 'rr'), e.g. ['gyro rrw']; [] for none."""
+        """The IEEE Std 952 terms and run-to-run errors the IMU sets (non-zero 'q', 'rrw', 'rr', 'b_std', 'sf',
+        'ma'), e.g. ['gyro rrw', 'gyro sf']; [] for none.  Only K1 and K9 make them."""
         return ['%s %s' % (s, k) for s, err in (('gyro', self.imu.gyro_err), ('accel', self.imu.accel_err))
-                for k in _lib.set_terms(err)]
+                for k in _lib.set_terms(err) + _lib.set_run_errors(err)]
+
+    def imu_run_errors(self):
+        """The run-to-run errors every run of the experiment draws: {'accel': [R, 3, 4], 'gyro': [R, 3, 4]} (numpy;
+        R = the runs of the last run(), all ranks' runs), row i = (S[i][0], S[i][1], S[i][2], b_run[i]): the run's
+        measurement is the truth plus b_run + S truth plus everything else the IMU model makes.  Computed on the
+        device from the global run ids (run_base + r) and the seed, so every rank gets the same table.  All zero for
+        an IMU without 'b_std', 'sf' or 'ma'."""
+        if self.imu is None:
+            raise ValueError('imu_run_errors needs an IMU model')
+        t = engine.imu_run_errors(self.sim_count, self.imu.gyro_err, self.imu.accel_err, self.seed,
+                                  run_offset=self.run_base).cpu().numpy()
+        return {'accel': t[:, 0], 'gyro': t[:, 1]}
 
     def _fed(self, ai):
         """True if free-integration plugin ai runs as K1 then K2 on the materialised series (the IMU has terms

@@ -75,6 +75,22 @@ typedef struct b2ins_noise_terms {
   double r[3];
 } b2ins_noise_terms;
 
+/* The run-to-run errors of one triad (DESIGN.md section 4): 1-sigma values in SI units, each drawn once per run
+ * from the run's global id and constant over the run.  Per axis c of run r:
+ *   b:  turn-on bias [rad/s; accel m/s^2]: b_run[c] = b[c] z, added to b2ins_sensor_err.b;
+ *   sf: scale factor [-]: S[c][c] = sf[c] z;
+ *   ma: misalignment [rad]: S[i][j] = ma[i][j] z (i != j), the sensitivity of sensor axis i to true axis j;
+ *       the diagonal must be 0.
+ * The measurement gains delta[c] = b_run[c] + sum_j S[c][j] ref[j]: M = I + S scales the true rate or specific
+ * force, not the vibration.  Draws: counter t = 0xFFFFFFFD, id 44 + 6 sensor + j (sensor 0 accel, 1 gyro);
+ * j = 0..2: (z0, z1) = (b_run[j], sf[j]); j = 3..5: the off-diagonals of row j - 3 in column order.
+ * Every value must be finite and >= 0. */
+typedef struct b2ins_run_err {
+  double b[3];
+  double sf[3];
+  double ma[3][3];
+} b2ins_run_err;
+
 /* Vibration model of one triad: Sim.__parse_env output (ins_sim.py:642-701). */
 typedef struct b2ins_vib {
   int32_t type; /* B2INS_VIB_* */
@@ -351,6 +367,30 @@ int b2ins_imu_noise_ex_f64_host(double fs, int64_t runs, int64_t n,
                                 uint64_t seed, int64_t run_offset, int layout,
                                 double* gyro, double* accel, double* z_dump);
 
+/* K1 with the IEEE Std 952 terms and the run-to-run errors of b2ins_run_err (gyro_run / accel_run nullable:
+ * none).  With every run error zero these are b2ins_imu_noise_ex_f64[_host], which are this entry point with
+ * null run errors. */
+int b2ins_imu_noise_rx_f64(double fs, int64_t runs, int64_t n,
+                           const double* ref_gyro, const double* ref_accel,
+                           const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                           const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                           const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                           uint64_t seed, int64_t run_offset, int layout,
+                           double* gyro, double* accel, double* z_dump,
+                           const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, void* stream);
+int b2ins_imu_noise_rx_f64_host(double fs, int64_t runs, int64_t n,
+                                const double* ref_gyro, const double* ref_accel,
+                                const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                                const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                                const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                                uint64_t seed, int64_t run_offset, int layout,
+                                double* gyro, double* accel, double* z_dump,
+                                const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run);
+/* The run errors K1-rx and K9-rx draw for runs run_offset .. run_offset + runs - 1:
+ * out [runs][2][12] (device; sensor 0 accel, 1 gyro): S row-major [9], then b_run [3].  Asynchronous. */
+int b2ins_imu_run_err_f64(uint64_t seed, int64_t runs, int64_t run_offset, const b2ins_run_err* gyro_run,
+                          const b2ins_run_err* accel_run, double* out, void* stream);
+
 /* ---- K12: fused Monte-Carlo run (noise -> integration -> per-run errors) --
  * Replaces loop A (ins_sim.py:490-496) + loop B (ins_algo_manager.py:73-95) + the per-run
  * part of InsDataMgr.calc_data_err / array_error (ins_data_manager.py:454-541).
@@ -625,6 +665,16 @@ int b2ins_imu_err_stats_ex_f64(double fs, int64_t runs, int64_t n,
                                const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
                                uint64_t seed, int64_t run_offset, int64_t stats_start,
                                double* end_err, double* proc_stats, void* stream);
+/* K9 of the measurements b2ins_imu_noise_rx_f64 makes (the _ex arguments plus the nullable run errors); with
+ * null or all-zero run errors, b2ins_imu_err_stats_ex_f64. */
+int b2ins_imu_err_stats_rx_f64(double fs, int64_t runs, int64_t n,
+                               const double* ref_gyro, const double* ref_accel,
+                               const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err,
+                               const b2ins_noise_terms* gyro_terms, const b2ins_noise_terms* accel_terms,
+                               const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                               uint64_t seed, int64_t run_offset, int64_t stats_start,
+                               double* end_err, double* proc_stats,
+                               const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, void* stream);
 
 /* ---- K3p: per-run error statistics of a device array ----------------------------------
  * x [runs][m][ncomp] against the shared ref [m][ncomp] (device), e = x - ref:

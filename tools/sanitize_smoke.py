@@ -123,6 +123,13 @@ def main():
     long_r = engine.to_device(np.zeros((300001, 3)))
     engine.imu_noise(100.0, 1, long_r, long_r, tg, ta, 1)
     engine.imu_err_stats(100.0, 1, long_r, long_r, tg, ta, 1, stats_start=1000)
+    # K1-rx and K9-rx with the run-to-run errors (alone, and with the terms on the segmented plan) and their table
+    xg, xa = dict(MID_G, b_std=np.full(3, 1e-5), sf=np.full(3, 1e-3), ma=1e-3), dict(MID_A, sf=np.full(3, 1e-4))
+    engine.imu_noise(100.0, 5, rg, ra, xg, xa, 1)
+    engine.imu_err_stats(100.0, 5, rg, ra, xg, xa, 1, stats_start=250)
+    engine.imu_noise(100.0, 1, long_r, long_r, dict(tg, **xg), xa, 1)
+    engine.imu_err_stats(100.0, 1, long_r, long_r, dict(tg, **xg), xa, 1, stats_start=1000)
+    engine.imu_run_errors(300, xg, xa, 1, run_offset=2 ** 32 - 5)
     engine.proc_stats(mag, ref_mag, 7)
     torch.cuda.synchronize()
     print('sanitize smoke ok')
