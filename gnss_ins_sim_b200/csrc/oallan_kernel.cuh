@@ -8,7 +8,9 @@
 //
 // Precision.  C grows with the series (accelerometer z at 14.4 M samples: ~1.4e8, one ulp 3e-8,
 // against m = 1 differences of 1e-2; a ramp grows it quadratically, and the shift by x_0 does not
-// remove a ramp), so C is kept as a double-double (hi, lo): an error-free TwoSum per sample.  A term
+// remove a ramp), so C is kept as a double-double (hi, lo) accumulated by TwoSum.  The shift v - x_0 itself
+// rounds where the result needs more than 53 bits (an outlier x_0, a wide drift); a double-double add then
+// errs by O(u^2) of its operands, not zero.  A term
 // is formed from D_L = C[k+L] - C[k] (TwoDiff of the hi parts, exact, plus the lo difference), then
 // d = (D_2m.hi - 2 D_m.hi) + (D_2m.lo - 2 D_m.lo): both hi terms are ~2 S and the subtraction is
 // exact whenever they are within a factor of two.
@@ -51,7 +53,9 @@
 // the same lags, and pass 5 gives NaN if there is one, else +inf.  A Hadamard term is NaN exactly when
 // its signed contributions +S2, -2 S1, +S0 hold both infinities: a window holds both signs, or S2 and
 // S0 are infinite with opposite signs, or S1 is infinite with the sign of S2 or of S0.  That is what
-// the definitional sum gives in IEEE arithmetic, whatever the order of its additions.
+// the definitional sum gives in IEEE arithmetic, whatever the order of its additions.  A series of finite
+// samples never gives NaN: if its shifted prefix overflows (x_0 = -1e305, the rest +1e305), TwoSum of the
+// infinite sum is NaN, and pass 5 reports that series' taus as +inf, which its terms' squares are.
 #pragma once
 #include <cmath>
 #include <cstring>
@@ -396,6 +400,8 @@ __global__ void __launch_bounds__(128) oallan_final_kernel(const __grid_constant
       a = NAN;
     else if (mode == kOallanInf)
       a = v > 0.0 ? NAN : INFINITY;
+    else if (isnan(v))   // finite samples: only an overflowing prefix (inf - inf in its TwoSum) gives NaN
+      a = INFINITY;
     else if (HAD)
       a = v / (6.0 * m * m * static_cast<double>(p.n - 3 * p.m[i] + 1));
     else
