@@ -262,8 +262,8 @@ def set_terms(err):
 
 
 def noise_terms(err):
-    """imu_model dict -> NoiseTerms (absent keys: zero), or None when it has no non-zero term: the _ex entry
-    points then run the kernels without terms."""
+    """imu_model dict -> NoiseTerms (absent keys: zero), or None when it has no non-zero term: the K1 and K9
+    entry points then launch their forms without terms."""
     if not set_terms(err):
         return None
     t = NoiseTerms()
@@ -284,7 +284,7 @@ def set_run_errors(err):
 
 def run_err(err):
     """imu_model dict -> RunErr (absent keys: zero; 'ma' a scalar for every off-diagonal or 3x3), or None when it
-    has no non-zero run error: the _rx entry points then launch what the _ex ones do."""
+    has no non-zero run error: the K1 and K9 entry points then launch their forms without run errors."""
     if not set_run_errors(err):
         return None
     e = RunErr()
@@ -301,7 +301,9 @@ def run_err(err):
 
 
 def vib(vib_def, series_ptr=None, series_len=0):
-    """Sim.__parse_env-style dict (or None) -> Vib."""
+    """Sim.__parse_env-style dict (or None) -> Vib; a Vib is returned as it is."""
+    if isinstance(vib_def, Vib):
+        return vib_def
     v = Vib()
     v.type = VIB_NONE
     if vib_def is None:

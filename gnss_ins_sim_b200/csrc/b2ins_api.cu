@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/b2ins.h"
@@ -421,48 +422,92 @@ int digest_run_err(const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run
   return B2INS_OK;
 }
 
-// K1's parameters and time segmentation, shared by K1 and K9; with segments, pass 1 and the carry chain are
-// launched here and *scratch holds their buffers until the caller has queued pass 0 on s.  x (nullable): the
-// IEEE Std 952 terms, whose rate random walk is carried across the segments like the drift, with a = 1.
-int noise_prepare(double fs, int64_t runs, int64_t n, const double* ref_gyro, const double* ref_accel,
-                  const b2ins_sensor_err* gyro_err, const b2ins_sensor_err* accel_err, const b2ins_vib* vib_gyro,
-                  const b2ins_vib* vib_accel, uint64_t seed, int64_t run_offset, cudaStream_t s, NoiseParams* out,
-                  AsyncBuf* scratch, NoiseTerms* x = nullptr, bool walk = false) {
-  NoiseParams& p = *out;
+// The error model of a K1 or K9 call, digested for the device and checked
+struct NoiseModel {
+  NoiseParams p;        // n, runs, dt and the two triads; noise_plan and the entry point fill in the rest
+  NoiseTerms x;
+  RunErrs re;
+  bool terms, walk;     // a term is non-zero; a rate random walk is (digest_terms)
+  bool runerr;          // a run error is non-zero (digest_run_err)
+};
+
+// The terms and the run errors are checked whatever the size; a call with no runs or no samples returns after
+// them (the caller then returns B2INS_OK) and digests no triad.
+int digest_noise(double fs, int64_t runs, int64_t n, const b2ins_sensor_err* gyro_err,
+                 const b2ins_sensor_err* accel_err, const b2ins_noise_terms* gyro_terms,
+                 const b2ins_noise_terms* accel_terms, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
+                 const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, NoiseModel* m) {
+  int rc = digest_terms(gyro_terms, accel_terms, fs, &m->x, &m->terms, &m->walk);
+  if (rc != B2INS_OK) return rc;
+  rc = digest_run_err(gyro_run, accel_run, &m->re, &m->runerr);
+  if (rc != B2INS_OK || runs == 0 || n == 0) return rc;
+  ARG_CHECK(gyro_err && accel_err, "null buffer");
+  NoiseParams& p = m->p;
   std::memset(&p, 0, sizeof(p));
   p.n = n;
   p.runs = runs;
-  p.run_offset = run_offset;
   p.dt = 1.0 / fs;
+  rc = digest_triad(gyro_err, vib_gyro, fs, &p.gyro);
+  if (rc != B2INS_OK) return rc;
+  return digest_triad(accel_err, vib_accel, fs, &p.accel);
+}
+
+// The one launch site of K1 (Params = NoiseParams, pass 0 or 1) and K9 (ErrStatsParams): the form with the
+// model's terms when it has any, and with its run errors when runerr
+template <class Params>
+void launch_noise(const Params& P, const NoiseModel& m, bool runerr, unsigned ctas, cudaStream_t s) {
+  if constexpr (std::is_same_v<Params, NoiseParams>) {
+    if (m.terms && runerr)
+      imu_noise_ex_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, m.x, m.re);
+    else if (m.terms)
+      imu_noise_ex_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, m.x);
+    else if (runerr)
+      imu_noise_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, m.re);
+    else
+      imu_noise_kernel<<<ctas, kNoiseThreads, 0, s>>>(P);
+  } else {
+    if (m.terms && runerr)
+      imu_err_stats_ex_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, m.x, m.re);
+    else if (m.terms)
+      imu_err_stats_ex_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, m.x);
+    else if (runerr)
+      imu_err_stats_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, m.re);
+    else
+      imu_err_stats_kernel<<<ctas, kNoiseThreads, 0, s>>>(P);
+  }
+}
+
+// The rest of K1's parameters and its time segmentation on this device, shared by K1 and K9, after every argument
+// is checked; with segments, pass 1 and the carry chain are launched here and *scratch holds their buffers until
+// the caller has queued pass 0 on s.  The terms' rate random walk is carried across the segments like the drift,
+// with a = 1; the run errors have no state in time, so pass 1 runs without them.
+int noise_prepare(NoiseModel* m, const double* ref_gyro, const double* ref_accel, uint64_t seed, int64_t run_offset,
+                  cudaStream_t s, AsyncBuf* scratch) {
+  NoiseParams& p = m->p;
+  const int64_t runs = p.runs;
+  p.run_offset = run_offset;
   p.k0 = static_cast<uint32_t>(seed);
   p.k1 = static_cast<uint32_t>(seed >> 32);
-  int rc = digest_triad(gyro_err, vib_gyro, fs, &p.gyro);
-  if (rc != B2INS_OK) return rc;
-  rc = digest_triad(accel_err, vib_accel, fs, &p.accel);
-  if (rc != B2INS_OK) return rc;
   p.ref_gyro = ref_gyro;
   p.ref_accel = ref_accel;
-  noise_plan(&p, sm_count(), walk);
-  p.pass = 0;
-  p.seg_carry = nullptr;
-  p.seg_end = nullptr;
+  noise_plan(&p, sm_count(), m->walk);
   if (p.nseg > 1) {
-    CU_CHECK(scratch->alloc(sizeof(double) * runs * p.nseg * (x ? 24 : 12)));
+    CU_CHECK(scratch->alloc(sizeof(double) * runs * p.nseg * (m->terms ? 24 : 12)));
     p.seg_end = scratch->p;
     p.seg_carry = scratch->p + runs * p.nseg * 6;
+    if (m->terms) {
+      m->x.seg_end = scratch->p + runs * p.nseg * 12;
+      m->x.seg_carry = scratch->p + runs * p.nseg * 18;
+    }
     p.pass = 1;
+    launch_noise(p, *m, false, static_cast<unsigned>(runs * (p.nseg - 1)), s);
     const unsigned ctas = static_cast<unsigned>((runs * 6 + 127) / 128);
-    if (x) {
-      x->seg_end = scratch->p + runs * p.nseg * 12;
-      x->seg_carry = scratch->p + runs * p.nseg * 18;
-      imu_noise_ex_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p, *x);
+    if (m->terms) {
       NoiseParams pw = p;      // the walk's carry chain: noise_carry_kernel with a = 1
       for (int c = 0; c < 3; ++c) pw.accel.gm_a[c] = pw.gyro.gm_a[c] = 1.0;
-      pw.seg_end = x->seg_end;
-      pw.seg_carry = x->seg_carry;
+      pw.seg_end = m->x.seg_end;
+      pw.seg_carry = m->x.seg_carry;
       noise_carry_kernel<<<ctas, 128, 0, s>>>(pw);
-    } else {
-      imu_noise_kernel<<<static_cast<unsigned>(runs * (p.nseg - 1)), kNoiseThreads, 0, s>>>(p);
     }
     noise_carry_kernel<<<ctas, 128, 0, s>>>(p);
     p.pass = 0;
@@ -618,36 +663,22 @@ int b2ins_imu_noise_rx_f64(double fs, int64_t runs, int64_t n, const double* ref
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   ARG_CHECK(layout >= 0 && layout <= 2, "layout must be B2INS_LAYOUT_*");
-  NoiseTerms x;
-  bool terms = false, walk = false;
-  int rc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
-  if (rc != B2INS_OK) return rc;
-  RunErrs re;
-  bool runerr = false;
-  rc = digest_run_err(gyro_run, accel_run, &re, &runerr);
-  if (rc != B2INS_OK) return rc;
-  if (runs == 0 || n == 0) return B2INS_OK;
-  ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && gyro && accel, "null buffer");
+  NoiseModel m;
+  int rc = digest_noise(fs, runs, n, gyro_err, accel_err, gyro_terms, accel_terms, vib_gyro, vib_accel, gyro_run,
+                        accel_run, &m);
+  if (rc != B2INS_OK || runs == 0 || n == 0) return rc;
+  ARG_CHECK(ref_gyro && ref_accel && gyro && accel, "null buffer");
   ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
-  NoiseParams p;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AsyncBuf scratch(s);
-  rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed, run_offset, s,
-                     &p, &scratch, terms ? &x : nullptr, walk);
+  rc = noise_prepare(&m, ref_gyro, ref_accel, seed, run_offset, s, &scratch);
   if (rc != B2INS_OK) return rc;
+  NoiseParams& p = m.p;
   p.out_gyro = gyro;
   p.out_accel = accel;
   layout_strides(layout, runs, n, &p.osr, &p.ost, &p.osc);
   p.z_dump = z_dump;
-  const unsigned ctas = static_cast<unsigned>(runs * p.nseg);
-  if (terms && runerr)
-    imu_noise_ex_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(p, x, re);
-  else if (terms)
-    imu_noise_ex_kernel<<<ctas, kNoiseThreads, 0, s>>>(p, x);
-  else if (runerr)
-    imu_noise_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(p, re);
-  else
-    imu_noise_kernel<<<ctas, kNoiseThreads, 0, s>>>(p);
+  launch_noise(p, m, m.runerr, static_cast<unsigned>(runs * p.nseg), s);
   CU_CHECK(scratch.free());
   CU_CHECK(cudaGetLastError());
   return B2INS_OK;
@@ -698,25 +729,20 @@ int b2ins_imu_err_stats_rx_f64(double fs, int64_t runs, int64_t n, const double*
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs >= 0 && n >= 0, "runs and n must be non-negative");
   ARG_CHECK(stats_start < n || n == 0, "stats_start must be < n");
-  NoiseTerms x;
-  bool terms = false, walk = false;
-  const int trc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
-  if (trc != B2INS_OK) return trc;
-  RunErrs re;
-  bool runerr = false;
-  const int xrc = digest_run_err(gyro_run, accel_run, &re, &runerr);
-  if (xrc != B2INS_OK) return xrc;
-  if (runs == 0 || n == 0) return B2INS_OK;
-  ARG_CHECK(ref_gyro && ref_accel && gyro_err && accel_err && end_err, "null buffer");
+  NoiseModel m;
+  int rc = digest_noise(fs, runs, n, gyro_err, accel_err, gyro_terms, accel_terms, vib_gyro, vib_accel, gyro_run,
+                        accel_run, &m);
+  if (rc != B2INS_OK || runs == 0 || n == 0) return rc;
+  ARG_CHECK(ref_gyro && ref_accel && end_err, "null buffer");
   ARG_CHECK(stats_start < 0 || proc_stats, "stats_start >= 0 needs proc_stats");
   ARG_CHECK(n < (int64_t(1) << 32), "n must be < 2^32");
-  ErrStatsParams P;
-  std::memset(&P, 0, sizeof(P));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AsyncBuf scratch(s), partial(s);
-  const int rc = noise_prepare(fs, runs, n, ref_gyro, ref_accel, gyro_err, accel_err, vib_gyro, vib_accel, seed,
-                               run_offset, s, &P.np, &scratch, terms ? &x : nullptr, walk);
+  rc = noise_prepare(&m, ref_gyro, ref_accel, seed, run_offset, s, &scratch);
   if (rc != B2INS_OK) return rc;
+  ErrStatsParams P;
+  std::memset(&P, 0, sizeof(P));
+  P.np = m.p;
   P.stats_start = stats_start;
   P.end_err = end_err;
   P.proc_stats = proc_stats;
@@ -726,15 +752,7 @@ int b2ins_imu_err_stats_rx_f64(double fs, int64_t runs, int64_t n, const double*
       return fail(B2INS_ERR_CUDA, "cudaMallocAsync of the segment partials: %s", cudaGetErrorString(e));
     P.partial = partial.p;
   }
-  const unsigned ctas = static_cast<unsigned>(runs * P.np.nseg);
-  if (terms && runerr)
-    imu_err_stats_ex_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, x, re);
-  else if (terms)
-    imu_err_stats_ex_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, x);
-  else if (runerr)
-    imu_err_stats_rx_kernel<<<ctas, kNoiseThreads, 0, s>>>(P, re);
-  else
-    imu_err_stats_kernel<<<ctas, kNoiseThreads, 0, s>>>(P);
+  launch_noise(P, m, m.runerr, static_cast<unsigned>(runs * P.np.nseg), s);
   if (partial.p) {
     err_stats_fold_kernel<<<static_cast<unsigned>((runs * kErrCh + 127) / 128), 128, 0, s>>>(P);
     CU_CHECK(partial.free());
@@ -1901,19 +1919,12 @@ int b2ins_diag_noise_plan_ex(double fs, int64_t runs, int64_t n, const b2ins_sen
   ARG_CHECK(fs > 0.0, "fs must be positive");
   ARG_CHECK(runs > 0 && n > 0, "runs and n must be positive");
   ARG_CHECK(gyro_err && accel_err && coef && plan, "null buffer");
-  NoiseTerms x;
-  bool terms = false, walk = false;
-  const int trc = digest_terms(gyro_terms, accel_terms, fs, &x, &terms, &walk);
-  if (trc != B2INS_OK) return trc;
-  NoiseParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.n = n;
-  p.runs = runs;
-  int rc = digest_triad(gyro_err, nullptr, fs, &p.gyro);
+  NoiseModel m;
+  const int rc = digest_noise(fs, runs, n, gyro_err, accel_err, gyro_terms, accel_terms, nullptr, nullptr, nullptr,
+                              nullptr, &m);
   if (rc != B2INS_OK) return rc;
-  rc = digest_triad(accel_err, nullptr, fs, &p.accel);
-  if (rc != B2INS_OK) return rc;
-  noise_plan(&p, sm_count_arg > 0 ? sm_count_arg : sm_count(), walk);
+  NoiseParams& p = m.p;
+  noise_plan(&p, sm_count_arg > 0 ? sm_count_arg : sm_count(), m.walk);
   for (int c = 0; c < 6; ++c) {
     const TriadNoise& e = (c < 3) ? p.accel : p.gyro;
     coef[c] = e.gm_a[c % 3];

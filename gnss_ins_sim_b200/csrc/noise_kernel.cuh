@@ -8,9 +8,8 @@
 // shared memory: ONE exchange per kNoisePer samples instead of one per sample -- after which every
 // thread adds a^q S to its samples and the tile leaves shared memory in the caller's layout with
 // coalesced stores.  imu_err_stats_kernel (K9, sensor_stats_kernel.cuh) reduces the tile instead of
-// storing it; it calls noise_prologue and the scan of common.cuh, and repeats only the stretch loop
-// (triad_sample into the stage): with that loop in a shared function the compiler allocates K9's
-// registers differently, so a change to the loop here goes there too.
+// storing it: both bodies make their CTA's prologue with noise_prologue and every tile up to the end of
+// the scan with noise_tile, and differ only in what they do with the finished tile.
 #pragma once
 #include "mc_kernel.cuh"
 
@@ -139,12 +138,32 @@ __device__ __forceinline__ void run_err_add(const double* e12, const double* ref
   }
 }
 
-// the prologue of a K1 or K9 CTA, before its first __syncthreads: a^q per channel into apow[kNoisePer + 1][6],
-// the run's sinusoidal gyro-vibration phase and, with carry_in, the Gauss-Markov state at the segment start
-// (zero without)
-__device__ __forceinline__ void noise_prologue(const NoiseParams& p, double (*apow)[6], int64_t run, int seg,
-                                               uint32_t run_lo, uint32_t run_hi, bool carry_in, double (&phase)[3],
-                                               double (&carry)[6]) {
+// what a K1 or K9 CTA works on: its run, its time segment and that segment's samples [seg_lo, seg_hi), and the
+// halves of the global run id that key its draws
+struct NoiseCta {
+  int64_t run, seg_lo, seg_hi;
+  int seg;
+  uint32_t run_lo, run_hi;
+};
+
+// The prologue of a K1 or K9 CTA, up to and including its first __syncthreads.  blockIdx.x = run * segs + seg:
+// segs = nseg, or nseg - 1 in K1's pass 1, which covers only the last pass1_len samples of a segment (K9 runs
+// pass 0 only).  It writes a^q per channel into apow[kNoisePer + 1][6], the run's sinusoidal gyro-vibration
+// phase, and carry: the Gauss-Markov state (and under TERMS the walk) at the segment start, zero in pass 1 and
+// for seg 0.  Under RUNERR, 12 threads draw the run's (S, b_run) of both sensors into rerr, one pair each.
+template <bool TERMS, bool RUNERR, int C>
+__device__ __forceinline__ NoiseCta noise_prologue(const NoiseParams& p, const NoiseTerms* x, const RunErrs* re,
+                                                   int pass, double (*apow)[6], double (*rerr)[12],
+                                                   double (&phase)[3], double (&carry)[C]) {
+  NoiseCta cta;
+  const int segs = (pass == 1) ? p.nseg - 1 : p.nseg;
+  cta.run = blockIdx.x / segs;
+  cta.seg = static_cast<int>(blockIdx.x % segs);
+  cta.seg_hi = min64(p.n, (cta.seg + 1) * p.seg_len);
+  cta.seg_lo = (pass == 1) ? cta.seg_hi - p.pass1_len : cta.seg * p.seg_len;
+  const int64_t grun = p.run_offset + cta.run;
+  cta.run_lo = static_cast<uint32_t>(grun);
+  cta.run_hi = static_cast<uint32_t>(grun >> 32);
   const int tid = threadIdx.x;
   if (tid < 6) {
     const double a = (tid < 3) ? p.accel.gm_a[tid] : p.gyro.gm_a[tid - 3];
@@ -159,14 +178,87 @@ __device__ __forceinline__ void noise_prologue(const NoiseParams& p, double (*ap
   if (p.gyro.vib_type == 2) {
 #pragma unroll
     for (int c = 0; c < 3; ++c)
-      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, run_lo, run_hi, p.k0, p.k1) * 2.0) * kPi;
+      phase[c] = (uniform01(0xFFFFFFFFu, kDrawPhase + c, cta.run_lo, cta.run_hi, p.k0, p.k1) * 2.0) * kPi;
   }
+  const int64_t at = (cta.run * p.nseg + cta.seg) * 6;
 #pragma unroll
   for (int c = 0; c < 6; ++c) carry[c] = 0.0;
-  if (carry_in && p.seg_carry) {
+  if (pass == 0 && p.seg_carry) {
 #pragma unroll
-    for (int c = 0; c < 6; ++c) carry[c] = p.seg_carry[(run * p.nseg + seg) * 6 + c];
+    for (int c = 0; c < 6; ++c) carry[c] = p.seg_carry[at + c];
   }
+  if constexpr (TERMS) {
+#pragma unroll
+    for (int c = 0; c < 6; ++c) carry[6 + c] = (pass == 0 && x->seg_carry) ? x->seg_carry[at + c] : 0.0;
+  }
+  if constexpr (RUNERR) {
+    if (tid < 12) run_err_pair(re->s[tid / 6], tid / 6, tid % 6, cta.run_lo, cta.run_hi, p.k0, p.k1, rerr[tid / 6]);
+  }
+  __syncthreads();
+  return cta;
+}
+
+// One tile of a K1 or K9 CTA, its samples tile0 .. tile0 + cnt - 1, up to the end of the scan.  The thread makes
+// its stretch (the kNoisePer consecutive samples tid kNoisePer ..) one sensor triad at a time (three Box-Muller
+// chains in flight) into stage[sensor][sample * 3 + axis]: each measurement without the drift (and walk) at the
+// stretch start.  Then the affine scan over the threads, (A, E) o (A', E') = (A A', A' E + E'), leaves in S the
+// drift (and under TERMS the walk) at the stretch start, and advances carry to the next tile.  Returns the
+// stretch's live samples.  In K1's pass 1 only the drift and the walk advance.
+template <bool TERMS, bool RUNERR, int C>
+__device__ __forceinline__ int noise_tile(const NoiseParams& p, const NoiseTerms* x, const NoiseCta& cta,
+                                          const double (&phase)[3], const double (*apow)[6],
+                                          const double (*rerr)[12], double (*stage)[kNoiseTile * 3],
+                                          double (*wtot)[kNoiseWarps][2], int64_t tile0, int cnt, int pass,
+                                          double (&carry)[C], double (&S)[C]) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  double r[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) r[c] = 0.0;
+  int mine = cnt - tid * kNoisePer;                 // live samples of this thread's stretch
+  mine = mine < 0 ? 0 : (mine > kNoisePer ? kNoisePer : mine);
+  double qe[TERMS ? 6 : 1];                         // TERMS: the quantisation error e[t] of each channel
+  if constexpr (TERMS) {
+    if (mine > 0 && pass == 0) {
+      const uint32_t t0 = static_cast<uint32_t>(tile0 + tid * kNoisePer);
+#pragma unroll
+      for (int c = 0; c < 6; ++c)
+        qe[c] = x->q[c] != 0.0
+                    ? x->q[c] * (uniform01(t0, kDrawQuant + c, cta.run_lo, cta.run_hi, p.k0, p.k1) - 0.5)
+                    : 0.0;
+    }
+  }
+#pragma unroll 1
+  for (int q = 0; q < mine; ++q) {
+    const int el = tid * kNoisePer + q;
+    const int64_t t = tile0 + el;
+    double m3[3];
+    triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), cta.run_lo, cta.run_hi, cta.run,
+                    phase, pass == 1, r, m3);
+    if constexpr (TERMS) terms_sample<0>(p, *x, t, cta.run_lo, cta.run_hi, pass == 1, r + 6, qe, m3);
+    if constexpr (RUNERR) {
+      if (pass == 0) run_err_add(rerr[0], p.ref_accel + t * 3, m3);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
+    triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), cta.run_lo, cta.run_hi, cta.run,
+                    phase, pass == 1, r + 3, m3);
+    if constexpr (TERMS) terms_sample<1>(p, *x, t, cta.run_lo, cta.run_hi, pass == 1, r + 9, qe + 3, m3);
+    if constexpr (RUNERR) {
+      if (pass == 0) run_err_add(rerr[1], p.ref_gyro + t * 3, m3);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
+  }
+  double sA[C], sE[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    sA[c] = c < 6 ? apow[mine][c] : 1.0;
+    sE[c] = r[c];
+  }
+  affine_scan_warp<C, kNoiseWarps>(sA, sE, wtot, lane, warp);
+  __syncthreads();   // warp totals; the staged tile is complete
+  affine_scan_block<C, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
+  return mine;
 }
 
 // K1's body.  TERMS adds the IEEE Std 952 terms of x (DESIGN.md section 4): the rate random walk k runs as six
@@ -182,75 +274,15 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
   __shared__ double wtot[C][kNoiseWarps][2];      // (A, E) of every warp's stretch, per channel
   __shared__ double apow[kNoisePer + 1][6];       // a^q per channel
   __shared__ double rerr[RUNERR ? 2 : 1][12];     // RUNERR: (S row-major, b_run) of accel, gyro for this run
-  const int segs = (p.pass == 1) ? p.nseg - 1 : p.nseg;
-  const int64_t run = blockIdx.x / segs;
-  const int seg = static_cast<int>(blockIdx.x % segs);
-  const int64_t seg_hi = min64(p.n, (seg + 1) * p.seg_len);
-  const int64_t seg_lo = (p.pass == 1) ? seg_hi - p.pass1_len : seg * p.seg_len;
-  const int64_t grun = p.run_offset + run;
-  const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   double phase[3], carry[C];                      // carry: d (and k) at the first sample of the tile
-  noise_prologue(p, apow, run, seg, run_lo, run_hi, p.pass == 0, phase, *reinterpret_cast<double(*)[6]>(carry));
-  if constexpr (TERMS) {
-#pragma unroll
-    for (int c = 0; c < 6; ++c) carry[6 + c] = (p.pass == 0 && x->seg_carry) ? x->seg_carry[(run * p.nseg + seg) * 6 + c] : 0.0;
-  }
-  if constexpr (RUNERR) {
-    if (tid < 12) run_err_pair(re->s[tid / 6], tid / 6, tid % 6, run_lo, run_hi, p.k0, p.k1, rerr[tid / 6]);
-  }
-  __syncthreads();
+  const NoiseCta cta = noise_prologue<TERMS, RUNERR>(p, x, re, p.pass, apow, rerr, phase, carry);
 
-  for (int64_t tile0 = seg_lo; tile0 < seg_hi; tile0 += kNoiseTile) {
-    const int cnt = static_cast<int>(min64(kNoiseTile, seg_hi - tile0));
-    // ---- the thread's stretch: one sensor triad at a time (three Box-Muller chains in flight) -------
-    double r[C];
-#pragma unroll
-    for (int c = 0; c < C; ++c) r[c] = 0.0;
-    int mine = cnt - tid * kNoisePer;                 // live samples of this thread's stretch
-    mine = mine < 0 ? 0 : (mine > kNoisePer ? kNoisePer : mine);
-    double qe[TERMS ? 6 : 1];                         // TERMS: the quantisation error e[t] of each channel
-    if constexpr (TERMS) {
-      if (mine > 0 && p.pass == 0) {
-        const uint32_t t0 = static_cast<uint32_t>(tile0 + tid * kNoisePer);
-#pragma unroll
-        for (int c = 0; c < 6; ++c)
-          qe[c] = x->q[c] != 0.0 ? x->q[c] * (uniform01(t0, kDrawQuant + c, run_lo, run_hi, p.k0, p.k1) - 0.5) : 0.0;
-      }
-    }
-#pragma unroll 1
-    for (int q = 0; q < mine; ++q) {
-      const int el = tid * kNoisePer + q;
-      const int64_t t = tile0 + el;
-      double m3[3];
-      triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase,
-                      p.pass == 1, r, m3);
-      if constexpr (TERMS) terms_sample<0>(p, *x, t, run_lo, run_hi, p.pass == 1, r + 6, qe, m3);
-      if constexpr (RUNERR) {
-        if (p.pass == 0) run_err_add(rerr[0], p.ref_accel + t * 3, m3);
-      }
-#pragma unroll
-      for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
-      triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase,
-                      p.pass == 1, r + 3, m3);
-      if constexpr (TERMS) terms_sample<1>(p, *x, t, run_lo, run_hi, p.pass == 1, r + 9, qe + 3, m3);
-      if constexpr (RUNERR) {
-        if (p.pass == 0) run_err_add(rerr[1], p.ref_gyro + t * 3, m3);
-      }
-#pragma unroll
-      for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
-    }
-    // ---- affine scan over the threads, six channels: (A, E) o (A', E') = (A A', A' E + E') -------
-    double sA[C], sE[C];
-#pragma unroll
-    for (int c = 0; c < C; ++c) {
-      sA[c] = c < 6 ? apow[mine][c] : 1.0;
-      sE[c] = r[c];
-    }
-    affine_scan_warp<C, kNoiseWarps>(sA, sE, wtot, lane, warp);
-    __syncthreads();   // warp totals; the staged tile is complete
-    double S[C];       // drift at the first sample of this thread's stretch
-    affine_scan_block<C, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
+  for (int64_t tile0 = cta.seg_lo; tile0 < cta.seg_hi; tile0 += kNoiseTile) {
+    const int cnt = static_cast<int>(min64(kNoiseTile, cta.seg_hi - tile0));
+    double S[C];       // drift (and walk) at the first sample of this thread's stretch
+    const int mine =
+        noise_tile<TERMS, RUNERR>(p, x, cta, phase, apow, rerr, stage, wtot, tile0, cnt, p.pass, carry, S);
     if (p.pass == 0) {
       // ---- + a^q S on the thread's own samples, then the tile leaves in the caller's layout -------
 #pragma unroll 1
@@ -267,7 +299,7 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
         }
       }
       __syncthreads();
-      const int64_t base = run * p.osr + tile0 * p.ost;
+      const int64_t base = cta.run * p.osr + tile0 * p.ost;
       if (p.osc == 1 && p.ost == 3) {            // [R][n][3]: the staged tile is the output, verbatim
         for (int e = tid; e < cnt * 3; e += kNoiseThreads) {
           p.out_accel[base + e] = stage[0][e];
@@ -285,11 +317,12 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
         // (acc_gm[3], acc_w[3], gyr_gm[3], gyr_w[3]) of every sample, recovered from the same Philox draws
         for (int el = tid; el < cnt; el += kNoiseThreads) {
           const int64_t t = tile0 + el;
-          double* zd = p.z_dump + (run * p.n + t) * 12;
+          double* zd = p.z_dump + (cta.run * p.n + t) * 12;
 #pragma unroll
           for (int c = 0; c < 3; ++c) {
-            const Normal2 za = normal_pair(static_cast<uint32_t>(t), kDrawAccel + c, run_lo, run_hi, p.k0, p.k1);
-            const Normal2 zg = normal_pair(static_cast<uint32_t>(t), kDrawGyro + c, run_lo, run_hi, p.k0, p.k1);
+            const uint32_t t32 = static_cast<uint32_t>(t);
+            const Normal2 za = normal_pair(t32, kDrawAccel + c, cta.run_lo, cta.run_hi, p.k0, p.k1);
+            const Normal2 zg = normal_pair(t32, kDrawGyro + c, cta.run_lo, cta.run_hi, p.k0, p.k1);
             zd[c] = za.z0;
             zd[3 + c] = za.z1;
             zd[6 + c] = zg.z0;
@@ -304,10 +337,10 @@ __device__ __forceinline__ void imu_noise_body(const NoiseParams& p, const Noise
     // the tiles of a segment are whole (seg_len is a multiple of the tile) except in the last
     // segment, whose end value is never used
 #pragma unroll
-    for (int c = 0; c < 6; ++c) p.seg_end[(run * p.nseg + seg) * 6 + c] = carry[c];
+    for (int c = 0; c < 6; ++c) p.seg_end[(cta.run * p.nseg + cta.seg) * 6 + c] = carry[c];
     if constexpr (TERMS) {
 #pragma unroll
-      for (int c = 0; c < 6; ++c) x->seg_end[(run * p.nseg + seg) * 6 + c] = carry[6 + c];
+      for (int c = 0; c < 6; ++c) x->seg_end[(cta.run * p.nseg + cta.seg) * 6 + c] = carry[6 + c];
     }
   }
 }

@@ -5,10 +5,9 @@
 // and std (ddof 0).
 //
 // K9 has K1's launch shape (one CTA per (run, time segment), 896-sample tiles; the segmented form's pass 1
-// and noise_carry_kernel are K1's own) and calls K1's generator: noise_prologue, triad_sample and the
-// affine Gauss-Markov scan over the threads (common.cuh).  The stretch loop around triad_sample is K1's,
-// repeated (noise_kernel.cuh says why).  The finished tile is reduced instead of stored: nothing of the
-// series leaves the SM.
+// and noise_carry_kernel are K1's own) and runs K1's generator: noise_prologue, then for every tile
+// noise_tile (the stretch loop and the affine Gauss-Markov scan over the threads).  The finished tile is
+// reduced instead of stored: nothing of the series leaves the SM.
 //
 // Determinism: every reduction runs in a fixed order, with no floating-point atomics.  A thread reduces
 // its own stretch of a tile in two passes (sum and max, then the squared deviations from the stretch
@@ -70,73 +69,18 @@ __device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, cons
   __shared__ double wtot[C][kNoiseWarps][2];
   __shared__ double apow[kNoisePer + 1][6];
   __shared__ double rerr[RUNERR ? 2 : 1][12];     // RUNERR: (S row-major, b_run) of accel, gyro for this run
-  const int64_t run = blockIdx.x / p.nseg;
-  const int seg = static_cast<int>(blockIdx.x % p.nseg);
-  const int64_t seg_hi = min64(p.n, (seg + 1) * p.seg_len);
-  const int64_t seg_lo = seg * p.seg_len;
-  const int64_t grun = p.run_offset + run;
-  const uint32_t run_lo = static_cast<uint32_t>(grun), run_hi = static_cast<uint32_t>(grun >> 32);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool want_stats = P.stats_start >= 0;
-  double phase[3], carry[C];
-  noise_prologue(p, apow, run, seg, run_lo, run_hi, true, phase, *reinterpret_cast<double(*)[6]>(carry));
-  if constexpr (TERMS) {
-#pragma unroll
-    for (int c = 0; c < 6; ++c) carry[6 + c] = x->seg_carry ? x->seg_carry[(run * p.nseg + seg) * 6 + c] : 0.0;
-  }
-  if constexpr (RUNERR) {
-    if (tid < 12) run_err_pair(re->s[tid / 6], tid / 6, tid % 6, run_lo, run_hi, p.k0, p.k1, rerr[tid / 6]);
-  }
   double an = 0.0, am[6], a2[6], ax[6];           // the thread's running statistics
 #pragma unroll
   for (int c = 0; c < 6; ++c) am[c] = a2[c] = ax[c] = 0.0;
-  __syncthreads();
+  double phase[3], carry[C];
+  const NoiseCta cta = noise_prologue<TERMS, RUNERR>(p, x, re, 0, apow, rerr, phase, carry);
 
-  for (int64_t tile0 = seg_lo; tile0 < seg_hi; tile0 += kNoiseTile) {
-    const int cnt = static_cast<int>(min64(kNoiseTile, seg_hi - tile0));
-    double r[C];
-#pragma unroll
-    for (int c = 0; c < C; ++c) r[c] = 0.0;
-    int mine = cnt - tid * kNoisePer;
-    mine = mine < 0 ? 0 : (mine > kNoisePer ? kNoisePer : mine);
-    double qe[TERMS ? 6 : 1];
-    if constexpr (TERMS) {
-      if (mine > 0) {
-        const uint32_t t0 = static_cast<uint32_t>(tile0 + tid * kNoisePer);
-#pragma unroll
-        for (int c = 0; c < 6; ++c)
-          qe[c] = x->q[c] != 0.0 ? x->q[c] * (uniform01(t0, kDrawQuant + c, run_lo, run_hi, p.k0, p.k1) - 0.5) : 0.0;
-      }
-    }
-#pragma unroll 1
-    for (int q = 0; q < mine; ++q) {
-      const int el = tid * kNoisePer + q;
-      const int64_t t = tile0 + el;
-      double m3[3];
-      triad_sample<0>(p, p.accel, p.ref_accel + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase, false,
-                      r, m3);
-      if constexpr (TERMS) terms_sample<0>(p, *x, t, run_lo, run_hi, false, r + 6, qe, m3);
-      if constexpr (RUNERR) run_err_add(rerr[0], p.ref_accel + t * 3, m3);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) stage[0][el * 3 + c] = m3[c];
-      triad_sample<1>(p, p.gyro, p.ref_gyro + t * 3, static_cast<uint32_t>(t), run_lo, run_hi, run, phase, false,
-                      r + 3, m3);
-      if constexpr (TERMS) terms_sample<1>(p, *x, t, run_lo, run_hi, false, r + 9, qe + 3, m3);
-      if constexpr (RUNERR) run_err_add(rerr[1], p.ref_gyro + t * 3, m3);
-#pragma unroll
-      for (int c = 0; c < 3; ++c) stage[1][el * 3 + c] = m3[c];
-    }
-    // ---- the affine scan of K1 ------------------------------------------------------------------
-    double sA[C], sE[C];
-#pragma unroll
-    for (int c = 0; c < C; ++c) {
-      sA[c] = c < 6 ? apow[mine][c] : 1.0;
-      sE[c] = r[c];
-    }
-    affine_scan_warp<C, kNoiseWarps>(sA, sE, wtot, lane, warp);
-    __syncthreads();
+  for (int64_t tile0 = cta.seg_lo; tile0 < cta.seg_hi; tile0 += kNoiseTile) {
+    const int cnt = static_cast<int>(min64(kNoiseTile, cta.seg_hi - tile0));
     double S[C];
-    affine_scan_block<C, kNoiseWarps>(sA, sE, wtot, lane, warp, carry, S);
+    const int mine = noise_tile<TERMS, RUNERR>(p, x, cta, phase, apow, rerr, stage, wtot, tile0, cnt, 0, carry, S);
     // ---- the thread's own samples: the measurement exactly as K1 stores it, minus the truth --------
     // pass A: e (kept in the stage), the end-point error, sum and max over the samples >= stats_start
     const int64_t t_lo = tile0 + tid * kNoisePer;
@@ -165,7 +109,7 @@ __device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, cons
       }
       if (t == p.n - 1) {
 #pragma unroll
-        for (int c = 0; c < 6; ++c) P.end_err[run * kErrCh + c] = e[c];
+        for (int c = 0; c < 6; ++c) P.end_err[cta.run * kErrCh + c] = e[c];
       }
       if (q >= q0) {
 #pragma unroll
@@ -237,9 +181,9 @@ __device__ __forceinline__ void imu_err_stats_body(const ErrStatsParams& P, cons
       chan_merge(n, m, m2, mx, red[w * kErrPartial], red[w * kErrPartial + 1 + c], red[w * kErrPartial + 7 + c],
                  red[w * kErrPartial + 13 + c]);
     if (p.nseg == 1) {
-      write_stats(P.proc_stats + run * 3 * kErrCh, c, kErrCh, n, m, m2, mx);
+      write_stats(P.proc_stats + cta.run * 3 * kErrCh, c, kErrCh, n, m, m2, mx);
     } else {
-      double* o = P.partial + (run * p.nseg + seg) * kErrPartial;
+      double* o = P.partial + (cta.run * p.nseg + cta.seg) * kErrPartial;
       if (c == 0) o[0] = n;
       o[1 + c] = m;
       o[7 + c] = m2;

@@ -103,9 +103,9 @@ def free_integration_odo(ref_frame, fs, gyro, odo, ini, earth_rot=True, layout=L
 
 def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0,
               vib_gyro=None, vib_accel=None, layout=LAYOUT_RUN_MAJOR, dump_z=False):
-    """K1.  ref_gyro/ref_accel: CUDA f64 [n,3]; *_err: imu_model dicts (with a non-zero 'q', 'rrw' or 'rr':
-    K1 with the IEEE Std 952 terms, b2ins_imu_noise_ex_f64; with a non-zero 'b_std', 'sf' or 'ma': K1 with the
-    run-to-run errors, b2ins_imu_noise_rx_f64).
+    """K1 (b2ins_imu_noise_rx_f64).  ref_gyro/ref_accel: CUDA f64 [n,3]; *_err: imu_model dicts (a non-zero
+    'q', 'rrw' or 'rr' adds the IEEE Std 952 terms, a non-zero 'b_std', 'sf' or 'ma' the run-to-run errors; the
+    entry point launches the K1 form with what is set).
     Returns gyro, accel ([R,n,3], [n,3,R] or, LAYOUT_CHANNEL_MAJOR, [R,3,n]) and, if dump_z,
     z [R,n,12]."""
     _require_cuda()
@@ -117,25 +117,12 @@ def imu_noise(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offs
     accel = torch.empty_like(gyro)
     z = torch.empty((runs, n, 12), dtype=torch.float64, device=ref_gyro.device) if dump_z else None
     ge, ae = _lib.sensor_err(gyro_err, 'arw'), _lib.sensor_err(accel_err, 'vrw')
-    vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
-    va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
-    tg, ta = _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err)
-    xg, xa = _lib.run_err(gyro_err), _lib.run_err(accel_err)
-    if xg is not None or xa is not None:
-        _lib.check(lib.b2ins_imu_noise_rx_f64(
-            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
-            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
-            _ptr(gyro), _ptr(accel), _ptr(z), xg, xa, _stream()))
-    elif tg is None and ta is None:
-        _lib.check(lib.b2ins_imu_noise_f64(
-            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
-            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
-            _ptr(gyro), _ptr(accel), _ptr(z), _stream()))
-    else:
-        _lib.check(lib.b2ins_imu_noise_ex_f64(
-            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
-            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), layout,
-            _ptr(gyro), _ptr(accel), _ptr(z), _stream()))
+    vg, va = _lib.vib(vib_gyro), _lib.vib(vib_accel)
+    _lib.check(lib.b2ins_imu_noise_rx_f64(
+        float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
+        _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err), ctypes.byref(vg), ctypes.byref(va), int(seed),
+        int(run_offset), layout, _ptr(gyro), _ptr(accel), _ptr(z), _lib.run_err(gyro_err), _lib.run_err(accel_err),
+        _stream()))
     return (gyro, accel, z) if dump_z else (gyro, accel)
 
 
@@ -242,7 +229,8 @@ def mag_calibrate_mc(runs, segments, ref_mag, mag_err, seed, run_offset=0, want_
 
 def imu_err_stats(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_offset=0,
                   vib_gyro=None, vib_accel=None, stats_start=-1):
-    """K9: error statistics of the measurements imu_noise would make, reduced inside the generator.
+    """K9 (b2ins_imu_err_stats_rx_f64): error statistics of the measurements imu_noise would make, reduced
+    inside the generator.
     Returns end_err [R,6] (e = meas - ref at the last sample; accel x y z, gyro x y z) and, if
     stats_start >= 0, proc_stats [R,3,6] (max|e|, mean, std over samples >= stats_start), else None."""
     _require_cuda()
@@ -252,25 +240,12 @@ def imu_err_stats(fs, runs, ref_gyro, ref_accel, gyro_err, accel_err, seed, run_
     end_err = torch.empty((runs, 6), dtype=torch.float64, device=dev)
     proc = torch.empty((runs, 3, 6), dtype=torch.float64, device=dev) if stats_start >= 0 else None
     ge, ae = _lib.sensor_err(gyro_err, 'arw'), _lib.sensor_err(accel_err, 'vrw')
-    vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
-    va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
-    tg, ta = _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err)
-    xg, xa = _lib.run_err(gyro_err), _lib.run_err(accel_err)
-    if xg is not None or xa is not None:
-        _lib.check(lib.b2ins_imu_err_stats_rx_f64(
-            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
-            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
-            _ptr(end_err), _ptr(proc), xg, xa, _stream()))
-    elif tg is None and ta is None:
-        _lib.check(lib.b2ins_imu_err_stats_f64(
-            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
-            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
-            _ptr(end_err), _ptr(proc), _stream()))
-    else:
-        _lib.check(lib.b2ins_imu_err_stats_ex_f64(
-            float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae), tg, ta,
-            ctypes.byref(vg), ctypes.byref(va), int(seed), int(run_offset), int(stats_start),
-            _ptr(end_err), _ptr(proc), _stream()))
+    vg, va = _lib.vib(vib_gyro), _lib.vib(vib_accel)
+    _lib.check(lib.b2ins_imu_err_stats_rx_f64(
+        float(fs), runs, n, _ptr(ref_gyro), _ptr(ref_accel), ctypes.byref(ge), ctypes.byref(ae),
+        _lib.noise_terms(gyro_err), _lib.noise_terms(accel_err), ctypes.byref(vg), ctypes.byref(va), int(seed),
+        int(run_offset), int(stats_start), _ptr(end_err), _ptr(proc), _lib.run_err(gyro_err), _lib.run_err(accel_err),
+        _stream()))
     return end_err, proc
 
 
@@ -320,8 +295,8 @@ def make_mc_config(ref_frame, fs, n, runs, seed, gyro_err, accel_err, ini_sets, 
     cfg.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
     cfg.gyro_err = _lib.sensor_err(gyro_err, 'arw')
     cfg.accel_err = _lib.sensor_err(accel_err, 'vrw')
-    cfg.vib_gyro = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
-    cfg.vib_accel = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
+    cfg.vib_gyro = _lib.vib(vib_gyro)
+    cfg.vib_accel = _lib.vib(vib_accel)
     cfg._keep_vib = (vib_gyro, vib_accel)   # assignment copies the structs: keep the series tensors alive
     cfg.ini_sets = int(ini_sets)
     cfg.ini_rows = int(ini_rows)
@@ -740,8 +715,7 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     cfg = _ekf_config(fs, n, runs, m, seed, gyro_err, accel_err, gps_err, _ekf_ini(ini, align), run_offset,
                       ini_att_std, earth_rot, stats_start, dump_runs, dump_stride, vel_rw, att_rw)
     # Vib structs are passed by pointer; a VIB_SERIES Vib keeps its series tensor alive through the call
-    vg = vib_gyro if isinstance(vib_gyro, _lib.Vib) else _lib.vib(vib_gyro)
-    va = vib_accel if isinstance(vib_accel, _lib.Vib) else _lib.vib(vib_accel)
+    vg, va = _lib.vib(vib_gyro), _lib.vib(vib_accel)
     res = _ekf_result(out, runs, n, dump_runs, dump_stride, dev, end_err=True)
     res.consist = _reuse(res.consist, (runs, 19), dev)
     refs = (_ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps), ctypes.c_void_p(gps_idx.data_ptr()),

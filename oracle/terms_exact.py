@@ -1,7 +1,7 @@
 """The exact IEEE Std 952 terms (quantisation, rate random walk, rate ramp) and run-to-run errors of K1's and K9's
 _ex and _rx forms, built from the doubles the device uses: the reference of tests/test_gpu_terms_exact.py.
 
-Coefficients, as digest_terms and noise_prepare make them from the imu_model values Q, K, R (SI units):
+Coefficients, as digest_terms and digest_noise make them from the imu_model values Q, K, R (SI units):
     q = fl(Q fl(sqrt 12)),   k = fl(K fl(sqrt(dt))),   dt = fl(1 / fs)
 Per axis of one sensor, sample t (noise952_np states the model):
     quantisation   e[t] = fl(q (u[t] - 1/2)), u[t] = uniform01 (an integer times 2^-52 in [0, 1), so u - 1/2 is
