@@ -144,6 +144,10 @@ SIGNATURES = {
     'b2ins_ins_loose_align_f64': (_I, [ctypes.POINTER(EkfConfig), ctypes.POINTER(EkfAlign), _VB, _VB, _L, _I]
                                   + [_P] * 16),
     'b2ins_ins_loose_fed_align_f64': (_I, [ctypes.POINTER(EkfConfig), ctypes.POINTER(EkfAlign)] + [_P] * 14),
+    'b2ins_ins_loose_rx_f64': (_I, [ctypes.POINTER(EkfConfig), ctypes.POINTER(EkfAlign), _VB, _VB, _L, _I]
+                               + [_P] * 15 + [_RE, _RE, _P, _P]),
+    'b2ins_ins_loose_fed_rx_f64': (_I, [ctypes.POINTER(EkfConfig), ctypes.POINTER(EkfAlign), _I] + [_P] * 13
+                                   + [_RE, _RE, _P]),
     'b2ins_diag_dfma_rate': (_I, [c_double_p]),
     'b2ins_diag_auto_lanes': (_I, [_L, _I, _I]),
     'b2ins_diag_mc_shape': (_I, [_I, _I, ctypes.POINTER(ctypes.c_int)]),

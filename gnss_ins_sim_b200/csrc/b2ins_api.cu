@@ -1226,19 +1226,10 @@ double* b2ins_mc_plan_err_device(b2ins_mc_plan* plan) { return plan ? plan->d_ou
 void* b2ins_mc_plan_stream(b2ins_mc_plan* plan) { return plan ? plan->stream : nullptr; }
 
 // ---------------------------------------------------------------- K7 --------
+static int ekf_run_bias(const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, double* rb, bool* any);
 static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
-                      int ndump, EkfParams* out);
+                      const double* rb, int ndump, EkfParams* out);
 static int ekf_align_params(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, EkfParams* p);
-static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
-                         const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame, const double* ref_gyro,
-                         const double* ref_accel, const double* ref_nav, const double* ref_gps,
-                         const int64_t* gps_idx, const double* gps_vis, double* end_err, double* end_bias,
-                         double* consist, double* proc_stats, double* dump_att, double* dump_pos, double* dump_vel,
-                         double* dump_wb, double* dump_ab, void* stream);
-static int ins_loose_fed(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, int ini_draw, const double* gyro,
-                         const double* accel, const double* gps, const int64_t* gps_idx, const double* gps_vis,
-                         const double* ref_nav, double* end_err, double* end_bias, double* dump_att, double* dump_pos,
-                         double* dump_vel, double* dump_wb, double* dump_ab, void* stream);
 
 int b2ins_ins_loose_f64(const b2ins_ekf_config* cfg, const double* ref_gyro, const double* ref_accel,
                         const double* ref_nav, const double* ref_gps, const int64_t* gps_idx,
@@ -1254,9 +1245,9 @@ int b2ins_ins_loose_ex_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyr
                            const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
                            double* end_bias, double* consist, double* dump_att, double* dump_pos,
                            double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
-  return ins_loose_gen(cfg, nullptr, vib_gyro, vib_accel, -1, B2INS_POS_FRAME_LLA, ref_gyro, ref_accel, ref_nav,
-                       ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, nullptr, dump_att, dump_pos, dump_vel,
-                       dump_wb, dump_ab, stream);
+  return b2ins_ins_loose_rx_f64(cfg, nullptr, vib_gyro, vib_accel, -1, B2INS_POS_FRAME_LLA, ref_gyro, ref_accel,
+                                ref_nav, ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, nullptr, dump_att,
+                                dump_pos, dump_vel, dump_wb, dump_ab, nullptr, nullptr, nullptr, stream);
 }
 
 int b2ins_ins_loose_proc_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
@@ -1270,9 +1261,9 @@ int b2ins_ins_loose_proc_f64(const b2ins_ekf_config* cfg, const b2ins_vib* vib_g
             "proc_pos_frame must be B2INS_POS_FRAME_*");
   ARG_CHECK(proc_stats, "null buffer: proc_stats is required");
   ARG_CHECK(proc_start >= 0 && proc_start < cfg->n, "proc_start must be in [0, n)");
-  return ins_loose_gen(cfg, nullptr, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel, ref_nav,
-                       ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att, dump_pos, dump_vel,
-                       dump_wb, dump_ab, stream);
+  return b2ins_ins_loose_rx_f64(cfg, nullptr, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel,
+                                ref_nav, ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att,
+                                dump_pos, dump_vel, dump_wb, dump_ab, nullptr, nullptr, nullptr, stream);
 }
 
 int b2ins_ins_loose_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
@@ -1281,26 +1272,32 @@ int b2ins_ins_loose_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align
                               const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
                               double* end_bias, double* consist, double* proc_stats, double* dump_att,
                               double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+  return b2ins_ins_loose_rx_f64(cfg, align, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel,
+                                ref_nav, ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att,
+                                dump_pos, dump_vel, dump_wb, dump_ab, nullptr, nullptr, nullptr, stream);
+}
+
+// K7 on generated measurements, the launch site of every generated form: ekf_kernel<VIB, false, PROC> (PROC:
+// proc_stats given), and with a turn-on bias or end_bias_err its RB form
+int b2ins_ins_loose_rx_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
+                           const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame,
+                           const double* ref_gyro, const double* ref_accel, const double* ref_nav,
+                           const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
+                           double* end_bias, double* consist, double* proc_stats, double* dump_att,
+                           double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab,
+                           const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, double* end_bias_err,
+                           void* stream) {
   ARG_CHECK(cfg, "cfg is null");
-  ARG_CHECK((proc_stats == nullptr) == (proc_start == -1), "proc_stats and proc_start >= 0 must be given together");
   if (proc_stats) {
     ARG_CHECK(proc_pos_frame >= B2INS_POS_FRAME_LLA && proc_pos_frame <= B2INS_POS_FRAME_ECEF,
               "proc_pos_frame must be B2INS_POS_FRAME_*");
     ARG_CHECK(proc_start >= 0 && proc_start < cfg->n, "proc_start must be in [0, n)");
   }
-  return ins_loose_gen(cfg, align, vib_gyro, vib_accel, proc_start, proc_pos_frame, ref_gyro, ref_accel, ref_nav,
-                       ref_gps, gps_idx, gps_vis, end_err, end_bias, consist, proc_stats, dump_att, dump_pos, dump_vel,
-                       dump_wb, dump_ab, stream);
-}
-
-// K7 on generated measurements; proc_stats NULL: no process statistics (ekf_kernel<VIB, false, false>)
-static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
-                         const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame, const double* ref_gyro,
-                         const double* ref_accel, const double* ref_nav, const double* ref_gps,
-                         const int64_t* gps_idx, const double* gps_vis, double* end_err, double* end_bias,
-                         double* consist, double* proc_stats, double* dump_att, double* dump_pos, double* dump_vel,
-                         double* dump_wb, double* dump_ab, void* stream) {
-  ARG_CHECK(cfg, "cfg is null");
+  ARG_CHECK((proc_stats == nullptr) == (proc_start == -1), "proc_stats and proc_start >= 0 must be given together");
+  double rb[6];
+  bool any_rb;
+  int rc = ekf_run_bias(gyro_run, accel_run, rb, &any_rb);
+  if (rc != B2INS_OK) return rc;
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
   if (cfg->runs == 0 || cfg->n == 0) return B2INS_OK;
@@ -1313,7 +1310,7 @@ static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_ekf_align* ali
   ARG_CHECK(ndump == 0 || ndump == 5, "dump_att/pos/vel/wb/ab must be given together");
   ARG_CHECK(cfg->dump_stride >= 0, "dump_stride must be >= 0");
   EkfParams p;
-  int rc = ekf_params(cfg, vib_gyro, vib_accel, ndump, &p);
+  rc = ekf_params(cfg, vib_gyro, vib_accel, rb, ndump, &p);
   if (rc != B2INS_OK) return rc;
   rc = ekf_align_params(cfg, align, &p);
   if (rc != B2INS_OK) return rc;
@@ -1335,10 +1332,23 @@ static int ins_loose_gen(const b2ins_ekf_config* cfg, const b2ins_ekf_align* ali
   p.proc_stats = proc_stats;
   p.proc_start = proc_start;
   p.proc_pos_frame = proc_pos_frame;
+  p.end_bias_err = end_bias_err;
   const unsigned grid = static_cast<unsigned>((cfg->runs + kEkfRuns - 1) / kEkfRuns);
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool vib = !(p.gyro.vib_type == B2INS_VIB_NONE && p.accel.vib_type == B2INS_VIB_NONE);
-  if (proc_stats) {
+  if (any_rb || end_bias_err) {
+    if (proc_stats) {
+      if (vib)
+        ekf_kernel<true, false, true, false, true><<<grid, kEkfThreads, 0, s>>>(p);
+      else
+        ekf_kernel<false, false, true, false, true><<<grid, kEkfThreads, 0, s>>>(p);
+    } else {
+      if (vib)
+        ekf_kernel<true, false, false, false, true><<<grid, kEkfThreads, 0, s>>>(p);
+      else
+        ekf_kernel<false, false, false, false, true><<<grid, kEkfThreads, 0, s>>>(p);
+    }
+  } else if (proc_stats) {
     if (vib)
       ekf_kernel<true, false, true><<<grid, kEkfThreads, 0, s>>>(p);
     else
@@ -1357,8 +1367,8 @@ int b2ins_ins_loose_fed_f64(const b2ins_ekf_config* cfg, int ini_draw, const dou
                             const double* gps, const int64_t* gps_idx, const double* gps_vis,
                             const double* ref_nav, double* end_err, double* end_bias, double* dump_att,
                             double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
-  return ins_loose_fed(cfg, nullptr, ini_draw, gyro, accel, gps, gps_idx, gps_vis, ref_nav, end_err, end_bias,
-                       dump_att, dump_pos, dump_vel, dump_wb, dump_ab, stream);
+  return b2ins_ins_loose_fed_rx_f64(cfg, nullptr, ini_draw, gyro, accel, gps, gps_idx, gps_vis, ref_nav, end_err,
+                                    end_bias, dump_att, dump_pos, dump_vel, dump_wb, dump_ab, nullptr, nullptr, stream);
 }
 
 int b2ins_ins_loose_fed_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const double* gyro,
@@ -1366,20 +1376,27 @@ int b2ins_ins_loose_fed_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_a
                                   const double* gps_vis, const double* ref_nav, double* end_err, double* end_bias,
                                   double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb,
                                   double* dump_ab, void* stream) {
-  return ins_loose_fed(cfg, align, 0, gyro, accel, gps, gps_idx, gps_vis, ref_nav, end_err, end_bias, dump_att,
-                       dump_pos, dump_vel, dump_wb, dump_ab, stream);
+  return b2ins_ins_loose_fed_rx_f64(cfg, align, 0, gyro, accel, gps, gps_idx, gps_vis, ref_nav, end_err, end_bias,
+                                    dump_att, dump_pos, dump_vel, dump_wb, dump_ab, nullptr, nullptr, stream);
 }
 
-// K7 on supplied measurements (ekf_kernel<false, true, false, aligned>)
-static int ins_loose_fed(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, int ini_draw, const double* gyro,
-                         const double* accel, const double* gps, const int64_t* gps_idx, const double* gps_vis,
-                         const double* ref_nav, double* end_err, double* end_bias, double* dump_att, double* dump_pos,
-                         double* dump_vel, double* dump_wb, double* dump_ab, void* stream) {
+// K7 on supplied measurements, the launch site of every fed form (ekf_kernel<false, true, false, aligned>); the
+// turn-on bias is in the data and enters the model through P0 only
+int b2ins_ins_loose_fed_rx_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, int ini_draw,
+                               const double* gyro, const double* accel, const double* gps, const int64_t* gps_idx,
+                               const double* gps_vis, const double* ref_nav, double* end_err, double* end_bias,
+                               double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab,
+                               const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, void* stream) {
   ARG_CHECK(cfg, "cfg is null");
   ARG_CHECK(cfg->fs > 0.0, "fs must be positive");
   ARG_CHECK(cfg->runs >= 0 && cfg->n >= 0 && cfg->m >= 0, "runs, n and m must be non-negative");
   ARG_CHECK(ini_draw == 0 || ini_draw == 1, "ini_draw must be 0 or 1");
+  ARG_CHECK(ini_draw == 0 || !align || align->mode == B2INS_ALIGN_OFF, "an aligned filter makes no initial draw");
   ARG_CHECK((end_err == nullptr) == (ref_nav == nullptr), "end_err and ref_nav must be given together");
+  double rb[6];
+  bool any_rb;
+  int rc = ekf_run_bias(gyro_run, accel_run, rb, &any_rb);
+  if (rc != B2INS_OK) return rc;
   if (cfg->runs == 0 || cfg->n == 0) return B2INS_OK;
   ARG_CHECK(cfg->n < (int64_t(1) << 32), "n must be < 2^32");
   ARG_CHECK(gyro && accel, "null buffer: gyro and accel are required");
@@ -1390,7 +1407,7 @@ static int ins_loose_fed(const b2ins_ekf_config* cfg, const b2ins_ekf_align* ali
   ARG_CHECK(ndump == 0 || ndump == 5, "dump_att/pos/vel/wb/ab must be given together");
   ARG_CHECK(cfg->dump_stride >= 0, "dump_stride must be >= 0");
   EkfParams p;
-  int rc = ekf_params(cfg, nullptr, nullptr, ndump, &p);
+  rc = ekf_params(cfg, nullptr, nullptr, rb, ndump, &p);
   if (rc != B2INS_OK) return rc;
   rc = ekf_align_params(cfg, align, &p);
   if (rc != B2INS_OK) return rc;
@@ -1417,10 +1434,32 @@ static int ins_loose_fed(const b2ins_ekf_config* cfg, const b2ins_ekf_align* ali
   return B2INS_OK;
 }
 
+// The turn-on bias of the run errors for K7: rb = the 1-sigma per generator channel (accel x y z, gyro x y z), zero
+// for a null struct; *any is false when all are zero.  The filter's states hold a bias but no scale factor or
+// misalignment, so sf and ma must be zero; b is checked as digest_run_err checks it.
+static int ekf_run_bias(const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, double* rb, bool* any) {
+  RunErrs re;
+  bool unused;
+  const int rc = digest_run_err(gyro_run, accel_run, &re, &unused);
+  if (rc != B2INS_OK) return rc;
+  *any = false;
+  for (int s = 0; s < 2; ++s) {
+    for (int c = 0; c < 3; ++c) {
+      ARG_CHECK(re.s[s].sf[c] == 0.0, "the loosely-coupled filter takes no run-to-run scale factor: sf must be 0");
+      for (int j = 0; j < 3; ++j)
+        ARG_CHECK(re.s[s].ma[c][j] == 0.0, "the loosely-coupled filter takes no run-to-run misalignment: ma must be 0");
+      rb[3 * s + c] = re.s[s].b[c];
+      *any = *any || rb[3 * s + c] != 0.0;
+    }
+  }
+  return B2INS_OK;
+}
+
 // The filter model of cfg (Q, R, P0, bias model, initial state) and the launch geometry of K7; the
-// caller sets the buffers.  vib_*: the generator's vibration (NULL for supplied measurements).
+// caller sets the buffers.  vib_*: the generator's vibration (NULL for supplied measurements); rb: the turn-on
+// bias sigmas of ekf_run_bias.
 static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, const b2ins_vib* vib_accel,
-                      int ndump, EkfParams* out) {
+                      const double* rb, int ndump, EkfParams* out) {
   EkfParams& p = *out;
   std::memset(&p, 0, sizeof(p));
   p.n = cfg->n;
@@ -1441,8 +1480,13 @@ static int ekf_params(const b2ins_ekf_config* cfg, const b2ins_vib* vib_gyro, co
     p.p0[c] = cfg->gps_stdp[c] * cfg->gps_stdp[c];
     p.p0[3 + c] = cfg->gps_stdv[c] * cfg->gps_stdv[c];
     p.p0[6 + c] = cfg->ini_att_std[c] * cfg->ini_att_std[c];
-    p.p0[9 + c] = cfg->gyro_err.b_drift[c] * cfg->gyro_err.b_drift[c] + cfg->gyro_err.b[c] * cfg->gyro_err.b[c];
-    p.p0[12 + c] = cfg->accel_err.b_drift[c] * cfg->accel_err.b_drift[c] + cfg->accel_err.b[c] * cfg->accel_err.b[c];
+    // the bias states: the drift, the constant bias the filter does not know and the run's turn-on bias
+    p.rb[c] = rb[c];
+    p.rb[3 + c] = rb[3 + c];
+    p.p0[9 + c] = cfg->gyro_err.b_drift[c] * cfg->gyro_err.b_drift[c] + cfg->gyro_err.b[c] * cfg->gyro_err.b[c] +
+                  rb[3 + c] * rb[3 + c];
+    p.p0[12 + c] = cfg->accel_err.b_drift[c] * cfg->accel_err.b_drift[c] + cfg->accel_err.b[c] * cfg->accel_err.b[c] +
+                   rb[c] * rb[c];
     // the filter's bias model is the generator's: a = 1 - dt/tau, b^2 (white drift: a = 0, b = drift)
     const bool wg = std::isinf(cfg->gyro_err.b_corr[c]), wa = std::isinf(cfg->accel_err.b_corr[c]);
     p.ag[c] = wg ? 0.0 : p.gyro.gm_a[c];
@@ -1476,7 +1520,8 @@ static int ekf_align_params(const b2ins_ekf_config* cfg, const b2ins_ekf_align* 
   const b2ins_sensor_err& a = cfg->accel_err;
   for (int c = 0; c < 2; ++c) {
     const int ax = 1 - c;
-    p->align_p0[c] = (a.b[ax] * a.b[ax] + a.b_drift[ax] * a.b_drift[ax] + a.rw[ax] * a.rw[ax] * cfg->fs / kAlignN) /
+    p->align_p0[c] = (a.b[ax] * a.b[ax] + a.b_drift[ax] * a.b_drift[ax] + p->rb[ax] * p->rb[ax] +
+                      a.rw[ax] * a.rw[ax] * cfg->fs / kAlignN) /
                      (kG * kG);
   }
   p->align_yaw = align->yaw;

@@ -97,6 +97,13 @@ __device__ __forceinline__ Normal2 normal_pair(uint32_t t, uint32_t draw, uint32
   return normal_from_words(philox4x32_10(t, draw, run_lo, run_hi, k0, k1));
 }
 
+// pair j (0..5) of a run's run-to-run errors of sensor 0 (accel) or 1 (gyro): for j < 3, z0 is the turn-on bias of
+// axis j in units of its sigma (DESIGN.md section 4).  K1's and K9's run_err_pair and K7's RB forms draw through it.
+__device__ __forceinline__ Normal2 run_err_normals(int sensor, int j, uint32_t run_lo, uint32_t run_hi, uint32_t k0,
+                                                   uint32_t k1) {
+  return normal_pair(kRunErrT, kDrawRunErr + 6 * sensor + j, run_lo, run_hi, k0, k1);
+}
+
 __device__ __forceinline__ double uniform01(uint32_t t, uint32_t draw, uint32_t run_lo,
                                             uint32_t run_hi, uint32_t k0, uint32_t k1) {
   const PhiloxOut x = philox4x32_10(t, draw, run_lo, run_hi, k0, k1);

@@ -71,6 +71,11 @@ struct EkfParams {
   // yaw; P0 of the level N / E misalignment and of the given yaw; the gyro's arw^2 per axis
   int align;
   double align_yaw, align_p0[3], arw2[3];
+  // run-to-run turn-on bias (ekf_kernel<..., RB>; DESIGN.md section 11): the 1-sigma of every generator channel
+  // (accel x y z, gyro x y z), drawn per run and folded into the channel's constant bias; the bias estimates minus
+  // the true biases at sample n - 1, [runs][6] gyro then accel (NULL: not written)
+  double rb[6];
+  double* end_bias_err;
 };
 
 // The GPS row an aligned run starts at: the latest visible row at sample <= kAlignN - 1, else the first
@@ -177,9 +182,14 @@ __device__ __forceinline__ int ekf_own(int q, int m) {
 // in shared memory behind P, as [12][32 lanes], and lane 0 writes the run's [3][9] at the end.
 // FA (FED only): alignment is compiled in and on; on supplied data it is a compile-time choice, because the
 // run-time flag costs the fed form spills (ptxas -v).
-template <bool VIB, bool FED, bool PROC, bool FA = false>
+// RB (generated measurements only): every run draws its turn-on bias, p.rb[c] times z0 of run-error pair c % 3 of
+// sensor c / 3 (K1's draw, run_err_normals), once per channel in the prologue of the channel's owner lane, which
+// folds it into the channel's constant bias.  The consistency record's true bias and p.end_bias_err take each
+// channel's folded bias from its owner by quad shuffle, as they take its drift.
+template <bool VIB, bool FED, bool PROC, bool FA = false, bool RB = false>
 __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant__ EkfParams p) {
   static_assert(!(VIB && FED), "supplied measurements carry their vibration already");
+  static_assert(!(FED && RB), "supplied measurements carry their turn-on bias already");
   static_assert(FED || !FA, "generated measurements select the alignment at run time (p.align)");
   const bool aligned = FED ? FA : (p.align != 0);
   static_assert(!(FED && PROC), "supplied-data histories are on the host: their statistics are taken there");
@@ -263,6 +273,12 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   double b0, w0, wd0, ga0, gb0, b1, w1, wd1, ga1, gb1;
   model(c0, &b0, &w0, &wd0, &ga0, &gb0);
   model(two ? c1 : c0, &b1, &w1, &wd1, &ga1, &gb1);
+  if constexpr (RB) {
+    // lanes 2 and 3 draw channel c0 twice and drop the second, like their second chain
+    const int cc = two ? c1 : c0;
+    b0 += p.rb[c0] * run_err_normals(c0 / 3, c0 % 3, run_lo, run_hi, p.k0, p.k1).z0;
+    b1 += p.rb[cc] * run_err_normals(cc / 3, cc % 3, run_lo, run_hi, p.k0, p.k1).z0;
+  }
   double carry0 = 0.0, carry1 = 0.0;                              // d[i] of the lane's channels
   // vibration (VIB only) of the lane's accelerometer channel (axis q, lanes 0..2) and gyro channel (c0 of
   // lane 3: x; c1 of lanes 0 and 1: y, z; lane 2 computes axis z and drops it): amplitude, the PSD model's
@@ -556,6 +572,17 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
         double dch[6];
         dch[0] = quad(carry0, 0); dch[1] = quad(carry0, 1); dch[2] = quad(carry0, 2); dch[3] = quad(carry0, 3);
         dch[4] = quad(carry1, 0); dch[5] = quad(carry1, 1);
+        // the generator's constant bias of every channel; RB: with the run's turn-on bias, from its owner
+        double bch[6];
+#pragma unroll
+        for (int c3 = 0; c3 < 3; ++c3) {
+          bch[c3] = p.accel.b[c3];
+          bch[3 + c3] = p.gyro.b[c3];
+        }
+        if constexpr (RB) {
+          bch[0] = quad(b0, 0); bch[1] = quad(b0, 1); bch[2] = quad(b0, 2); bch[3] = quad(b0, 3);
+          bch[4] = quad(b1, 0); bch[5] = quad(b1, 1);
+        }
         const double* rn9 = p.ref_nav + i * 9;
         const GeoParam gp = geo_param(rn9[3], rn9[5]);
         double e[kEkfN];
@@ -579,8 +606,8 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
         e[8] = -0.5 * (m10 - m01);
 #pragma unroll
         for (int c3 = 0; c3 < 3; ++c3) {
-          e[9 + c3] = bg[c3] - (p.gyro.b[c3] + dch[3 + c3]);
-          e[12 + c3] = ba[c3] - (p.accel.b[c3] + dch[c3]);
+          e[9 + c3] = bg[c3] - (bch[3 + c3] + dch[3 + c3]);
+          e[12 + c3] = ba[c3] - (bch[c3] + dch[c3]);
         }
 #pragma unroll
         for (int b = 0; b < 3; ++b) {
@@ -739,6 +766,13 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
   }
 
   if constexpr (PROC) __syncwarp();       // lane 0 reads the accumulators of lanes 8 and 16 of its run
+  // RB: the true bias of every channel at sample n - 1, b + b_run + d[n-1], from its owner
+  double btrue[6];
+  if constexpr (RB) {
+    const double t0 = b0 + carry0, t1 = b1 + carry1;
+    btrue[0] = quad(t0, 0); btrue[1] = quad(t0, 1); btrue[2] = quad(t0, 2); btrue[3] = quad(t0, 3);
+    btrue[4] = quad(t1, 0); btrue[5] = quad(t1, 1);
+  }
   if (active && q == 0) {
     if constexpr (PROC) {
       double* o = p.proc_stats + run * 27;
@@ -769,6 +803,13 @@ __global__ void __launch_bounds__(kEkfThreads) ekf_kernel(const __grid_constant_
       for (int c3 = 0; c3 < 3; ++c3) {
         p.end_bias[run * 6 + c3] = bg[c3];
         p.end_bias[run * 6 + 3 + c3] = ba[c3];
+      }
+    }
+    if (RB && p.end_bias_err) {
+#pragma unroll
+      for (int c3 = 0; c3 < 3; ++c3) {
+        p.end_bias_err[run * 6 + c3] = bg[c3] - btrue[3 + c3];
+        p.end_bias_err[run * 6 + 3 + c3] = ba[c3] - btrue[c3];
       }
     }
     if (!FED && p.consist) {

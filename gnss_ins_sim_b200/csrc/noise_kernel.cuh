@@ -116,7 +116,7 @@ struct RunErrs {
 // K1's and K9's prologues (one thread per pair) and imu_run_err_kernel (one thread per sensor) share it.
 __device__ __forceinline__ void run_err_pair(const RunErrSigma& s, int sensor, int j, uint32_t run_lo,
                                              uint32_t run_hi, uint32_t k0, uint32_t k1, double* e12) {
-  const Normal2 z = normal_pair(kRunErrT, kDrawRunErr + 6 * sensor + j, run_lo, run_hi, k0, k1);
+  const Normal2 z = run_err_normals(sensor, j, run_lo, run_hi, k0, k1);
   if (j < 3) {
     e12[9 + j] = s.b[j] * z.z0;
     e12[4 * j] = s.sf[j] * z.z1;

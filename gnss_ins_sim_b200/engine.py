@@ -687,6 +687,7 @@ class EkfResult:
         self.end_bias = None     # [R,6] gyro, accel bias estimates at the last sample
         self.consist = None      # [R,19] NEES sums (pos, vel, att), inside-3-sigma counts [15], epochs
         self.proc_stats = None   # [R,3,9] max|e|, mean, std of att, pos, vel per run (proc_start given)
+        self.end_bias_err = None # [R,6] gyro, accel bias estimates minus the true biases at the last sample (bias_err)
         self.att = self.pos = self.vel = self.wb = self.ab = None   # [dump_runs,rows,3]
         self.start = 0           # first sample of the filter (aligned: the fix sample, align_fix)
 
@@ -694,7 +695,7 @@ class EkfResult:
 def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_accel, ref_nav, ref_gps,
               gps_idx, gps_vis, run_offset=0, ini_att_std=(0.02, 0.005, 0.005), earth_rot=True,
               stats_start=0, dump_runs=0, dump_stride=1, out=None, vel_rw=0.02, att_rw=0.0,
-              vib_gyro=None, vib_accel=None, proc_start=None, proc_pos_frame=0, align=None):
+              vib_gyro=None, vib_accel=None, proc_start=None, proc_pos_frame=0, align=None, bias_err=False):
     """K7: Monte-Carlo loosely-coupled GNSS/INS filter (the spec: DESIGN.md section 11; csrc/ekf_kernel.cuh).
     ref_gyro, ref_accel [n,3], ref_nav [n,9], ref_gps [m,6], gps_vis [m]: CUDA f64; gps_idx [m]: CUDA
     int64 (IMU sample index of every GPS row).  ini: the 9 true initial values (LLA, body velocity, Euler
@@ -705,8 +706,11 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     POS_FRAME_* proc_pos_frame (b2ins_ins_loose_proc_f64); every other output is unchanged.  align = (yaw, yaw_var):
     every run initialises itself from its measurements (b2ins_ins_loose_align_f64; yaw a heading [rad] with
     variance yaw_var, or 'gps'); ini is then unused, res.start is the fix sample (align_fix), the consistency
-    record takes the epochs after it and proc statistics start at max(proc_start, res.start).  Asynchronous on
-    the current stream (with align, after one host copy of gps_idx / gps_vis)."""
+    record takes the epochs after it and proc statistics start at max(proc_start, res.start).  The IMU's turn-on bias
+    'b_std' (imu_model; 'sf' and 'ma' are refused) is drawn per run as K1 draws it and is in the filter's P0 and in
+    the consistency record's truth (b2ins_ins_loose_rx_f64).  bias_err: also res.end_bias_err [R,6], the bias
+    estimates minus the true biases at the last sample.  Asynchronous on the current stream (with align, after one
+    host copy of gps_idx / gps_vis)."""
     _require_cuda()
     lib = _lib.load()
     n, m = ref_gyro.shape[0], ref_gps.shape[0]
@@ -718,23 +722,30 @@ def ins_loose(fs, runs, seed, gyro_err, accel_err, gps_err, ini, ref_gyro, ref_a
     vg, va = _lib.vib(vib_gyro), _lib.vib(vib_accel)
     res = _ekf_result(out, runs, n, dump_runs, dump_stride, dev, end_err=True)
     res.consist = _reuse(res.consist, (runs, 19), dev)
+    res.proc_stats = None if proc_start is None else _reuse(res.proc_stats, (runs, 3, 9), dev)
+    res.end_bias_err = _reuse(res.end_bias_err, (runs, 6), dev) if bias_err else None
     refs = (_ptr(ref_gyro), _ptr(ref_accel), _ptr(ref_nav), _ptr(ref_gps), ctypes.c_void_p(gps_idx.data_ptr()),
             _ptr(gps_vis), _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.consist))
-    dumps = (_ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _stream())
+    dumps = (_ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab))
     if align is not None:
         res.start = align_fix(gps_idx.cpu().numpy(), gps_vis.cpu().numpy())[1]
-        res.proc_stats = None if proc_start is None else _reuse(res.proc_stats, (runs, 3, 9), dev)
+    ps = -1 if proc_start is None else int(proc_start)
+    gr, ar = _lib.run_err(gyro_err), _lib.run_err(accel_err)
+    if gr is not None or ar is not None or bias_err:
+        _lib.check(lib.b2ins_ins_loose_rx_f64(
+            ctypes.byref(cfg), None if align is None else ctypes.byref(_ekf_align(align)), ctypes.byref(vg),
+            ctypes.byref(va), ps, int(proc_pos_frame), *refs, _ptr(res.proc_stats), *dumps, gr, ar,
+            _ptr(res.end_bias_err), _stream()))
+    elif align is not None:
         _lib.check(lib.b2ins_ins_loose_align_f64(
-            ctypes.byref(cfg), ctypes.byref(_ekf_align(align)), ctypes.byref(vg), ctypes.byref(va),
-            -1 if proc_start is None else int(proc_start), int(proc_pos_frame), *refs, _ptr(res.proc_stats), *dumps))
+            ctypes.byref(cfg), ctypes.byref(_ekf_align(align)), ctypes.byref(vg), ctypes.byref(va), ps,
+            int(proc_pos_frame), *refs, _ptr(res.proc_stats), *dumps, _stream()))
     elif proc_start is None:
-        res.proc_stats = None
-        _lib.check(lib.b2ins_ins_loose_ex_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), *refs, *dumps))
+        _lib.check(lib.b2ins_ins_loose_ex_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), *refs, *dumps,
+                                              _stream()))
     else:
-        res.proc_stats = _reuse(res.proc_stats, (runs, 3, 9), dev)
-        _lib.check(lib.b2ins_ins_loose_proc_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va),
-                                                int(proc_start), int(proc_pos_frame), *refs,
-                                                _ptr(res.proc_stats), *dumps))
+        _lib.check(lib.b2ins_ins_loose_proc_f64(ctypes.byref(cfg), ctypes.byref(vg), ctypes.byref(va), ps,
+                                                int(proc_pos_frame), *refs, _ptr(res.proc_stats), *dumps, _stream()))
     return res
 
 
@@ -748,7 +759,9 @@ def ins_loose_fed(fs, gyro, accel, gps, gps_idx, gps_vis, gyro_err, accel_err, g
     experiment's draw).  ref_nav [n,9] (optional): end_err as engine.ins_loose makes it.  Returns an
     EkfResult without consist (and without end_err when ref_nav is None).  align = (yaw, yaw_var): every run
     initialises itself from its measurements instead (b2ins_ins_loose_fed_align_f64; ini, seed and ini_draw are
-    unused), res.start is the fix sample.  Asynchronous on the current stream."""
+    unused), res.start is the fix sample.  The model's turn-on bias 'b_std' enters P0 as in ins_loose (the
+    measurements carry each run's bias); its 'sf' and 'ma' are not filter states and are not used.  Asynchronous on
+    the current stream."""
     _require_cuda()
     lib = _lib.load()
     R, n, three = gyro.shape
@@ -765,12 +778,18 @@ def ins_loose_fed(fs, gyro, accel, gps, gps_idx, gps_vis, gyro_err, accel_err, g
                       earth_rot, -1, dump_runs, dump_stride, vel_rw, att_rw)
     res = _ekf_result(out, R, n, dump_runs, dump_stride, gyro.device, end_err=ref_nav is not None)
     res.consist = None
-    bufs = (_ptr(gyro), _ptr(accel), _ptr(gps), ctypes.c_void_p(gps_idx.data_ptr()), _ptr(gps_vis), _ptr(ref_nav),
-            _ptr(res.end_err), _ptr(res.end_bias), _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb),
-            _ptr(res.ab), _stream())
-    if align is None:
-        _lib.check(lib.b2ins_ins_loose_fed_f64(ctypes.byref(cfg), int(bool(ini_draw)), *bufs))
-    else:
+    if align is not None:
         res.start = align_fix(gps_idx.cpu().numpy(), gps_vis.cpu().numpy())[1]
-        _lib.check(lib.b2ins_ins_loose_fed_align_f64(ctypes.byref(cfg), ctypes.byref(_ekf_align(align)), *bufs))
+    _lib.check(lib.b2ins_ins_loose_fed_rx_f64(
+        ctypes.byref(cfg), None if align is None else ctypes.byref(_ekf_align(align)),
+        int(bool(ini_draw)) if align is None else 0, _ptr(gyro), _ptr(accel), _ptr(gps),
+        ctypes.c_void_p(gps_idx.data_ptr()), _ptr(gps_vis), _ptr(ref_nav), _ptr(res.end_err), _ptr(res.end_bias),
+        _ptr(res.att), _ptr(res.pos), _ptr(res.vel), _ptr(res.wb), _ptr(res.ab), _turn_on_bias(gyro_err),
+        _turn_on_bias(accel_err), _stream()))
     return res
+
+
+def _turn_on_bias(err):
+    """RunErr of an imu_model dict's turn-on bias 'b_std' alone (None without one): what the fed filter's model
+    takes of the run-to-run errors."""
+    return _lib.run_err({'b_std': err['b_std']} if 'b_std' in err else {})

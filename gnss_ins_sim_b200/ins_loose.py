@@ -83,6 +83,16 @@ class InsLoose(object):
         (plus any att_model_std of its own, in quadrature).  With the default model the velocity and
         attitude blocks become overconfident (DESIGN.md section 11 has the figures).
 
+        Turn-on bias: an IMU with gyro_b_std / accel_b_std (imu_model 'b_std') gives every run of a Sim its own
+        constant bias, drawn as K1 draws it (Sim.imu_run_errors() lists them).  The filter's model knows its
+        spread: the bias states start at b_drift^2 + b^2 + b_std^2 (and the aligned level and gap terms grow
+        with it), so the gyro- and accel-bias states estimate each run's bias.  Sim.ekf_consistency()['bias_err']
+        gives how far each run's estimate ends from the truth.  The bias states are Gauss-Markov: on runs much
+        longer than the bias correlation time the filter lets the constant part decay and becomes overconfident
+        on the bias and attitude states (DESIGN.md section 11, "Turn-on bias", has the config-5 figures).  On
+        supplied measurements the model's b_std enters the same P0.  The other run-to-run and IEEE Std 952 errors (scale factor, misalignment, quantisation,
+        rate random walk, rate ramp) are not among the 15 states: a Sim refuses such an IMU.
+
         align_yaw: None (default): every run starts at the initial state above plus a draw from the initial
             covariance.  A heading [rad] or 'gps': every run initialises itself from its own measurements, with no
             initial state (DESIGN.md section 11, "Alignment"):

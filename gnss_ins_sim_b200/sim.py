@@ -480,10 +480,16 @@ class Sim(object):
             raise ValueError('imu must be an IMU model when data are generated from a trajectory')
         terms = self._imu_terms()
         for a in self.algo or []:       # refused before anything of the Sim is reset
-            if terms and isinstance(a, (InsLoose, FreeIntegrationOdo)):
+            if terms and isinstance(a, FreeIntegrationOdo):
                 raise ValueError('%s generates its IMU inside its kernel, which makes no quantisation, rate '
                                  'random walk, rate ramp or run-to-run bias, scale-factor or misalignment error: '
                                  'the IMU sets %s' % (type(a).__name__, terms))
+            # K7 draws the turn-on bias; its 15 states have no place for the rest
+            rest = [t for t in terms if not t.endswith(' b_std')]
+            if rest and isinstance(a, InsLoose):
+                raise ValueError('%s generates its IMU inside its kernel, which makes no quantisation, rate '
+                                 'random walk, rate ramp or run-to-run scale-factor or misalignment error: '
+                                 'the IMU sets %s' % (type(a).__name__, rest))
         self._blocks = {}        # (block, name) -> [runs of the block, ...] host histories (_history)
         self._proc = {}          # (algo index, start [s], position frame) -> [R, 3, 9] process statistics
         self._sens = {}          # (source, first row) -> sensor error statistics (_sensor_launch)
@@ -974,7 +980,7 @@ class Sim(object):
         return d['ref_gps'], d['gps_idx'], d['gps_vis']
 
     def _ekf_launch(self, algo, r0, runs, stats_start=0, dump_runs=0, dump_stride=1, proc_start=None,
-                    proc_pos_frame=0):
+                    proc_pos_frame=0, bias_err=False):
         gps = self._ekf_inputs()
         d = self._dev
         ini = algo.ini if algo.ini is not None else self._traj.get('ini')
@@ -992,7 +998,7 @@ class Sim(object):
                                 stats_start=stats_start, dump_runs=dump_runs, dump_stride=dump_stride,
                                 vel_rw=algo.vel_model_std, att_rw=algo.att_model_std,
                                 vib_gyro=vib_gyro, vib_accel=vib_acc, proc_start=proc_start,
-                                proc_pos_frame=proc_pos_frame, align=algo.align())
+                                proc_pos_frame=proc_pos_frame, align=algo.align(), bias_err=bias_err)
 
     def _ekf_blocks(self, algo, **kw):
         """K7 over this rank's shard (kw: _ekf_launch's), in run blocks sized to the free device memory with PSD
@@ -1011,7 +1017,8 @@ class Sim(object):
     def _run_ins_loose(self, i, algo):
         """demo_ins_loose.py semantics, all runs of this rank in one K7 launch (in run blocks sized to the free
         device memory with PSD vibration, whose series K5 materialises, as for K9): end-point errors and their
-        ensemble statistics (as for free integration), bias estimates, the consistency record."""
+        ensemble statistics (as for free integration), bias estimates, the consistency record and, when the IMU
+        draws a turn-on bias, the bias-estimate errors."""
         name = self.algo_name(i)
         if algo.imu is not None and algo.imu is not self.imu:
             raise ValueError('a generating Sim filters with the IMU that makes its data: InsLoose(imu=...) must be '
@@ -1019,15 +1026,19 @@ class Sim(object):
         lo, hi = self._shard
         self._mc[i] = {'base': 0, 'end_err': None}
         err, stats, con, bias = np.zeros((0, 9)), np.zeros((3, 9)), np.zeros((0, 19)), np.zeros((0, 6))
+        turn_on = any(_lib.set_run_errors(e) for e in (self.imu.gyro_err, self.imu.accel_err))   # only 'b_std' here
+        bias_err = np.zeros((0, 6)) if turn_on else None
         if hi > lo:
             start = int(round(min(30.0, 0.1 * len(self.data['time']) / self.fs[0]) * self.fs[0]))
-            parts = self._ekf_blocks(algo, stats_start=start)
+            parts = self._ekf_blocks(algo, stats_start=start, bias_err=turn_on)
             end_err = torch.cat([r.end_err for r in parts])
             stats = engine.error_stats(end_err).cpu().numpy()
             err = end_err.cpu().numpy()
             con = torch.cat([r.consist for r in parts]).cpu().numpy()
             bias = torch.cat([r.end_bias for r in parts]).cpu().numpy()
-        self._mc[i].update({'end_err': err, 'consist': con, 'end_bias': bias})
+            if turn_on:
+                bias_err = torch.cat([r.end_bias_err for r in parts]).cpu().numpy()
+        self._mc[i].update({'end_err': err, 'consist': con, 'end_bias': bias, 'bias_err': bias_err})
         self.err_stats[name] = dist.combine_local_stats(stats, hi - lo)
         algo.run_times += self.sim_count
         for out in ('att_euler', 'pos', 'vel', 'wb', 'ab'):
@@ -1038,12 +1049,14 @@ class Sim(object):
         The filter's consistency record over this rank's runs (GPS epochs after the settling time,
         after the update): {'nees': [R,3] mean NEES of the position / velocity / attitude blocks
         (expected 3 each), 'inside3': [R,15] fraction of epochs with |error| <= 3 sigma per state
-        (p, v, phi, bg, ba), 'epochs': count, 'end_bias': [R,6] bias estimates at the last sample}.
+        (p, v, phi, bg, ba), 'epochs': count, 'end_bias': [R,6] bias estimates at the last sample,
+        'bias_err': [R,6] those estimates minus each run's true gyro then accel bias (the IMU's 'b', the run's
+        turn-on bias and the drift) when the IMU draws a turn-on bias ('b_std'), else None}.
         '''
         c = self._mc[algo_index]['consist']
         ep = np.maximum(c[:, 18:19], 1.0)
         return {'nees': c[:, 0:3] / ep, 'inside3': c[:, 3:18] / ep, 'epochs': int(c[0, 18]) if len(c) else 0,
-                'end_bias': self._mc[algo_index]['end_bias']}
+                'end_bias': self._mc[algo_index]['end_bias'], 'bias_err': self._mc[algo_index]['bias_err']}
 
     # ---- lazy histories -------------------------------------------------------
     def _history(self, name, run):

@@ -289,6 +289,35 @@ int b2ins_ins_loose_fed_align_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_a
                                   double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb,
                                   double* dump_ab, void* stream);
 
+/* Run-to-run turn-on bias (DESIGN.md sections 4 and 11): b2ins_ins_loose_align_f64 where every run also draws the
+ * turn-on bias of gyro_run / accel_run (each nullable = none), b_run[c] = b[c] z0 of b2ins_run_err's pair j = c
+ * (the draw b2ins_imu_noise_rx_f64 and b2ins_imu_run_err_f64 make for the same global run), added to the constant
+ * bias cfg->*_err.b of the measurements.  The filter's model takes it into P0: the bias states start at
+ * b_drift^2 + b^2 + b_std^2, the aligned level term at (b^2 + b_drift^2 + b_std^2 + vrw^2 fs / 10) / 9.80665^2 and
+ * the gyro's growth over the gap at arw^2 dt_gap + (b^2 + b_drift^2 + b_std^2) dt_gap^2; Q is unchanged.  The
+ * consistency record's true bias is b + b_run + the drift.  end_bias_err [runs][6] (nullable): the gyro then accel
+ * bias estimates minus the true biases at sample n-1.  sf and ma must be zero (the filter has no states for them),
+ * b finite and >= 0: B2INS_ERR_ARG before any CUDA call otherwise.  With no non-zero b and end_bias_err NULL this
+ * is b2ins_ins_loose_align_f64, bit for bit.  DEVICE pointers. */
+int b2ins_ins_loose_rx_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, const b2ins_vib* vib_gyro,
+                           const b2ins_vib* vib_accel, int64_t proc_start, int proc_pos_frame,
+                           const double* ref_gyro, const double* ref_accel, const double* ref_nav,
+                           const double* ref_gps, const int64_t* gps_idx, const double* gps_vis, double* end_err,
+                           double* end_bias, double* consist, double* proc_stats, double* dump_att,
+                           double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab,
+                           const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, double* end_bias_err,
+                           void* stream);
+
+/* b2ins_ins_loose_fed_f64 (align NULL or B2INS_ALIGN_OFF) or b2ins_ins_loose_fed_align_f64 (ini_draw must then be
+ * 0) whose model knows the turn-on bias of gyro_run / accel_run (each nullable): the supplied measurements carry
+ * each run's bias, and only b enters the filter, in P0 as in b2ins_ins_loose_rx_f64.  Checks as there.  DEVICE
+ * pointers. */
+int b2ins_ins_loose_fed_rx_f64(const b2ins_ekf_config* cfg, const b2ins_ekf_align* align, int ini_draw,
+                               const double* gyro, const double* accel, const double* gps, const int64_t* gps_idx,
+                               const double* gps_vis, const double* ref_nav, double* end_err, double* end_bias,
+                               double* dump_att, double* dump_pos, double* dump_vel, double* dump_wb, double* dump_ab,
+                               const b2ins_run_err* gyro_run, const b2ins_run_err* accel_run, void* stream);
+
 /* ---- housekeeping ------------------------------------------------------ */
 int b2ins_version(void);
 const char* b2ins_last_error(void);
