@@ -1834,8 +1834,8 @@ int b2ins_diag_psd_plan(int64_t n, int* P) {
 }
 
 // ---------------------------------------------------------------- K11 -------
-// [0, 16): the bin scale; then K5's chirp transform (Bluestein, P <= 8192 complex); then the chunk sums
-static int64_t welch_partial_offset(const WelchPlan& w) { return 16 + (w.bluestein ? int64_t(w.P) * 16 : 0); }
+// [0, 32): the bin scale, the power's and the window's prescales; then K5's chirp transform (Bluestein, P <= 8192 complex); then the chunk sums
+static int64_t welch_partial_offset(const WelchPlan& w) { return 32 + (w.bluestein ? int64_t(w.P) * 16 : 0); }
 
 int64_t b2ins_welch_workspace_bytes(int64_t n, int64_t nseries, int64_t nperseg, int64_t noverlap) {
   WelchPlan w;
@@ -1889,9 +1889,18 @@ int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x, int6
   p.window = window;
   unsigned char* ws = static_cast<unsigned char*>(workspace);
   p.wscale = reinterpret_cast<double*>(ws);
-  p.bhat = reinterpret_cast<const double2*>(ws + 16);
+  p.bhat = reinterpret_cast<const double2*>(ws + 32);
   p.part = reinterpret_cast<double*>(ws + welch_partial_offset(w));
-  p.post = w.bluestein ? 0.25 / (static_cast<double>(w.P) * w.P) : 0.25;
+  p.post = w.bluestein ? 0.5 / static_cast<double>(w.P) : 0.5;
+  int e = 0;
+  while ((int64_t(1) << e) < w.N) ++e;
+  p.mean_scale = std::ldexp(1.0, -e);
+  p.mean_div = std::ldexp(static_cast<double>(w.N), -e);
+  int qc = 0, qn = 0;
+  while ((int64_t(1) << qc) < w.Q) ++qc;
+  while (w.nchunk > 1 && (int64_t(1) << qn) < w.nchunk) ++qn;
+  p.chunk_scale = std::ldexp(1.0, -qc);
+  p.part_scale = std::ldexp(1.0, -qn);
   p.psd = psd;
   p.freq = freq;
   welch_prep_kernel<<<1, kWelchThreads, 0, s>>>(p);
@@ -1907,7 +1916,7 @@ int b2ins_welch_f64(double fs, int64_t n, int64_t nseries, const double* x, int6
     f.P = w.P;
     f.logP = w.logP;
     f.bluestein = 1;
-    f.bhat = reinterpret_cast<double2*>(ws + 16);
+    f.bhat = reinterpret_cast<double2*>(ws + 32);
     CU_CHECK(cudaFuncSetAttribute(psd_chirp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 24));
     psd_chirp_kernel<<<1, kFftThreads, fft_smem, s>>>(f);
     CU_CHECK(cudaGetLastError());

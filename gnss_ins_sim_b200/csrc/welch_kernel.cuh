@@ -18,6 +18,27 @@
 // K5's 192 KB of shared memory with one segment; the window is read through L1/L2.  Consecutive segments of a
 // chunk overlap, so their second read of a sample comes from L2.
 //
+// Mean.  The segment mean is removed as a pair hi + lo: hi is the sum of x 2^-e (2^e >= N) divided by N 2^-e,
+// lo the same of the residuals x - hi, and y = ((x - hi) - lo) w.  A one-pass mean carries a rounding of order
+// u |mean| into every sample, which leaks u |mean| sum w into bins 0 and 1: 5 % of bin 0 for an offset of 1e4
+// under noise of 1e-9.  The pair leaves u^2 |mean| plus the roundings of the residuals, and nothing for a
+// constant series (its residuals are exact and lo = (N d 2^-e) / (N 2^-e) = d).
+//
+// Range.  Every rescaling is a power of two, so the bits are those of the plain formula wherever nothing over-
+// or underflows:
+//   * the mean sums x 2^-e, and y is formed as ((x 2^-e - hi 2^-e) - lo 2^-e) (w 2^-c), 2^c >= 16 sqrt(sum w^2)
+//     (times P^3 more on the Bluestein path): no value of the transform can overflow, so finite samples never
+//     give NaN;
+//   * re and im are scaled by g = 2^(e+c-a-4) (1/2, or 1/(2P) on the Bluestein path) before squaring, with
+//     2^(2a) near fs sum w^2, so |g 2X|^2 is at most 2^-6 of the segment's own PSD;
+//   * each power is scaled by 2^-ceil(log2 Q) in a chunk and each chunk sum by 2^-ceil(log2 nchunk) in
+//     welch_finish_kernel;
+// welch_prep_kernel folds 2^(2a+8), the two chunk factors and 1/4 (1/(4P^2)) into wscale.  A bin is +inf
+// where the PSD exceeds DBL_MAX, and below that only where one segment's own PSD exceeds 16 DBL_MAX.  The
+// trade-off is at the small end: the scaled terms keep full precision down to a PSD of about
+// 2^(-1014 + ceil(log2 Q) + ceil(log2 nchunk)) (1e-300 for every N at up to 2^8 chunks, whatever fs); below
+// that they round as subnormals, where the unscaled |2X|^2, about fs sum w^2 times the PSD, kept more bits.
+//
 // Determinism.  The chunk length Q (segments) depends on N alone and G on N alone, so each series gives the
 // same bits whatever the batch, layout or position.  With more than one chunk, welch_finish_kernel adds the
 // chunk partials in chunk order.  A NaN or +-inf sample inside a used segment makes its mean non-finite and
@@ -68,8 +89,13 @@ struct WelchParams {
   double fs;
   const double* window;   // [N]
   const double2* bhat;    // [P] K5's transform of the conjugate chirp (Bluestein)
-  double* wscale;         // [1] c-free scale of a bin's sum: post / (K fs sum w^2), set by welch_prep_kernel
-  double post;            // 1/4 (|2X|^2), times 1/P^2 on the Bluestein path
+  double* wscale;         // [3] set by welch_prep_kernel: the c-free scale of a bin's sum
+                          // 2^(2a + 8 + qc + qn) / (K fs sum w^2), g = 2^(e+c-a-4) post, and 2^-c
+  double post;            // 1/2, times 1/P on the Bluestein path
+  double mean_scale;      // 2^-e, 2^e >= N: the mean's summands and y
+  double mean_div;        // N 2^-e
+  double chunk_scale;     // 2^-qc, 2^qc >= Q: each power within a chunk
+  double part_scale;      // 2^-qn, 2^qn >= nchunk (1 for one chunk): each chunk sum
   double* psd;            // [nseries][M + 1]
   double* part;           // [nseries][nchunk][M + 1] chunk sums (nchunk > 1)
   double* freq;           // [M + 1]
@@ -94,7 +120,20 @@ __global__ void __launch_bounds__(kWelchThreads) welch_prep_kernel(const __grid_
   double s = 0.0;
   for (int m = threadIdx.x; m < p.N; m += kWelchThreads) s = fma(p.window[m], p.window[m], s);
   s = welch_group_sum(s, kWelchThreads, red);
-  if (threadIdx.x == 0) *p.wscale = p.post / (static_cast<double>(p.K) * (p.fs * s));
+  if (threadIdx.x == 0) {
+    const double f = p.fs * s;
+    // 2^(2a) within a factor 4 of fs sum w^2, so |g 2X|^2 is near the bin's power times fs
+    int a = (f > 0.0 && isfinite(f)) ? ilogb(f) / 2 : 0;
+    a = a < -500 ? -500 : (a > 500 ? 500 : a);
+    // 2^-8 more: a segment's term overflows only where it is 64 times the largest finite PSD
+    const double back = ldexp(1.0, 2 * a + 8) / (p.chunk_scale * p.part_scale);
+    // 2^c >= 16 max |w| (max |w| <= sqrt(sum w^2)); P^3 bounds the Bluestein pipeline's growth over M
+    const int c = (s > 0.0 && isfinite(s) ? ilogb(s) / 2 : 0) + 5 + (p.bluestein ? 3 * p.logP : 0);
+    const int e = ilogb(1.0 / p.mean_scale);
+    p.wscale[0] = back / (static_cast<double>(p.K) * f);
+    p.wscale[1] = ldexp(p.post, e + c - a - 4);
+    p.wscale[2] = ldexp(1.0, -c);
+  }
   const double val = 1.0 / (static_cast<double>(p.N) * (1.0 / p.fs));
   for (int k = threadIdx.x; k <= p.M; k += kWelchThreads) p.freq[k] = static_cast<double>(k) * val;
 }
@@ -107,10 +146,11 @@ __device__ __forceinline__ double2 welch_z(const double2* z, int k, const WelchP
   return make_double2(r.x, -r.y);
 }
 
-// |2 X_k|^2 (times P^2 on the Bluestein path), k <= M; tw: e^{2 pi j i / M}, i < M / 2 (radix-2 path)
+// |g 2 X_k|^2 (g: wscale[1], 1/P of it undoing the Bluestein path's factor P), k <= M;
+// tw: e^{2 pi j i / M}, i < M / 2 (radix-2 path)
 template <bool BLUE>
 __device__ __forceinline__ double welch_bin_power(const double2* z, int k, const WelchParams& p,
-                                                  const double2* tw, double2 half_step) {
+                                                  const double2* tw, double2 half_step, double g) {
   const double2 zk = welch_z<BLUE>(z, k == p.M ? 0 : k, p);
   const double2 zc = welch_z<BLUE>(z, k == 0 ? 0 : p.M - k, p);
   const double2 a = make_double2(zk.x + zc.x, zk.y - zc.y);      // Z_k + conj Z_{M-k}
@@ -124,7 +164,7 @@ __device__ __forceinline__ double welch_bin_power(const double2* z, int k, const
     sincospi(-static_cast<double>(k) / static_cast<double>(p.M), &w.y, &w.x);
   }
   const double2 t = cmul(w, make_double2(d.y, -d.x));             // e^{-pi j k / M} (-j D_k)
-  const double re = a.x + t.x, im = a.y + t.y;
+  const double re = (a.x + t.x) * g, im = (a.y + t.y) * g;
   return fma(re, re, im * im);
 }
 
@@ -142,7 +182,7 @@ __global__ void __launch_bounds__(kWelchThreads, 1) welch_kernel(const __grid_co
   const int kb = tid / p.G, kstep = kWelchThreads / p.G;
   double2 half_step;                                      // e^{-pi j / M}
   sincospi(-1.0 / static_cast<double>(p.M), &half_step.y, &half_step.x);
-  const double inv_n = 1.0 / static_cast<double>(p.N);
+  const double g = p.wscale[1], wsc = p.wscale[2], ms = p.mean_scale;
   const int L = p.M + 1;
   const int64_t ss = p.sample_stride;
   for (int64_t item = blockIdx.x; item < p.nseries * p.nchunk; item += gridDim.x) {
@@ -162,14 +202,24 @@ __global__ void __launch_bounds__(kWelchThreads, 1) welch_kernel(const __grid_co
         for (int m = lr; m < p.M; m += gsz) {
           const double u = seg[(2 * static_cast<int64_t>(m)) * ss], v = seg[(2 * static_cast<int64_t>(m) + 1) * ss];
           xg[bitrev(m, p.logP)] = make_double2(u, v);
-          sum += u + v;
+          sum += u * ms + v * ms;
         }
       }
-      const double mean = welch_group_sum(sum, gsz, red) * inv_n;
+      const double hi = welch_group_sum(sum, gsz, red) / p.mean_div;
+      double res = 0.0;
+      if (live) {
+        for (int m = lr; m < p.M; m += gsz) {
+          const double2 v = xg[bitrev(m, p.logP)];
+          res += (v.x * ms - hi * ms) + (v.y * ms - hi * ms);
+        }
+      }
+      if (gsz > 32) __syncthreads();   // every warp has read red
+      const double lo = welch_group_sum(res, gsz, red) / p.mean_div;
       for (int m = lr; m < p.M; m += gsz) {
         const int i = bitrev(m, p.logP);
         const double2 v = live ? xg[i] : make_double2(0.0, 0.0);
-        const double2 y = make_double2((v.x - mean) * __ldg(p.window + 2 * m), (v.y - mean) * __ldg(p.window + 2 * m + 1));
+        const double2 y = make_double2(((v.x * ms - hi * ms) - lo * ms) * (__ldg(p.window + 2 * m) * wsc),
+                                       ((v.y * ms - hi * ms) - lo * ms) * (__ldg(p.window + 2 * m + 1) * wsc));
         xg[i] = BLUE ? cmul(make_double2(y.x, -y.y), chirp(m, p.M)) : y;
       }
       if (BLUE) {
@@ -188,7 +238,7 @@ __global__ void __launch_bounds__(kWelchThreads, 1) welch_kernel(const __grid_co
           // those of all ACC bins out of the round loop spills the accumulators
           int k = kb + r * kstep;
           asm volatile("" : "+r"(k));
-          if (k < L) acc[r] += welch_bin_power<BLUE>(z, k, p, tw, half_step);
+          if (k < L) acc[r] += welch_bin_power<BLUE>(z, k, p, tw, half_step, g) * p.chunk_scale;
         }
       }
     }
@@ -198,7 +248,7 @@ __global__ void __launch_bounds__(kWelchThreads, 1) welch_kernel(const __grid_co
       for (int r = 0; r < ACC; ++r) acc[r] += __shfl_xor_sync(0xffffffffu, acc[r], o);
     }
     if (slot == 0) {
-      const double scale = *p.wscale;
+      const double scale = p.wscale[0];
 #pragma unroll
       for (int r = 0; r < ACC; ++r) {
         const int k = kb + r * kstep;
@@ -220,9 +270,9 @@ __global__ void __launch_bounds__(256) welch_finish_kernel(const __grid_constant
   const int64_t s = i / L;
   const int k = static_cast<int>(i % L);
   const double* part = p.part + s * p.nchunk * L + k;
-  double acc = part[0];
-  for (int64_t c = 1; c < p.nchunk; ++c) acc += part[c * L];
-  p.psd[i] = ((k == 0 || k == p.M) ? acc : 2.0 * acc) * *p.wscale;
+  double acc = part[0] * p.part_scale;
+  for (int64_t c = 1; c < p.nchunk; ++c) acc += part[c * L] * p.part_scale;
+  p.psd[i] = ((k == 0 || k == p.M) ? acc : 2.0 * acc) * p.wscale[0];
 }
 
 }  // namespace b2ins
