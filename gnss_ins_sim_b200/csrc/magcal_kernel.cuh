@@ -5,12 +5,15 @@
 //   the plane-fit normals (M^T M) v = M^T 1 from the moments shifted back: the rows of O;
 //   pass 2  per segment, max and min of the two columns of c = O m whose ranges give the sensitivities;
 //   the sphere fit [2u, 1] p' = |u|^2 on u = S d, S = diag(s) O, as a linear transform of the pass-1 moments,
-//           then hard_iron = [p' + S t, sqrt(p'_3 + |p'|^2)].
+//           then hard_iron = [p' + S t, sqrt(p'_3 + |p'|^2)].  The 4x4 system is equilibrated by a power of two
+//           (u -> f u, f ~ 1 / rms |u|), so its pivot rule does not depend on the units of the samples and
+//           the result scales with them bit for bit wherever the moments neither overflow nor underflow.
 // The samples are K8's (generated form: mag_sample, regenerated in each pass) or read from memory (fed form).
 // Reductions are a fixed butterfly within each warp and the warps in order: a run's result depends only on
 // its samples, whatever the batch, run_offset or sharding.  A singular 3x3 or 4x4 system (a pivot at or below
-// kMagCalSingTol * max|A|, or a NaN) gives NaN in all 13 outputs of the run.  Spec: oracle/magcal_np.py
-// (calibrate_moments); DESIGN.md section 3.11.
+// kMagCalSingTol * max|A|, or a NaN), or any non-finite output (a non-finite sample, overflowing moments), gives
+// NaN in all 13 outputs of the run and in its mag_cal rows.  Spec: oracle/magcal_np.py (calibrate_moments);
+// exact reference and rounding bound: oracle/magcal_exact.py; DESIGN.md section 3.11.
 #pragma once
 #include "common.cuh"
 #include "mag_kernel.cuh"
@@ -271,22 +274,37 @@ __global__ void __launch_bounds__(kMagCalThreads) magcal_kernel(const __grid_con
       w[a] = acc;
     }
     for (int i = 0; i < 3; ++i) v[i] = (Sm[i][0] * w[0] + Sm[i][1] * w[1]) + Sm[i][2] * w[2];
+    // the fit on f u, f = 2^-e, e = floor((e_tr - e_N) / 2) from the binary exponents of trace(sum u u^T) and N,
+    // so f is within a factor 2 of 1 / rms |u|: every entry of HH is then on the scale of N, the pivot rule does
+    // not depend on the units of the samples, and every scaling is exact (no division or root on the way)
+    const double tr = (U2[0][0] + U2[1][1]) + U2[2][2];
+    int e = 0;
+    if (isfinite(tr) && tr > 0.0) {
+      int etr, en;
+      frexp(tr, &etr);
+      frexp(N, &en);
+      e = (etr - en) >> 1;
+    }
+    const double f = ldexp(1.0, -e), f2 = f * f, g = ldexp(1.0, e), g2 = g * g;   // g = 1 / f
     double HH[4][4], q[4];
     for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j) HH[i][j] = 4.0 * U2[i][j];
-      HH[i][3] = HH[3][i] = 2.0 * U1[i];
-      q[i] = 2.0 * v[i];
+      for (int j = 0; j < 3; ++j) HH[i][j] = (4.0 * U2[i][j]) * f2;
+      HH[i][3] = HH[3][i] = (2.0 * U1[i]) * f;
+      q[i] = (2.0 * v[i]) * (f2 * f);
     }
     HH[3][3] = N;
-    q[3] = (U2[0][0] + U2[1][1]) + U2[2][2];
-    const bool ok = magcal_solve<4>(HH, q) && !isnan(O[0]);
+    q[3] = tr * f2;
+    bool ok = magcal_solve<4>(HH, q) && !isnan(O[0]);
     double out[13];
     for (int i = 0; i < 3; ++i) {
       const double T = (Sm[i][0] * t[0] + Sm[i][1] * t[1]) + Sm[i][2] * t[2];
+      q[i] *= g;
       out[9 + i] = q[i] + T;
       for (int j = 0; j < 3; ++j) out[3 * i + j] = Sm[i][j];
     }
+    q[3] *= g2;
     out[12] = sqrt(q[3] + ((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]));
+    for (int i = 0; i < 13; ++i) ok = ok && isfinite(out[i]);
     if (!ok)
       for (int i = 0; i < 13; ++i) out[i] = __longlong_as_double(0x7ff8000000000000ll);
     for (int i = 0; i < 9; ++i) p.soft_iron[r * 9 + i] = out[i];

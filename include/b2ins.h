@@ -652,8 +652,9 @@ int b2ins_mag_noise_f64(int64_t runs, int64_t n, const double* ref_mag, const do
  * one CTA per run (DESIGN.md section 3.11).  seg: host [6] = (x0, xf, y0, yf, z0, zf), half-open sample
  * ranges of the rotations about the sensor's x, y and z axes, each >= 3 rows inside [0, n).
  * Outputs (device): soft_iron [runs][9] (row-major S) and hard_iron [runs][4] (hard iron, field radius);
- * calibrated samples are S m - hard_iron[0:3].  A singular 3x3 or 4x4 system gives NaN in all 13 values of
- * the run; a zero range gives what the division gives; a NaN sample gives NaN.  Deterministic: a run's
+ * calibrated samples are S m - hard_iron[0:3].  A singular 3x3 or 4x4 system, or any non-finite output (a
+ * NaN or +-inf sample, a zero range, moments past the range of double), gives NaN in all 13 values of the run
+ * and in its mag_cal rows.  The result scales with the samples' units bit for bit.  Deterministic: a run's
  * result is bit-identical whatever runs, run_offset or the other runs.
  * b2ins_magcal_f64: the samples of K8 (b2ins_mag_noise_f64 with the same ref_mag, si, hi, std, seed and
  *   run_offset), regenerated, never stored.  err [runs][13] (nullable): the calibration error against that

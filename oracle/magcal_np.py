@@ -11,7 +11,8 @@ z axes.  Both forms return (soft_iron [3, 3], hard_iron [4]) and give NaN in all
     sum d, sum d d^T and the ten cubic monomials of d = m - t (t = the first row of the x segment), the
     normals from the moments shifted back, the ranges from a second pass over the samples, and the sphere
     fit in the shifted calibrated frame u = S d, where the 4x4 system is well conditioned whatever the
-    hard iron.
+    hard iron, equilibrated by a power of two (sphere_scale) so that it is well scaled whatever the units.
+    Any non-finite output makes all 13 NaN.
 """
 import numpy as np
 
@@ -124,14 +125,45 @@ def calibrate_direct(mag, segments):
     return S, hi, c - hi[0:3]
 
 
-def moments(mag, seg, t):
-    """Per segment: count, sum d [3], sum d d^T [6] (QUAD), cubic sums [10] (CUBIC) of d = m - t."""
+THREADS = 256      # K10's CTA: thread j sums rows j, j + 256, ... of a segment, then 8 warps of 32 lanes
+
+
+def _kernel_sum(x):
+    """The column sums of x [L, K] in K10's order: per thread at stride THREADS, the xor butterfly within each
+    warp (lane l adds lane l ^ o, o = 16 .. 1), then the warps in order."""
+    L, K = x.shape
+    rounds = -(-L // THREADS)
+    xp = np.zeros((rounds * THREADS, K))
+    xp[:L] = x
+    xp = xp.reshape(rounds, THREADS, K)
+    acc = np.zeros((THREADS, K))
+    for i in range(rounds):
+        acc = acc + xp[i]
+    v = acc.reshape(THREADS // 32, 32, K)
+    lane = np.arange(32)
+    o = 16
+    while o:
+        v = v + v[:, lane ^ o]
+        o >>= 1
+    s = v[0, 0].copy()
+    for w in range(1, THREADS // 32):
+        s = s + v[w, 0]
+    return s
+
+
+def moments(mag, seg, t, order='numpy'):
+    """Per segment: count, sum d [3], sum d d^T [6] (QUAD), cubic sums [10] (CUBIC) of d = m - t; the sums in
+    NumPy's order, or in K10's (order='kernel', _kernel_sum)."""
     out = []
     for a, b in seg:
         d = mag[a:b] - t
         q = np.stack([d[:, i] * d[:, j] for i, j in QUAD], axis=1)
         cub = np.stack([q[:, QUAD.index((i, j))] * d[:, k] for i, j, k in CUBIC], axis=1)
-        out.append((b - a, d.sum(0), q.sum(0), cub.sum(0)))
+        if order == 'kernel':
+            s = _kernel_sum(np.concatenate([d, q, cub], axis=1))
+            out.append((b - a, s[0:3], s[3:9], s[9:19]))
+        else:
+            out.append((b - a, d.sum(0), q.sum(0), cub.sum(0)))
     return out
 
 
@@ -152,36 +184,52 @@ def cubic_tensor(cub):
     return T
 
 
-def calibrate_moments(mag, segments):
-    """K10's formulation (module docstring): soft_iron [3, 3], hard_iron [4]."""
+def sphere_scale(tr, N):
+    """(f, e): f = 2^-e, e = floor((e_tr - e_N) / 2) from the binary exponents (frexp) of tr = trace(sum u u^T)
+    and N, so f is within a factor 2 of 1 / rms |u|; e = 0 unless tr is finite and positive.  K10 fits the sphere
+    to f u, which puts every entry of its 4x4 system on the scale of N."""
+    if not (np.isfinite(tr) and tr > 0.0):
+        return 1.0, 0
+    e = (int(np.frexp(tr)[1]) - int(np.frexp(float(N))[1])) >> 1
+    return np.ldexp(1.0, -e), e
+
+
+def calibrate_moments(mag, segments, order='numpy'):
+    """K10's formulation (module docstring): soft_iron [3, 3], hard_iron [4].  order='kernel' sums the moments
+    in K10's order (_kernel_sum); the rest already follows K10's order of operations."""
     mag = np.asarray(mag, dtype=np.float64)
     seg = check_segments(segments, mag.shape[0])
     t = mag[seg[0, 0]].copy()
-    mom = moments(mag, seg, t)
-    normals = []
-    for N, s1, q, _ in mom:
-        A = sym3(q) + np.outer(t, s1) + np.outer(s1, t) + N * np.outer(t, t)
-        normals.append(_normal(solve(A, s1 + N * t)))
-    O = np.array(normals)
-    s = _sens(*(_ranges(mag[a:b].dot(O.T), k) for k, (a, b) in enumerate(seg)))
-    S = np.diag(s).dot(O)
-    N = sum(m[0] for m in mom)
-    D1 = sum(m[1] for m in mom)
-    D2 = sym3(sum(m[2] for m in mom))
-    D3 = cubic_tensor(sum(m[3] for m in mom))
-    U1 = S.dot(D1)
-    U2 = S.dot(D2).dot(S.T)
-    # sum u_i |u|^2 = (S w)_i with w_a = sum_bc (S^T S)_bc D3_abc
-    w = np.einsum('bc,abc->a', S.T.dot(S), D3)
-    HH = np.empty((4, 4))
-    HH[0:3, 0:3] = 4.0 * U2
-    HH[0:3, 3] = HH[3, 0:3] = 2.0 * U1
-    HH[3, 3] = N
-    HB = np.append(2.0 * S.dot(w), np.trace(U2))
-    q = solve(HH, HB)
-    T = S.dot(t)
-    hi = np.array([q[0] + T[0], q[1] + T[1], q[2] + T[2], np.sqrt(q[3] + q[0:3].dot(q[0:3]))])
-    if np.isnan(O).any() or np.isnan(q).any():
+    with np.errstate(all='ignore'):
+        mom = moments(mag, seg, t, order)
+        normals = []
+        for N, s1, q, _ in mom:
+            A = sym3(q) + np.outer(t, s1) + np.outer(s1, t) + N * np.outer(t, t)
+            normals.append(_normal(solve(A, s1 + N * t)))
+        O = np.array(normals)
+        s = _sens(*(_ranges(mag[a:b].dot(O.T), k) for k, (a, b) in enumerate(seg)))
+        S = np.diag(s).dot(O)
+        N = float(sum(m[0] for m in mom))
+        D = [(mom[0][i] + mom[1][i]) + mom[2][i] for i in (1, 2, 3)]
+        D1, D2, D3 = D[0], sym3(D[1]), cubic_tensor(D[2])
+        U1 = S.dot(D1)
+        U2 = S.dot(D2).dot(S.T)
+        # sum u_i |u|^2 = (S w)_i with w_a = sum_bc (S^T S)_bc D3_abc
+        w = np.einsum('bc,abc->a', S.T.dot(S), D3)
+        tr = (U2[0, 0] + U2[1, 1]) + U2[2, 2]
+        f, _ = sphere_scale(tr, N)
+        f2 = f * f
+        HH = np.empty((4, 4))
+        HH[0:3, 0:3] = (4.0 * U2) * f2
+        HH[0:3, 3] = HH[3, 0:3] = (2.0 * U1) * f
+        HH[3, 3] = N
+        HB = np.append((2.0 * S.dot(w)) * (f2 * f), tr * f2)
+        q = solve(HH, HB)
+        q[0:3] /= f
+        q[3] /= f2
+        T = S.dot(t)
+        hi = np.array([q[0] + T[0], q[1] + T[1], q[2] + T[2], np.sqrt(q[3] + q[0:3].dot(q[0:3]))])
+    if np.isnan(O).any() or np.isnan(q).any() or not (np.isfinite(S).all() and np.isfinite(hi).all()):
         return _nan_result(seg)
     return S, hi
 
